@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- frames/sec of the PocketSphinx hot path (senone evaluation + Viterbi) on B200.
+"""bench.py -- frames/sec of the PocketSphinx hot path (senone evaluation + Viterbi) on an H100.
 
 One "step" = one pass of the hot path over one batch of synthetic utterances: GMM senone
 evaluation of every frame (all senones, like `-compallsen yes`), the phone-loop Viterbi
@@ -29,7 +29,7 @@ import numpy as np
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
-from pocketsphinx_b200.model import PackedModel, synth_feats, synth_ms, synth_ptm, synth_semi  # noqa: E402
+from pocketsphinx_b200.model import PackedModel, load_npz, synth_feats, synth_ms, synth_ptm, synth_semi  # noqa: E402
 
 FRAMES_PER_SEC_AUDIO = 100          # 10 ms frames
 PL = dict(window=5, beam=-225, pbeam=-225, pip=0, weight=3.0)   # pl_beam 1e-10 etc. >> 10
@@ -118,36 +118,72 @@ def reference_model_dir(name, pm, raw):
     return _REF_DIR
 
 
-def ncu_traffic(kernel, workload):
-    """DRAM bytes per launch of `kernel` at `workload` from a committed ncu capture, or None."""
-    p = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    try:
-        with open(p) as f:
-            return json.load(f).get(kernel + "|" + workload)
-    except (OSError, ValueError):
-        return None
-
-
-def tensor_peak_bf16():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    try:
-        with open(p) as f:
-            return float(json.load(f)["bf16_tflops"])
-    except (OSError, ValueError, KeyError):
-        return 2250.0                                          # nominal dense bf16 (B200_PROFILING.md)
+# H100 SXM data sheet (700 W): HBM3 GB/s and dense TF32 TFLOP/s, the roofline peaks when no measured ones are on file
+H100_HBM_GBS = 3350.0
+H100_TF32_TFLOPS = 495.0
 
 
 def peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        with open(p) as f:
+    """(HBM GB/s, dense TF32 TFLOP/s, max SM MHz or None, source): MEASURED_PEAKS.json (peaks measured on the machine,
+    TF32 at half the measured dense bf16 rate) when it is present, else the H100 SXM data sheet."""
+    try:
+        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             d = json.load(f)
-        return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)", float(d.get("sm_max_mhz", 1965.0))
-    return 6650.0, "fallback (B200_PROFILING.md)", 1965.0
+        return float(d["hbm_gbs"]), float(d["bf16_tflops"]) / 2.0, d.get("sm_max_mhz"), "measured (MEASURED_PEAKS.json)"
+    except (OSError, ValueError, KeyError):
+        return H100_HBM_GBS, H100_TF32_TFLOPS, None, "H100 SXM data sheet (700 W)"
+
+
+def gpu_info(index):
+    """Name, power limit, max SM clock of the card (nvidia-smi), or None."""
+    try:
+        r = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=name,power.limit,clocks.max.sm",
+                            "--format=csv,noheader,nounits"], capture_output=True, text=True, timeout=30)
+        name, power, mhz = [c.strip() for c in r.stdout.strip().splitlines()[0].split(",")]
+        return {"name": name, "power_limit_w": float(power), "sm_max_mhz": float(mhz)}
+    except (OSError, ValueError, IndexError, subprocess.SubprocessError):
+        return None
+
+
+class _DeviceArray:
+    """A library device buffer for torch.as_tensor (CUDA array interface, no copy)."""
+
+    def __init__(self, ptr, shape, typestr):
+        self.__cuda_array_interface__ = {"data": (int(ptr), False), "shape": tuple(shape), "typestr": typestr, "version": 2}
+
+
+def dump_outputs(dirname, torch, dev, d_best, d_pen, d_senscr, total, H, n_sen, swbest, n_rows=1024, n_max=1 << 20):
+    """The timed step's results as DIR/<name>.npy: phone-loop best score per frame, the sweep's best path score per
+    frame and utterance, and for a seeded sample of frames their senone-score and penalty rows.  Integers are stored
+    exactly (int16 as float32, int32 as float64); arrays over n_max elements are sampled, so the files stay < 64 MB."""
+    os.makedirs(dirname, exist_ok=True)
+    rng = np.random.default_rng(2024)
+    rows = np.sort(rng.choice(total, min(total, n_rows), replace=False))
+    idx = torch.from_numpy(rows).to(dev)
+
+    def view(ptr, shape, typestr):
+        return torch.as_tensor(_DeviceArray(ptr, shape, typestr), device=dev)
+
+    def bounded(t):
+        t = t.reshape(-1)
+        if t.numel() <= n_max:
+            return t.cpu().numpy()
+        keep = np.sort(np.random.default_rng(2025).choice(t.numel(), n_max, replace=False))
+        return t[torch.from_numpy(keep).to(t.device)].cpu().numpy()
+
+    out = {"sample_frames": rows.astype(np.float64),
+           "phoneloop_best": bounded(view(d_best, (total,), "<i4")).astype(np.float64),
+           "phoneloop_pen_rows": view(d_pen, (total, H), "<i4")[idx].cpu().numpy().astype(np.float64),
+           "senscr_rows": view(d_senscr, (total, n_sen), "<i2")[idx].cpu().numpy().astype(np.float32)}
+    if swbest is not None:
+        out["sweep_best"] = bounded(swbest).astype(np.float64)
+    for name, a in out.items():
+        np.save(os.path.join(dirname, name + ".npy"), a)
+    return sorted(out)
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index):
         self.rows = []
@@ -316,8 +352,8 @@ def search_stage(api, torch, U=256):
     first utterance's tables compared against the reference's golden ones."""
     here = os.path.dirname(os.path.abspath(__file__))
     gd = os.path.join(here, "tests", "golden")
-    m = np.load(os.path.join(gd, "en_us_ptm_model.npz"))
-    gf = np.load(os.path.join(gd, "en_us_goforward.npz"))
+    m = load_npz(os.path.join(gd, "en_us_ptm_model.npz"))
+    gf = load_npz(os.path.join(gd, "en_us_goforward.npz"))
     scr = gf["senscr"]
     T = len(scr)
     d_scr = torch.from_numpy(np.ascontiguousarray(np.tile(scr, (U, 1)))).cuda()
@@ -333,12 +369,12 @@ def search_stage(api, torch, U=256):
         t0 = time.perf_counter()
         r = fn()
         return r, time.perf_counter() - t0
-    c = case(np.load(os.path.join(gd, "en_us_fsg.npz")), "cmd")
+    c = case(load_npz(os.path.join(gd, "en_us_fsg.npz")), "cmd")
     (hist, n), dt = timed(lambda: ctx.fsg(d_scr.data_ptr(), off, c, len(c["hist"]) + 64))
     out["fsg"] = {"kernel": "fsg_search_kernel", "pnodes": int(len(c["pnodes"])), "ms": dt * 1e3, "utts_per_s": U / dt,
                   "frames_per_s": U * T / dt, "matches_reference": bool(np.array_equal(hist[0], c["hist"]) and (n == n[0]).all())}
-    c = case(np.load(os.path.join(gd, "en_us_fwdtree.npz")), "flat_default")
-    first_ref = case(np.load(os.path.join(gd, "en_us_fwdtree.npz")), "lookahead")
+    c = case(load_npz(os.path.join(gd, "en_us_fwdtree.npz")), "flat_default")
+    first_ref = case(load_npz(os.path.join(gd, "en_us_fwdtree.npz")), "lookahead")
     nci = int(c["info"][6])
     cit, cis = m["phone_tmat"][:nci], m["phone_ssid"][:nci]
     win = int(gf["pl_params"][4])
@@ -356,7 +392,7 @@ def search_stage(api, torch, U=256):
     out["two_pass"] = {"call": "psb_ngram_two_pass_batch_device", "ms": dt3 * 1e3, "utts_per_s": U / dt3, "frames_per_s": U * T / dt3,
                        "matches_reference": bool(np.array_equal(both[0][0], c["bp"]) and np.array_equal(both[U - 1][0], c["bp"]))}
     try:                                               # the words, read from the tables alone (psb_result.cu)
-        dflt = case(np.load(os.path.join(gd, "en_us_fwdtree.npz")), "default")
+        dflt = case(load_npz(os.path.join(gd, "en_us_fwdtree.npz")), "default")
         vocab, words = str(dflt["vocab"]).split("\n"), dflt["words"]
         t0 = time.perf_counter()
         hyps = []
@@ -392,7 +428,7 @@ def search_coupled_stage(api, torch, batch, pm, off, U, T, kind, gmm_ms_per_fram
     Reported beside the headline: frames/s of the search call alone (tables downloaded) and of GMM + search in sequence."""
     here = os.path.dirname(os.path.abspath(__file__))
     gd = os.path.join(here, "tests", "golden")
-    m = np.load(os.path.join(gd, "en_us_ptm_model.npz"))
+    m = load_npz(os.path.join(gd, "en_us_ptm_model.npz"))
     if pm.n_sen < int(m["n_sen"]):
         return {"error": "model has fewer senones than the search description uses"}
     Us = min(U, 256 if kind == "fsg" else 64)          # the first pass's tables: 128 entries per frame allowed on random scores
@@ -404,10 +440,10 @@ def search_coupled_stage(api, torch, batch, pm, off, U, T, kind, gmm_ms_per_fram
     out = {"search": kind, "utts": Us, "frames_per_utt": T}
     try:
         if kind == "fsg":
-            c = case(np.load(os.path.join(gd, "en_us_fsg.npz")), "cmd")
+            c = case(load_npz(os.path.join(gd, "en_us_fsg.npz")), "cmd")
             fn = lambda: ctx.fsg(batch.senscr_device_ptr(), offs, c, 64 * T)
         else:
-            c = case(np.load(os.path.join(gd, "en_us_fwdtree.npz")), "default")
+            c = case(load_npz(os.path.join(gd, "en_us_fwdtree.npz")), "default")
             nci = int(c["info"][6])
             fn = lambda: ctx.ngram_fwdtree(batch.senscr_device_ptr(), offs, c["info"], c["model"], m["phone_tmat"][:nci], 128 * T, 128 * T * 32)
         fn()
@@ -541,7 +577,11 @@ def main():
     ap.add_argument("--cpu-budget", type=float, default=15.0)
     ap.add_argument("--search", default="none", choices=["none", "fwdtree", "fsg"],
                     help="also couple a search kernel to the GMM stage's scores (BASELINE configs 3 / 4), reported as `search_coupled`")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed to DIR/<name>.npy (rank 0)")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
 
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -631,12 +671,16 @@ def main():
     batch.event_record(0)
     kern = {"transpose": 0.0, "topn": 0.0, "senone": 0.0}
     for _ in range(args.steps):
-        batch.decode_device(pl, d_feats.data_ptr(), off)
+        d_best, d_pen = batch.decode_device(pl, d_feats.data_ptr(), off)
         sweep()
     batch.event_record(1)
     ms_total = batch.event_elapsed_ms()
     barrier()
     launches = api.lib().psb_kernel_launch_count() - launches1
+    dumped = None
+    if args.dump_outputs and rank == 0:
+        dumped = dump_outputs(args.dump_outputs, torch, torch.device("cuda", local), d_best, d_pen, batch.senscr_device_ptr(), total,
+                              H, pm.n_sen, d_swbest if hs is not None else None)
     # per-kernel durations for the roofline: two extra steps forced onto ONE stream (with
     # PSB_PIPELINE > 1 the timed region's kernels overlap and cannot be timed individually)
     batch.set_pipeline(1)
@@ -693,7 +737,9 @@ def main():
     ms_step, e2e_ms, e2e_scr_ms = pdist.reduce_max_ms([ms_step, e2e_ms, e2e_scr_ms], device="cuda")
 
     if rank == 0:
-        hbm_peak, peak_src, sm_max = peaks()
+        gpu = gpu_info(local)
+        hbm_peak, tf32_peak, sm_max, peak_src = peaks()
+        sm_max = sm_max or (gpu or {}).get("sm_max_mhz")
         frames_all = U_all * T
         value = frames_all / (ms_step * 1e-3)
         # roofline of the dominant kernel (the top-N kernel), algorithmic bytes per launch:
@@ -708,8 +754,8 @@ def main():
         gmm_ms = km["transpose"] + km["topn"] + km["senone"]
         flop = 4.0 * pm.n_mgau * pm.n_density * pm.sumlen * total      # sub, mul, mul, sub per (codeword, dim)
         sm_mhz = (clocks or {}).get("sm_mhz") or sm_max
-        fp32_peak = 148 * 128 * sm_mhz * 1e6 / 1e12                     # non-FMA FP32 lane-ops/s (TFLOP/s)
-        tf32_peak = tensor_peak_bf16() / 2.0
+        n_sm = torch.cuda.get_device_properties(local).multi_processor_count
+        fp32_peak = n_sm * 128 * sm_mhz * 1e6 / 1e12 if sm_mhz else None   # non-FMA FP32 lane-ops/s (TFLOP/s)
         variant = int(os.environ.get("PSB_TOPN_VARIANT", "6"))
         tc_path = variant >= 6 and pm.kind == "ptm" and all(int(x) == 13 for x in pm.featlen) and pm.n_density in (64, 128, 256) \
             and int(getattr(pm, "ds_ratio", 1)) == 1
@@ -717,11 +763,11 @@ def main():
             pm.kind, {0: "ptm_topn_kernel", 1: "ptm_topn2_kernel", 2: "ptm_topn2_kernel", 3: "ptm_topn_u2_kernel",
                       4: "ptm_topnq_kernel<NU=2>", 5: "ptm_topnq_kernel<NU=1>"}.get(variant, "ptm_topnq_kernel<NU=1>"))
         if tc_path:
-            topn_name = "ptm_tc5_kernel" if os.environ.get("PSB_TC_IMPL") != "mma" else "ptm_tc_kernel"
+            topn_name = "ptm_wgmma_kernel" if os.environ.get("PSB_TC_IMPL") != "mma" else "ptm_tc_kernel"
         out = {
             "metric": "frames/sec senone-eval+Viterbi", "value": value, "unit": "frames/s",
             "xRT": FRAMES_PER_SEC_AUDIO / value,
-            "n_gpus": world, "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms_step,
+            "n_gpus": world, "gpu": gpu, "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms_step,
             "higher_is_better": True, "scaling": "strong" if strong else "weak", "vs_baseline": None,
             "dtype": "f32->i16/i32", "data": "synthetic",
             "config": {"workload": workload_name(args, pm), "model": desc,
@@ -739,16 +785,13 @@ def main():
             "kernel_ms_unpipelined": {**km, "note": "separate single-stream pass after the timed region"},
             "roofline": {"bound": "hbm", "kernel": topn_name, "achieved": topn_gbs, "peak": hbm_peak,
                          "unit": "GB/s", "frac": topn_gbs / hbm_peak,
-                         # dram__bytes_read.sum + dram__bytes_write.sum of this kernel at this shape from an `ncu --set full`
-                         # capture, when one is on file (profiles/ncu_traffic.json, written by profiles/ncu_traffic.py); else null
-                         "traffic": ncu_traffic(topn_name, workload_name(args, pm)),
                          "peak_source": peak_src,
                          "algorithmic_bytes_per_launch": topn_bytes,
                          "note": "compute-bound by construction (SURVEY 8d): model is SMEM/L2 resident"},
             "roofline_fp32": {"bound": "fp32 non-FMA issue", "kernel": topn_name,
                               "achieved": flop / (km["topn"] * 1e-3) / 1e12, "peak": fp32_peak, "unit": "TFLOP/s",
-                              "frac": flop / (km["topn"] * 1e-3) / 1e12 / fp32_peak,
-                              "peak_source": "148 SMs x 128 lanes x sampled SM clock"},
+                              "frac": flop / (km["topn"] * 1e-3) / 1e12 / fp32_peak if fp32_peak else None,
+                              "peak_source": "%d SMs x 128 lanes x sampled SM clock" % n_sm},
             # the tensor-core filter of the top-N stage: 3 x TF32 GEMM [frames x 32] x [32 x n_density] per (codebook, stream) pair;
             # `achieved` counts those GEMM flops over the whole top-N stage (filter + exact rows + tie fix-up).  The stage's
             # algorithmic FP32 work (roofline_fp32) is what the scan kernels execute and this path mostly skips, so its
@@ -756,7 +799,7 @@ def main():
             "roofline_tensor": ({"bound": "tensor", "kernel": topn_name, "achieved": 3 * 2.0 * 32 * pm.n_density * K * total / (km["topn"] * 1e-3) / 1e12,
                                  "peak": tf32_peak, "unit": "TFLOP/s",
                                  "frac": 3 * 2.0 * 32 * pm.n_density * K * total / (km["topn"] * 1e-3) / 1e12 / tf32_peak,
-                                 "peak_source": "half the measured dense bf16 rate of MEASURED_PEAKS.json (TF32 runs at half the bf16 rate)"}
+                                 "peak_source": peak_src + ", dense TF32"}
                                 if tc_path else None),
             "gmm_stage": {"ms": gmm_ms, "algorithmic_bytes": stage_bytes,
                           "achieved_gbs": stage_bytes / (gmm_ms * 1e-3) / 1e9},
@@ -773,6 +816,8 @@ def main():
                                 "call": "psb_decode_batch_host with senscr != NULL (no search-scale Viterbi: the scores leave the device)"},
             "clocks": clocks,
         }
+        if dumped:
+            out["dumped_outputs"] = {"dir": args.dump_outputs, "arrays": dumped}
         if hs is not None:
             # registers hold the state, so the kernel's algorithmic traffic is the score rows (read once per CTA of a
             # segment; L2 serves the repeats) plus the state once: its bound is integer issue, not HBM

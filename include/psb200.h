@@ -1,4 +1,4 @@
-/* psb200.h -- C ABI of the B200-native PocketSphinx hot path (libpsb200.so).
+/* psb200.h -- C ABI of the H100-native PocketSphinx hot path (libpsb200.so).
  *
  * Plain C, no CUDA or torch types in any signature: a host program (the reference's own C,
  * or anything with an FFI) binds these exactly like the symbols they stand in for.  Every

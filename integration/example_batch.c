@@ -1,7 +1,7 @@
 /* integration/example_batch.c -- a plain-C host program against include/psb200.h: what a batch
  * front end (e.g. programs/pocketsphinx_batch.c of the reference) does with the library.  It is
  * compiled (C11, -Wall -Wextra -pedantic) by tests/test_abi.py to keep the header valid C; run it
- * on a machine with a B200:
+ * on a machine with an H100:
  *     gcc -std=c11 -Iinclude integration/example_batch.c -Lpocketsphinx_b200 -lpsb200 -o example
  * The model arrays come from the host's own loaders (here: a caller-supplied descriptor). */
 #include <stdio.h>

@@ -16,10 +16,46 @@ ROOT = os.path.dirname(HERE)
 sys.path.insert(0, ROOT)
 
 from oracle import refdrv  # noqa: E402
-from pocketsphinx_b200.model import PackedModel  # noqa: E402
+from pocketsphinx_b200.model import PackedModel, load_npz  # noqa: E402
 
 REF = os.environ.get("PS_REFERENCE", "/root/reference")
 OUT = os.path.join(ROOT, "tests", "golden")
+
+
+def save_golden(path, limit=950_000, **arrays):
+    """np.savez with LZMA members, split into parts (path, name.part1.npz, ...) that each stay under `limit` bytes: an
+    array too large for one part is cut along axis 0 (pocketsphinx_b200.model.load_npz concatenates the pieces)."""
+    import glob
+    import io
+    import lzma
+    import zipfile
+
+    def npy(a):
+        b = io.BytesIO()
+        np.lib.format.write_array(b, np.asanyarray(a), allow_pickle=False)
+        return b.getvalue()
+    pieces = []
+    for k, a in arrays.items():
+        a = np.asanyarray(a)
+        n = 1
+        while n < max(1, len(a) if a.ndim else 1) and len(lzma.compress(npy(a[:(len(a) + n - 1) // n]))) > limit * 0.9:
+            n *= 2
+        step = (len(a) + n - 1) // n if a.ndim else 1
+        for i in range(n if a.ndim else 1):
+            b = npy(a[i * step:(i + 1) * step] if a.ndim else a)
+            pieces.append((k, b, len(lzma.compress(b))))
+    stem = path[:-len(".npz")]
+    for old in glob.glob(glob.escape(stem) + ".part*.npz"):
+        os.remove(old)
+    files, size = [[]], 0
+    for pc in pieces:
+        if files[-1] and size + pc[2] > limit:
+            files.append([]); size = 0
+        files[-1].append(pc); size += pc[2]
+    for i, fl in enumerate(files):
+        with zipfile.ZipFile(path if i == 0 else "%s.part%d.npz" % (stem, i), "w", zipfile.ZIP_LZMA) as z:
+            for k, b, _ in fl:
+                z.writestr(k + ".npy", b)
 
 
 def save_model(name, pm_dict, keep_phones=None):
@@ -28,7 +64,7 @@ def save_model(name, pm_dict, keep_phones=None):
         pm.phone_ssid = pm.phone_ssid[:keep_phones]
         pm.phone_tmat = pm.phone_tmat[:keep_phones]
     path = os.path.join(OUT, name)
-    pm.save(path)
+    save_golden(path, **pm.to_npz_dict())
     print(name, os.path.getsize(path) // 1024, "KiB")
     return pm
 
@@ -45,7 +81,7 @@ def make_align():
         for k in ("ssid", "tmatid", "start", "dur", "score"):
             out[tag + "_" + k] = a[k]
         print("align", tag, len(a["ssid"]), "phones", a["dur"].sum(), "frames covered")
-    np.savez_compressed(os.path.join(OUT, "en_us_align.npz"), **out)
+    save_golden(os.path.join(OUT, "en_us_align.npz"), **out)
 
 
 def make_kws():
@@ -65,7 +101,7 @@ def make_kws():
         out[tag + "_beam"], out[tag + "_plp"] = np.int32(a["beam"]), np.int32(a["plp"])
         print("kws", tag, len(a["kp_off"]) - 1, "keyphrases", len(a["det"]), "detections")
     os.unlink(f.name)
-    np.savez_compressed(os.path.join(OUT, "en_us_kws.npz"), **out)
+    save_golden(os.path.join(OUT, "en_us_kws.npz"), **out)
 
 
 def make_allphone():
@@ -88,7 +124,7 @@ def make_allphone():
     for k in ("beam", "pbeam"):
         assert int(b[k]) == int(a[k])
     print("allphone + phone LM", len(b["segs"]), "segments")
-    np.savez_compressed(os.path.join(OUT, "en_us_allphone.npz"), **out)
+    save_golden(os.path.join(OUT, "en_us_allphone.npz"), **out)
 
 
 def make_fsg():
@@ -109,7 +145,7 @@ def make_fsg():
         for k, v in r.items():
             out[tag + "." + k] = np.array("\n".join(v)) if k == "vocab" else np.array(v)
         print("fsg", tag, len(r["pnodes"]), "pnodes", len(r["links"]), "links", len(r["hist"]), "history entries:", r["hyp"], r["score"])
-    np.savez_compressed(os.path.join(OUT, "en_us_fsg.npz"), **out)
+    save_golden(os.path.join(OUT, "en_us_fsg.npz"), **out)
 
 
 def make_fwdtree():
@@ -162,7 +198,27 @@ def make_fwdtree():
     r = refdrv.fwdtree(hd, os.path.join(REF, "test/data/turtle.lm.bin"), os.path.join(REF, "test/data/turtle.dic"), pcm,
                        dense_lm=False, fwdflat="yes")
     out["nodense.info"], out["nodense.model"] = r["info"], r["model"]          # same search, exported without the dense table
-    np.savez_compressed(os.path.join(OUT, "en_us_fwdtree.npz"), **out)
+    save_golden(os.path.join(OUT, "en_us_fwdtree.npz"), **out)
+
+
+def make_fe():
+    """tests/golden/fe_reference.npz: the reference front end's tables and outputs for oracle/fe_golden.cases()."""
+    from oracle import fe_golden
+    go = np.fromfile(os.path.join(REF, "test", "data", "goforward.raw"), np.int16)
+    out = {"goforward": go[:23000]}
+    hd = os.path.join(os.path.dirname(refdrv.LIB_PATH), "model", "en-us")
+    for kv, mf_in, ft_in in fe_golden.cases(go):
+        name = fe_golden.config_name(kv)
+        ref = refdrv.RefModel(hd, **kv)
+        for k, v in ref.fe_desc().items():
+            out["desc.%s.%s" % (name, k)] = np.asarray(v)
+        for pcm in mf_in:
+            out["mfcc.%s.%s" % (name, fe_golden.pcm_key(pcm))] = ref.mfcc(pcm)
+        for pcm in ft_in:
+            if len(pcm):
+                out["feat.%s.%s" % (name, fe_golden.pcm_key(pcm))] = ref.featurize_fresh(pcm)
+        ref.close()
+    save_golden(fe_golden.GOLDEN, **out)
 
 
 def make_fixed_point():
@@ -185,16 +241,18 @@ def make_fixed_point():
         dm = mean - (pm.mean.astype(np.float32) * np.float32(4096)).astype(np.int32)
         dv = var - pm.var.astype(np.int32)
         assert np.array_equal(det, pm.det.astype(np.int32)) and np.abs(dm).max() <= 1 and dv.min() >= 0 and dv.max() <= 1
-        ds = scr.astype(np.int32) - np.load(os.path.join(OUT, gg))["senscr"]
+        ds = scr.astype(np.int32) - load_npz(os.path.join(OUT, gg))["senscr"]
         assert np.abs(ds).max() < 32768
         path = os.path.join(OUT, "fx_%s.npz" % name)
-        np.savez_compressed(path, feats=feats, dmean=dm.astype(np.int8), dvar=dv.astype(np.int8), dsenscr=ds.astype(np.int16),
+        save_golden(path, feats=feats, dmean=dm.astype(np.int8), dvar=dv.astype(np.int8), dsenscr=ds.astype(np.int16),
                             topn=topn.astype(np.int32))
         print(path, os.path.getsize(path) // 1024, "KiB;", "%.0f %% of the scores differ from the float build's" % (100 * (ds != 0).mean()))
 
 
 def main():
     os.makedirs(OUT, exist_ok=True)
+    if len(sys.argv) > 1 and sys.argv[1] == "fe":
+        return make_fe()
     if len(sys.argv) > 1 and sys.argv[1] == "fx":
         return make_fixed_point()
     if len(sys.argv) > 1 and sys.argv[1] == "fwdtree":
@@ -217,7 +275,7 @@ def main():
     scr, topn = m.score(feats, want_topn=True)
     assert (scr == pl["senscr"]).all()
     par = pl["params"]
-    np.savez_compressed(
+    save_golden(
         os.path.join(OUT, "en_us_goforward.npz"), feats=feats, senscr=scr,
         topn_last=topn[-1], topn_first=topn[0],
         pl_hmm=pl["hmm"].view(np.uint8).reshape(pl["hmm"].shape + (88,)), pl_best=pl["best"], pl_pen=pl["pen"],
@@ -232,7 +290,7 @@ def main():
     flags[6, :] = 0
     flags[6, 4000] = 1
     ascr, nact, lists = m.score_active(feats[:T], flags)
-    np.savez_compressed(os.path.join(OUT, "en_us_active.npz"), flags=np.packbits(flags, axis=1),
+    save_golden(os.path.join(OUT, "en_us_active.npz"), flags=np.packbits(flags, axis=1),
                         n_sen=m.n_sen, senscr=ascr, nact=nact)
     m.close()
 
@@ -242,7 +300,7 @@ def main():
     save_model("tidigits_sc_model.npz", m.packed())
     f = m.featurize(pcm)
     s, tn = m.score(f, want_topn=True)
-    np.savez_compressed(os.path.join(OUT, "tidigits_goforward.npz"), feats=f, senscr=s, topn=tn)
+    save_golden(os.path.join(OUT, "tidigits_goforward.npz"), feats=f, senscr=s, topn=tn)
     m.close()
 
     # ---- an4 continuous (ms back-end, 1 Gaussian per senone) ----
@@ -251,7 +309,7 @@ def main():
     save_model("an4_cont_model.npz", m.packed())
     f = m.featurize(pcm)
     s = m.score(f)
-    np.savez_compressed(os.path.join(OUT, "an4_goforward.npz"), feats=f, senscr=s)
+    save_golden(os.path.join(OUT, "an4_goforward.npz"), feats=f, senscr=s)
     m.close()
 
     # ---- en-us through the ms back-end too (-senmgau .ptm. forces ms_mgau_init first) ----
@@ -301,7 +359,7 @@ def main():
         cases["n%d_after" % n_emit] = hm.view(np.uint8).reshape(n, 88)
         cases["n%d_best" % n_emit] = np.int32(best)
         ctx.close()
-    np.savez_compressed(os.path.join(OUT, "hmm_vit_eval.npz"), **cases)
+    save_golden(os.path.join(OUT, "hmm_vit_eval.npz"), **cases)
     make_align()
     make_kws()
     make_allphone()

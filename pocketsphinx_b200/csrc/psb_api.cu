@@ -340,7 +340,7 @@ extern "C" int psb_batch_create(psb_model_t *m, int32_t max_utts, int64_t max_fr
     b->max_frames = max_frames;
     {
         // tuning knob; default = tensor-core filter + exact rescoring (psb_ptm_tc.cu) where the model allows it,
-        // else packed FP32 with deferred insertion (ptm_topnq_kernel, variant 5)
+        // else codeword pairs with deferred insertion (ptm_topnq_kernel, variant 5)
         const char *v = getenv("PSB_TOPN_VARIANT");
         b->topn_variant = v ? atoi(v) : 6;
         const char *p = getenv("PSB_PIPELINE");         // sub-batches in flight for psb_decode_batch_*
@@ -559,8 +559,8 @@ static int decode_common_body(psb_batch_t *b, psb_phoneloop_t *p, const float *f
         PSB_CUDA(cudaMalloc(&b->d_pen, b->pen_cap * 4));
     }
     // auto: two ranges when the features come from the host (the copies of one overlap the
-    // kernels of the other), one when they are resident (measured on B200 at 1000 x 10 s: two
-    // concurrent top-N kernels only add launch/tail overhead, 110 ms vs 105 ms per step)
+    // kernels of the other), one when they are resident (two concurrent top-N kernels only add
+    // launch and tail overhead; PSB_PIPELINE overrides)
     const int want = b->n_pipe > 0 ? b->n_pipe : (feats_on_host ? 2 : 1);
     const int S = std::max(1, std::min<int>(want, n_utt));
     PSB_CUDA(cudaEventRecord(b->fork_ev, b->stream));

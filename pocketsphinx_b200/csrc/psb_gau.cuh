@@ -37,16 +37,13 @@ __device__ __forceinline__ float gau_dist(const float4 *__restrict__ r, const fl
 }
 
 // ---------------------------------------------------------------------------------------
-// Packed-FP32 variant (Blackwell FADD2/FMUL2, PTX add/mul.rn.f32x2): two *codewords* per
+// Pair variant (psb_fadd2_rn/psb_fmul2_rn: two scalar .rn operations each on sm_90): two *codewords* per
 // instruction.  Records are stored pair-interleaved with NEGATED means and variance terms,
 //   {detA, detB, -muA_0, -muB_0, -vA_0, -vB_0, -muA_1, ...}            (psb_api.cu build_records)
 // so that the reference's sub / mul / mul / sub chain becomes add / mul / mul / add on float2:
 //   x - mu == x + (-mu),  (sq * v) negated == sq * (-v),  d - c == d + (-c)   -- all exact in IEEE,
-// and __fadd2_rn/__fmul2_rn round each half exactly like __fadd_rn/__fmul_rn (sm_100_rt.h).
-// The final accumulation stays SCALAR on purpose: ptxas (12.9) contracts mul.rn.f32x2 followed by
-// add.rn.f32x2 into FFMA2 even with explicit .rn and -fmad=false, which would skip the separate
-// rounding of the product; scalar add.rn.f32 is never contracted.  FP issue slots per codeword:
-// 52 scalar -> 32.5 (FADD2 + 2 FMUL2 per pair of codewords and dimension, plus one FADD each).
+// and each half rounds exactly like __fadd_rn/__fmul_rn; one record load serves two codewords.
+// The final accumulation stays SCALAR, as in gau_dist.
 template <int FL, bool PEN = false>
 __device__ __forceinline__ float2 gau_dist2(const float4 *__restrict__ r, const float2 (&xx)[FL], float2 *dpen = nullptr)
 {
@@ -61,9 +58,9 @@ __device__ __forceinline__ float2 gau_dist2(const float4 *__restrict__ r, const 
     float2 d = rr[0];
 #pragma unroll
     for (int j = 0; j < FL; ++j) {
-        float2 t = __fadd2_rn(xx[j], rr[1 + 2 * j]);
-        t = __fmul2_rn(t, t);
-        t = __fmul2_rn(t, rr[2 + 2 * j]);
+        float2 t = psb_fadd2_rn(xx[j], rr[1 + 2 * j]);
+        t = psb_fmul2_rn(t, t);
+        t = psb_fmul2_rn(t, rr[2 + 2 * j]);
         if (PEN && j == FL - 1) *dpen = d;
         d.x = __fadd_rn(d.x, t.x);
         d.y = __fadd_rn(d.y, t.y);

@@ -526,7 +526,7 @@ extern "C" int psb_phoneloop_run_host(psb_phoneloop_t *p, const int16_t *senscr,
 // never reach the best score.
 constexpr int HS_V = 4;                     // instances per thread
 constexpr int HS_TS = 512;                  // storage tile: [tile][field][HS_TS], so a CTA's fields are one contiguous block
-// threads per CTA: 128 (default; measured 112.7 us vs 118.2 us per 6.08 M-instance frame) or 256 (PSB_HMMSET_THREADS)
+// threads per CTA: 128 (default) or 256 (PSB_HMMSET_THREADS)
 
 struct psb_hmmset_s {
     psb_hmmctx_t *c;
@@ -803,7 +803,7 @@ hmmset_eval_kernel(HmmSetDev s, HmmCtxDev c, const int16_t *__restrict__ senscr,
 // never evaluated again.  The CTAs of one segment form ONE thread-block cluster: every frame each CTA sends its
 // (maximum, count) into every peer's shared memory with st.async, whose completion is counted on the PEER's mbarrier
 // (8 bytes per peer; the peer waits on its own barrier: one distributed-shared-memory store latency per frame -- a
-// barrier.cluster per frame, ~380 cycles plus an L1 flush, measured 2.9x slower); only the rare histogram frames take
+// barrier.cluster per frame costs ~380 cycles plus an L1 flush); only the rare histogram frames take
 // a barrier.cluster and read the peers' bins (ld.shared::cluster).  No global-memory round trip, no launch per frame.
 __device__ __forceinline__ unsigned cluster_ctarank() { unsigned r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
 __device__ __forceinline__ unsigned cluster_nctarank() { unsigned r; asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r)); return r; }
@@ -836,8 +836,8 @@ hmmset_sweep_kernel(HmmSetDev s, HmmCtxDev c, const int16_t *__restrict__ senscr
 {
     static_assert(!BEAM || THREADS == 256, "the histogram walk maps one bin to one thread");
     // score rows in flight: two for the plain sweep (its frame is longer than half a bulk copy's latency), six under the
-    // beam, where a CTA whose instances have mostly left runs ahead of the copies (measured: no difference, the floor of
-    // the pruned sweep is the per-frame exchange, DESIGN 4.19)
+    // beam, where a CTA whose instances have mostly left runs ahead of the copies (the floor of the
+    // pruned sweep is the per-frame exchange, DESIGN 4.19)
     constexpr int NBUF = BEAM ? 6 : 2;
     extern __shared__ __align__(128) unsigned char sw_smem[];       // [NBUF][buf_bytes] score rows, then the transition matrices
     __shared__ __align__(8) uint64_t full[NBUF];

@@ -20,6 +20,19 @@
 void psb_set_error(const char *fmt, ...);
 extern std::atomic<long long> g_psb_launches;
 
+// Element-wise float2 add / multiply, each half rounded like __fadd_rn / __fmul_rn.  sm_90 has no packed FP32
+// instruction, so these are two scalar operations; the explicit .rn keeps ptxas from contracting them into FFMA.
+__device__ __forceinline__ float2 psb_fadd2_rn(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 psb_fmul2_rn(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+
+// SMs of `device`, for launch shapes that aim at a number of waves (a failed query leaves 1: the launch reports the error)
+inline int psb_sm_count(int device)
+{
+    int n = 1;
+    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, device);
+    return n;
+}
+
 #define PSB_CUDA(call)                                                                   \
     do {                                                                                 \
         cudaError_t e__ = (call);                                                        \
@@ -70,7 +83,7 @@ struct psb_model_s {
     float *d_rec;                 // records; (cb, f) block at rec_off[cb * n_feat + f]
     std::vector<size_t> rec_off;  // float offsets, host copy
     size_t *d_rec_off;
-    float *d_rec2;                // pair-interleaved, negated records for the packed-FP32 kernels
+    float *d_rec2;                // pair-interleaved, negated records for the codeword-pair kernels
     size_t *d_rec2_off;
     uint8_t *d_mixw;              // [n_feat][n_density][mixw_stride] (ptm/semi) or raw pdf (ms)
     uint8_t *d_mixw_cb;           // 16 bytes or null
@@ -117,8 +130,8 @@ struct psb_batch_s {
     long long last_frames;
     float2 *d_semi_dist; size_t semi_cap;      // semi-continuous split path: {d, partial} per (stream, frame, codeword)
     int32_t *d_uttoff; size_t uttoff_cap;
-    int topn_variant;             // PSB_TOPN_VARIANT: 0 scalar, 1/2 packed FP32, 3 two utterances per lane,
-                                  // 4/5 packed + deferred insertion (2 / 1 utterances per lane),
+    int topn_variant;             // PSB_TOPN_VARIANT: 0 scalar, 1/2 codeword pairs, 3 two utterances per lane,
+                                  // 4/5 pairs + deferred insertion (2 / 1 utterances per lane),
                                   // 6 (default) tensor-core filter + exact rescoring where the model allows, else 5
     unsigned *d_tc_flags; size_t tc_flag_cap, tc_flag_words;   // [K][words]: frames the tie fix-up redoes
     float *d_tc_check;            // debug (PSB_TC_CHECK=1): max |a - d| / eps, max candidates

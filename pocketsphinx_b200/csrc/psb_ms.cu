@@ -119,9 +119,9 @@ __device__ __forceinline__ int logadd_wide(const uint32_t *__restrict__ tab, int
 // registers, 32 warps per SM: twice the shared-memory instructions per floating-point operation, twice the warps to hide them).
 constexpr int MS_TCB = 32, MS_TFB = 64;      // codebooks per CTA, frames per block
 
-// PK: frame PAIRS through FADD2 / FMUL2 (x - m == x + (-m) exactly, the means are staged negated; every product and
-// difference is rounded separately as before and the running sums stay scalar -- ptxas would contract a packed
-// multiply-add): 3 packed + 2 scalar instructions per pair and (density, dimension) instead of 8 scalar.
+// PK: frame PAIRS through psb_fadd2_rn / psb_fmul2_rn (x - m == x + (-m) exactly, the means are staged negated; every
+// product and difference is rounded separately as before and the running sums stay scalar).  On sm_90 each float2
+// operation is two scalar instructions; a pair shares the loads of the mean and variance term.
 // FUSE (continuous models: senone s owns codebook s): the lane that holds a codebook's list evaluates the senone on the spot --
 // senone_eval (ms_senone.c:358-407) exactly as ms_senone_kernel does, first clamp, raw int16 score, per-frame minimum -- so
 // the lists (16 MB per 64 frames at 5138 x 8) never travel to HBM and back and one launch per chunk goes away.
@@ -213,9 +213,9 @@ ms_dist_tile_kernel(const float *__restrict__ gT, const float *__restrict__ detT
                         const float2 nm2 = make_float2(m, m), vv = make_float2(v, v);        // m holds the negated mean
 #pragma unroll
                         for (int q = 0; q < MS_TFT; q += 2) {
-                            float2 t = __fadd2_rn(make_float2(xv[q], xv[q + 1]), nm2);
-                            t = __fmul2_rn(t, t);
-                            t = __fmul2_rn(t, vv);
+                            float2 t = psb_fadd2_rn(make_float2(xv[q], xv[q + 1]), nm2);
+                            t = psb_fmul2_rn(t, t);
+                            t = psb_fmul2_rn(t, vv);
                             dv[q] = __fsub_rn(dv[q], t.x);                                   // :467-470
                             dv[q + 1] = __fsub_rn(dv[q + 1], t.y);
                         }
@@ -295,14 +295,11 @@ ms_dist_tile_kernel(const float *__restrict__ gT, const float *__restrict__ detT
     }
 }
 
-// EXPERIMENT (PSB_MS_PACKED=1; bit-identical -- the whole GPU suite passes with it -- but measured
-// slightly SLOWER on B200: 181 ms vs 174 ms, the kernel is not issue-bound).
-// Packed-FP32 variant of ms_dist_kernel: the FT = 4 frames of a thread go through FADD2 / FMUL2 two
-// at a time (features staged as float2 pairs, the mean and variance term are scalar-broadcast
-// operands); x - m == x + (-m) exactly, every product and difference is rounded separately and the
-// running sums stay scalar (ptxas would contract a packed multiply-add).  Same bits, fewer issue
-// slots: 2 LDG + 2 LDS.64 + 1 negate + 6 packed + 4 scalar per (density, dimension) instead of
-// 2 LDG + 4 LDS + 16 scalar.
+// EXPERIMENT (PSB_MS_PACKED=1; bit-identical -- the whole GPU suite passes with it).
+// Pair variant of ms_dist_kernel: the FT = 4 frames of a thread go through psb_fadd2_rn / psb_fmul2_rn two
+// at a time (features staged as float2 pairs, the mean and variance term shared by the pair);
+// x - m == x + (-m) exactly, every product and difference is rounded separately and the running sums
+// stay scalar.  Same bits; on sm_90 the float2 operations are scalar pairs, so only loads are saved.
 template <int NT>
 __global__ void __launch_bounds__(128)
 ms_dist2_kernel(const float *__restrict__ gT, const float *__restrict__ detT, const float *__restrict__ feats,
@@ -341,9 +338,9 @@ ms_dist2_kernel(const float *__restrict__ gT, const float *__restrict__ detT, co
                 const float2 nm = make_float2(-m, -m), vv = make_float2(v, v);
 #pragma unroll
                 for (int q = 0; q < FT; q += 2) {
-                    float2 t = __fadd2_rn(sx2[(q >> 1) * sumlen + fo + j], nm);
-                    t = __fmul2_rn(t, t);
-                    t = __fmul2_rn(t, vv);
+                    float2 t = psb_fadd2_rn(sx2[(q >> 1) * sumlen + fo + j], nm);
+                    t = psb_fmul2_rn(t, t);
+                    t = psb_fmul2_rn(t, vv);
                     dv[q] = __fsub_rn(dv[q], t.x);                                        // :467-470
                     dv[q + 1] = __fsub_rn(dv[q + 1], t.y);
                 }
@@ -441,8 +438,7 @@ __global__ void fill_i32(int32_t *p, long long n, int32_t v)
 }
 
 
-// EXPERIMENT (PSB_MS_REGTILE=1; bit-identical, but measured SLOWER on B200: 247 ms vs 174 ms for
-// 255 k frames of the 5138 x 8 x 39 model, so it is off by default).
+// EXPERIMENT (PSB_MS_REGTILE=1; bit-identical, off by default).
 // Register-tiled variant for small codebooks (n_density <= ND_MAX, the continuous-model case):
 // ms_dist_kernel issues one shared-memory load per 4 flops (the feature value of each frame for
 // every (density, dimension)); here a chunk of CH dimensions of the FT frames sits in registers
@@ -574,8 +570,8 @@ int psb_launch_ms_batch(psb_batch_t *b, const float *d_feats, const int32_t *utt
         dim3 g1((m->n_mgau + 127) / 128, (unsigned)((n + FT - 1) / FT));
         size_t smem = (size_t)FT * m->sumlen * sizeof(float);
         int2 *dist = reinterpret_cast<int2 *>(b->d_msdist);
-        static const bool packed = getenv("PSB_MS_PACKED") != nullptr;       // experiment, off: bit-identical, 181 vs 174 ms
-        static const bool no_tile = getenv("PSB_MS_NOTILE") != nullptr;     // PSB_MS_NOTILE=1: the round-1 kernel (parameters streamed from L2)
+        static const bool packed = getenv("PSB_MS_PACKED") != nullptr;       // experiment, off: bit-identical
+        static const bool no_tile = getenv("PSB_MS_NOTILE") != nullptr;     // PSB_MS_NOTILE=1: the untiled kernel (parameters streamed from L2)
         const size_t tile_smem = ((size_t)m->n_density * m->sumlen * 2 + (size_t)m->n_feat * m->n_density) * MS_TCB * sizeof(float)
                                  + (size_t)m->sumlen * MS_TFB * sizeof(float);
         const bool tile = !no_tile && !packed && !reg_tile_env() && tile_smem <= 100 * 1024;
@@ -583,10 +579,11 @@ int psb_launch_ms_batch(psb_batch_t *b, const float *d_feats, const int32_t *utt
         static const bool tile_pk = [] { const char *v = getenv("PSB_MS_PK"); return !(v && atoi(v) == 0); }();       // packed FP32 pairs (default) or scalar
         // frames per CTA: enough CTAs for ~4 waves of two resident CTAs per SM, whole 32-frame blocks
         const int tiles_x = (m->n_mgau + MS_TCB - 1) / MS_TCB;
-        long long fpc = (n * tiles_x + 148LL * 2 * 4 - 1) / (148LL * 2 * 4);
+        const long long waves = psb_sm_count(m->device) * 2LL * 4;
+        long long fpc = (n * tiles_x + waves - 1) / waves;
         fpc = std::max<long long>(MS_TFB, (fpc + MS_TFB - 1) / MS_TFB * MS_TFB);
         const dim3 gt((unsigned)tiles_x, (unsigned)((n + fpc - 1) / fpc));
-        static const bool reg_tile = getenv("PSB_MS_REGTILE") != nullptr;   // experiment, off: measured slower (247 vs 174 ms)
+        static const bool reg_tile = getenv("PSB_MS_REGTILE") != nullptr;   // experiment, off: bit-identical
         static const bool no_fuse = [] { const char *v = getenv("PSB_MS_FUSE"); return v && atoi(v) == 0; }();
         // continuous models: mixtures evaluated by the lane that holds the list (the kernel writes raw scores and minima)
         const bool fuse = tile && !no_fuse && m->sen_is_cb && tile_tft4 && tile_pk && m->n_mgau > 1;

@@ -1,4 +1,4 @@
-// psb_ptm.cu -- batched PTM senone evaluation for sm_100a.
+// psb_ptm.cu -- batched PTM senone evaluation for sm_90a.
 //
 // Replaces, for whole batches of utterances with all senones computed (compallsen):
 //   eval_topn / eval_cb / ptm_mgau_codebook_eval  (ptm_mgau.c:88-254)   -> ptm_topn_kernel
@@ -429,9 +429,9 @@ ptm_topn2_kernel(const float *__restrict__ rec2, const size_t *__restrict__ rec2
 // stream of Gaussian records at ~65 % of the shared-memory pipe with `short scoreboard` the top
 // stall: a broadcast load delivers 8 bytes per wavefront however many lanes listen.  Here every
 // record load feeds TWO utterances per lane: the pair (x_u0, x_u1) goes through one
-// FADD2 / FMUL2 / FMUL2 with the model value as a broadcast scalar operand (so the scalar records
-// are used as they are: t = x + (-mu), t*t, (t*t)*v, then d_u -= t_u with scalar FADDs, which
-// ptxas never contracts).  Shared-memory traffic per (utterance, codeword) halves and each warp
+// psb_fadd2_rn / psb_fmul2_rn / psb_fmul2_rn with the model value shared by both (so the scalar records
+// are used as they are: t = x + (-mu), t*t, (t*t)*v, then d_u -= t_u with scalar FADDs; on sm_90 each
+// float2 operation is two scalar instructions).  Shared-memory traffic per (utterance, codeword) halves and each warp
 // carries two independent dependency chains.
 struct U2State {
     unsigned cwp;           // four listed codewords, byte j = cw_j
@@ -574,9 +574,9 @@ ptm_topn_u2_kernel(const float *__restrict__ rec, const size_t *__restrict__ rec
                     float d0 = rr[0], d1 = rr[0], p0 = rr[0], p1 = rr[0];
 #pragma unroll
                     for (int j = 0; j < FL; ++j) {
-                        float2 tt = __fadd2_rn(xx[j], make_float2(-rr[1 + 2 * j], -rr[1 + 2 * j]));
-                        tt = __fmul2_rn(tt, tt);
-                        tt = __fmul2_rn(tt, make_float2(rr[2 + 2 * j], rr[2 + 2 * j]));
+                        float2 tt = psb_fadd2_rn(xx[j], make_float2(-rr[1 + 2 * j], -rr[1 + 2 * j]));
+                        tt = psb_fmul2_rn(tt, tt);
+                        tt = psb_fmul2_rn(tt, make_float2(rr[2 + 2 * j], rr[2 + 2 * j]));
                         if (SEMI && j == FL - 1) { p0 = d0; p1 = d1; }
                         d0 = __fsub_rn(d0, tt.x);
                         d1 = __fsub_rn(d1, tt.y);
@@ -810,9 +810,9 @@ ptm_topnq_kernel(const float *__restrict__ rec2, const size_t *__restrict__ rec2
                 for (int j = 0; j < FL; ++j) {
 #pragma unroll
                     for (int u = 0; u < NU; ++u) {
-                        float2 tt = __fadd2_rn(xx[u][j], rr[1 + 2 * j]);
-                        tt = __fmul2_rn(tt, tt);
-                        tt = __fmul2_rn(tt, rr[2 + 2 * j]);
+                        float2 tt = psb_fadd2_rn(xx[u][j], rr[1 + 2 * j]);
+                        tt = psb_fmul2_rn(tt, tt);
+                        tt = psb_fmul2_rn(tt, rr[2 + 2 * j]);
                         d[u].x = __fadd_rn(d[u].x, tt.x);             // scalar on purpose: see gau_dist2
                         d[u].y = __fadd_rn(d[u].y, tt.y);
                     }
@@ -1343,7 +1343,7 @@ int launch_topn(psb_batch_t *b, const int32_t *d_klist, int n_k, const GroupTabs
         size_t smem = (size_t)m->n_density * rec_floats(FL) * sizeof(float);
         auto kern = ptm_topn_kernel<FL, SEMI, true>;
         PSB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        const int warps = (long long)n_k * ((n_groups + TOPN_WARPS - 1) / TOPN_WARPS) >= 4 * 148 ? TOPN_WARPS : 1;
+        const int warps = (long long)n_k * ((n_groups + TOPN_WARPS - 1) / TOPN_WARPS) >= 4 * psb_sm_count(m->device) ? TOPN_WARPS : 1;
         dim3 grid(n_k, (n_groups + warps - 1) / warps);
         kern<<<grid, warps * 32, smem, b->stream>>>(m->d_rec, m->d_rec_off, d_klist, b->d_featT, tabs, b->d_topn, n_groups,
                                                    m->n_density, m->n_feat, m->sumlen, d_featoff, m->K, m->ds_ratio,
@@ -1364,7 +1364,7 @@ int launch_topn(psb_batch_t *b, const int32_t *d_klist, int n_k, const GroupTabs
         auto kern = ptm_topn_u2_kernel<FLU, SEMI>;
         PSB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         const int n_w = (n_groups + 1) / 2;
-        const int warps = (long long)n_k * ((n_w + 3) / 4) >= 2 * 148 ? 4 : 1;
+        const int warps = (long long)n_k * ((n_w + 3) / 4) >= 2 * psb_sm_count(m->device) ? 4 : 1;
         dim3 grid(n_k, (n_w + warps - 1) / warps);
         kern<<<grid, warps * 32, smem, b->stream>>>(m->d_rec, m->d_rec_off, d_klist, b->d_featT, tabs, b->d_topn, n_groups,
                                                    m->n_density, m->n_feat, m->sumlen, d_featoff, m->K, m->ds_ratio,
@@ -1373,7 +1373,7 @@ int launch_topn(psb_batch_t *b, const int32_t *d_klist, int n_k, const GroupTabs
         return PSB_OK;
     }
     if (FL <= 16 && m->d_rec2 && b->topn_variant != 0) {
-        // packed-FP32 kernels (FL <= 16 keeps the register budget): variant 1 = 2 warps/CTA with a
+        // codeword-pair kernels (FL <= 16 keeps the register budget): variant 1 = 2 warps/CTA with a
         // large register budget (two balanced waves), variant 2 = 4 warps/CTA at 72 registers
         if (b->topn_variant != 1) return launch_topn2<FL <= 16 ? FL : 1, SEMI, 4, 7>(b, d_klist, n_k, tabs, n_groups, d_featoff);
         return launch_topn2<FL <= 16 ? FL : 1, SEMI, 2, 7>(b, d_klist, n_k, tabs, n_groups, d_featoff);
@@ -1382,7 +1382,7 @@ int launch_topn(psb_batch_t *b, const int32_t *d_klist, int n_k, const GroupTabs
     PSB_CUDA(cudaFuncSetAttribute(ptm_topn_kernel<FL, SEMI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     // few (pair, group) items (semi-continuous models, small batches): one warp per CTA spreads
     // them over more SMs; otherwise 4 warps share one staged codebook
-    const int warps = (long long)n_k * ((n_groups + TOPN_WARPS - 1) / TOPN_WARPS) >= 4 * 148 ? TOPN_WARPS : 1;
+    const int warps = (long long)n_k * ((n_groups + TOPN_WARPS - 1) / TOPN_WARPS) >= 4 * psb_sm_count(m->device) ? TOPN_WARPS : 1;
     dim3 grid(n_k, (n_groups + warps - 1) / warps);
     ptm_topn_kernel<FL, SEMI><<<grid, warps * 32, smem, b->stream>>>(
         m->d_rec, m->d_rec_off, d_klist, b->d_featT, tabs, b->d_topn, n_groups, m->n_density,
@@ -1693,8 +1693,8 @@ int psb_launch_ptm_batch(psb_batch_t *b, const float *d_feats, const int32_t *ut
             // at least 256 threads (log-add table staging) and one thread per (codebook, stream) pair
             const int threads = std::min(512, std::max(std::max(256, roundup(K, 32)), roundup((n_quads + iters - 1) / iters, 32)));
             const size_t smem4 = smem + 8 + (size_t)K * 16;
-            // experiment, off by default: measured 30.8 ms vs 18.9 ms per 998 k frames -- the 4 KB two-index table trades two
-            // mostly-broadcast byte reads for one read that bank-conflicts across 1024 words (bit-identical either way)
+            // experiment, off by default: the 4 KB two-index table trades two mostly-broadcast byte reads for one read
+            // that bank-conflicts across 1024 words (bit-identical either way)
             static const bool use_tab2 = getenv("PSB_SENONE_TAB2") && atoi(getenv("PSB_SENONE_TAB2")) == 1;
             if (m->logadd8_zero_from <= 31 && use_tab2) {
                 const size_t smem5 = smem4 + 16 + 4096;

@@ -35,7 +35,7 @@
 //
 // The exact stage keeps the warp-uniform record stream of the old kernels: lane = frame (32
 // consecutive frames of the batch per warp), the warp walks the UNION of its lanes' E sets pair by
-// pair with the packed FADD2/FMUL2 distance (gau_dist2) and each lane keeps the five best of its
+// pair with the codeword-pair distance (gau_dist2) and each lane keeps the five best of its
 // own set.  A row whose candidate list overflows its shared-memory slots falls back to E = C; a warp
 // whose rows agree on nothing degrades towards the dense scan, never below it.
 //
@@ -369,168 +369,133 @@ ptm_tc_kernel(const float *__restrict__ feats, long long total, int D, const int
 }
 
 // ---------------------------------------------------------------------------------------
-// The same filter on the 5th-generation tensor cores (tcgen05): the legacy mma.sync path above tops out
-// near 290 TFLOP/s of TF32 (8 cycles per m16n8k8 and sub-core), which makes the 3 x TF32 GEMM -- 6.2 TFLOP
-// per 10^6-frame batch -- the longest stage.  Here one elected thread issues twelve
-// tcgen05.mma.cta_group::1.kind::tf32 (M 128 frames x N n_density x K 8; lo*hi, hi*lo, hi*hi over four
-// K steps) per 128-frame tile, A (the X tile, split into TF32 halves) and B (W, both halves) in shared memory
-// in the canonical K-major no-swizzle layout (8-row x 16-byte core matrices; descriptors built below), the
-// fp32 accumulator in TENSOR MEMORY: 128 lanes x n_density columns.  tcgen05.commit arrives on an mbarrier;
-// after the wait every thread reads ITS OWN frame's row (TMEM lane = frame = thread) with tcgen05.ld.32x32b in
-// slabs of 32 columns, twice: group maxima -> threshold, then the columns above it.  No accumulator registers
-// across the sweep, no shuffles, no shared-memory atomics -- the whole selection is thread-private.  A CTA keeps
-// W resident and walks `tiles_per_cta` consecutive tiles of its pair.
-__device__ __forceinline__ uint64_t umma_smem_desc(const void *p, unsigned lbo_bytes, unsigned sbo_bytes)
+// The same filter on Hopper's warpgroup MMA: each warpgroup issues twelve wgmma.mma_async m64nNDk8 TF32 (lo*hi, hi*lo,
+// hi*hi over four K steps) per 64 frames, A (X rows split into TF32 halves) and B (W, both halves) straight from shared
+// memory in the canonical K-major no-swizzle layout, the fp32 accumulator in registers.  A frame's row is spread over the
+// four lanes of a quad: group maxima meet by shuffles, candidates go to the row's shared-memory list, one thread per row
+// resolves it.  The two warpgroups of a CTA share W and run their 64-frame halves independently (named barriers), so the
+// GEMM of one overlaps the selection of the other; a CTA walks `tiles_per_cta` consecutive tiles of its pair.
+constexpr int WG_ROWS = 64;                                                   // frames per warpgroup and tile
+constexpr int WG_EXTRA = TC_CAP * WG_ROWS * 4 + WG_ROWS * 4 + WG_ROWS * 4 + TC_CAP * WG_ROWS;   // lists, counts, bounds
+
+__device__ __forceinline__ uint64_t wgmma_desc(const void *p, unsigned lbo_bytes, unsigned sbo_bytes)
 {
-    // cute::UMMA::SmemDescriptor (mma_sm100_desc.hpp): start address, leading / stride byte offsets in 16-byte units,
-    // version 1 (Blackwell) at bit 46, base offset 0, layout type 0 = no swizzle
-    const uint64_t a = (uint64_t)((unsigned)__cvta_generic_to_shared(p) >> 4) & 0x3fffu;
-    return a | ((uint64_t)((lbo_bytes >> 4) & 0x3fffu) << 16) | ((uint64_t)((sbo_bytes >> 4) & 0x3fffu) << 32) | (1ull << 46);
+    // sm_90 shared-memory matrix descriptor: start address, leading (K direction) and stride (M / N direction) byte
+    // offsets between core matrices, all in 16-byte units; base offset 0, layout type 0 = no swizzle
+    const uint64_t a = (uint64_t)(((unsigned)__cvta_generic_to_shared(p) >> 4) & 0x3fffu);
+    return a | ((uint64_t)((lbo_bytes >> 4) & 0x3fffu) << 16) | ((uint64_t)((sbo_bytes >> 4) & 0x3fffu) << 32);
 }
 
-__device__ __forceinline__ void umma_tf32(unsigned tmem_d, uint64_t adesc, uint64_t bdesc, unsigned idesc, unsigned accumulate)
+// the accumulator registers pass through here: nothing that reads or writes them moves across a wgmma fence or wait
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[R])
 {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, {%5, %5, %5, %5}, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(0u)
-        : "memory");
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-__device__ __forceinline__ void tmem_ld32_issue(unsigned taddr, float (&v)[32])
-{
-    // destination = the caller's registers themselves (bit-size operands take .f32 registers): no move may sit between the
-    // load and the wait that makes them valid
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-        : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]), "=f"(v[4]), "=f"(v[5]), "=f"(v[6]), "=f"(v[7]), "=f"(v[8]), "=f"(v[9]),
-          "=f"(v[10]), "=f"(v[11]), "=f"(v[12]), "=f"(v[13]), "=f"(v[14]), "=f"(v[15]), "=f"(v[16]), "=f"(v[17]), "=f"(v[18]),
-          "=f"(v[19]), "=f"(v[20]), "=f"(v[21]), "=f"(v[22]), "=f"(v[23]), "=f"(v[24]), "=f"(v[25]), "=f"(v[26]), "=f"(v[27]),
-          "=f"(v[28]), "=f"(v[29]), "=f"(v[30]), "=f"(v[31])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// the same wait, but the compiler is told that the slab's registers pass through it: nothing that reads them can be
-// scheduled above the wait when the load was issued earlier (software pipelining of the sweeps)
-__device__ __forceinline__ void tmem_wait_ld_dep(float (&v)[32])
-{
-    asm volatile("tcgen05.wait::ld.sync.aligned;"
-                 : "+f"(v[0]), "+f"(v[1]), "+f"(v[2]), "+f"(v[3]), "+f"(v[4]), "+f"(v[5]), "+f"(v[6]), "+f"(v[7]), "+f"(v[8]), "+f"(v[9]),
-                   "+f"(v[10]), "+f"(v[11]), "+f"(v[12]), "+f"(v[13]), "+f"(v[14]), "+f"(v[15]), "+f"(v[16]), "+f"(v[17]), "+f"(v[18]),
-                   "+f"(v[19]), "+f"(v[20]), "+f"(v[21]), "+f"(v[22]), "+f"(v[23]), "+f"(v[24]), "+f"(v[25]), "+f"(v[26]), "+f"(v[27]),
-                   "+f"(v[28]), "+f"(v[29]), "+f"(v[30]), "+f"(v[31])
-                 :
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(unsigned taddr, float (&v)[32])
-{
-    tmem_ld32_issue(taddr, v);
-    tmem_wait_ld();
-}
+__device__ __forceinline__ void warpgroup_bar(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
 
-__device__ __forceinline__ void mbar_init1(uint64_t *bar)
-{
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"((unsigned)__cvta_generic_to_shared(bar)));
-}
-__device__ __forceinline__ void mbar_wait_parity(uint64_t *bar, unsigned parity)
-{
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "TCW_%=:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-        "@p bra TCD_%=;\n"
-        "bra TCW_%=;\n"
-        "TCD_%=:\n"
-        "}\n" ::"r"((unsigned)__cvta_generic_to_shared(bar)),
-        "r"(parity)
-        : "memory");
-}
+// D[64 x N] (+)= A[64 x 8] * B[8 x N], TF32 in, fp32 accumulate, A and B from shared memory (descriptors)
+template <int N>
+struct Wgmma;
+#define PSB_ACC8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+template <> struct Wgmma<64> {
+    static __device__ __forceinline__ void mma(float (&d)[32], uint64_t a, uint64_t b, int accumulate)
+    {
+        asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\nwgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {"
+        "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,"
+        "%30,%31"
+        "}, %32, %33, p, 1, 1;\n}\n"
+        : PSB_ACC8(0), PSB_ACC8(8), PSB_ACC8(16), PSB_ACC8(24)
+        : "l"(a), "l"(b), "r"(accumulate));
+    }
+};
+template <> struct Wgmma<128> {
+    static __device__ __forceinline__ void mma(float (&d)[64], uint64_t a, uint64_t b, int accumulate)
+    {
+        asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\nwgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {"
+        "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,"
+        "%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,"
+        "%57,%58,%59,%60,%61,%62,%63"
+        "}, %64, %65, p, 1, 1;\n}\n"
+        : PSB_ACC8(0), PSB_ACC8(8), PSB_ACC8(16), PSB_ACC8(24), PSB_ACC8(32), PSB_ACC8(40), PSB_ACC8(48), PSB_ACC8(56)
+        : "l"(a), "l"(b), "r"(accumulate));
+    }
+};
+template <> struct Wgmma<256> {
+    static __device__ __forceinline__ void mma(float (&d)[128], uint64_t a, uint64_t b, int accumulate)
+    {
+        asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %130, 0;\nwgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 {"
+        "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,"
+        "%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,"
+        "%57,%58,%59,%60,%61,%62,%63,%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,%80,%81,%82,%83,"
+        "%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,"
+        "%109,%110,%111,%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127"
+        "}, %128, %129, p, 1, 1;\n}\n"
+        : PSB_ACC8(0), PSB_ACC8(8), PSB_ACC8(16), PSB_ACC8(24), PSB_ACC8(32), PSB_ACC8(40), PSB_ACC8(48), PSB_ACC8(56),
+          PSB_ACC8(64), PSB_ACC8(72), PSB_ACC8(80), PSB_ACC8(88), PSB_ACC8(96), PSB_ACC8(104), PSB_ACC8(112),
+          PSB_ACC8(120)
+        : "l"(a), "l"(b), "r"(accumulate));
+    }
+};
+#undef PSB_ACC8
 
 //   wumma   [K][2][8][ND][4] float   W halves (high, low) in the canonical K-major layout: chunk kc holds k = 4 kc .. 4 kc + 3
-// SPLIT = 2: two threads per frame (256 threads per CTA), each sweeping half of the columns of the SAME accumulator row
-// (warps w and w + 4 own the same 32 TMEM lanes): the accumulator sweeps are the longest serial stretch of a tile and the
-// tensor memory (two 256-column accumulators per SM) caps the CTAs at two, so this is the way to put sixteen warps on
-// an SM.  The halves meet twice: eight group maxima per row, and the two candidate sub-lists that thread 0 of the pair resolves.
-template <int FL, int ND, int SPLIT, bool CHECK>
-__global__ void __launch_bounds__(TC_ROWS * SPLIT, 2)
-ptm_tc5_kernel(const float *__restrict__ feats, long long total, int D, const int32_t *__restrict__ featoff,
-               const int32_t *__restrict__ klist, const float *__restrict__ wumma, const float *__restrict__ cen,
-               const float *__restrict__ bnd, const float *__restrict__ rec, const size_t *__restrict__ rec_off,
-               int4 *__restrict__ out, unsigned *__restrict__ flags, long long flag_words, int K, int n_feat,
-               int tiles_per_cta, uint4 *__restrict__ items, unsigned *__restrict__ n_items, unsigned item_cap,
-               float *__restrict__ check, unsigned long long *__restrict__ stats)
+template <int FL, int ND, bool CHECK>
+__global__ void __launch_bounds__(2 * 128, 1)
+ptm_wgmma_kernel(const float *__restrict__ feats, long long total, int D, const int32_t *__restrict__ featoff,
+                 const int32_t *__restrict__ klist, const float *__restrict__ wumma, const float *__restrict__ cen,
+                 const float *__restrict__ bnd, const float *__restrict__ rec, const size_t *__restrict__ rec_off,
+                 int4 *__restrict__ out, unsigned *__restrict__ flags, long long flag_words, int K, int n_feat,
+                 int tiles_per_cta, uint4 *__restrict__ items, unsigned *__restrict__ n_items, unsigned item_cap,
+                 float *__restrict__ check, unsigned long long *__restrict__ stats)
 {
     constexpr int RF = (1 + 2 * FL + 3) / 4 * 4;
-    constexpr int GW = ND / 8;                           // columns per maximum group: 8 groups per row
-    constexpr int NT_ = TC_ROWS * SPLIT;                 // threads
-    constexpr int NDH = ND / SPLIT;                      // columns per thread
-    constexpr int CAPH = SPLIT == 1 ? TC_CAP : 12;       // candidate slots per thread
-    constexpr int SD = 32 / SPLIT;                       // columns staged at a time
-    static_assert(2 * FL + 1 <= TC_K && ND % 32 == 0 && ND <= 256 && NDH % 64 == 0 && (SPLIT == 1 || SPLIT == 2), "shape");
-    extern __shared__ __align__(128) unsigned char t5_smem[];
-    float *sW = reinterpret_cast<float *>(t5_smem);                                   // [2][8][ND][4]
-    float *sX = sW + 2 * 8 * ND * 4;                                                  // [2][8][128][4]; after the MMA: lists + staging
-    // thread-private and transposed ([slot][thread]: conflict-free): candidate values, candidate columns, one 32-column slab
-    float *Lv = sX;                                                                   // [CAPH][threads]
-    unsigned char *Lc = reinterpret_cast<unsigned char *>(Lv + CAPH * NT_);           // [CAPH][threads]
-    float *stage = reinterpret_cast<float *>(Lc + ((CAPH * NT_ + 15) & ~15));         // [SD][threads]
-    static_assert(CAPH * NT_ * 5 + 16 + SD * NT_ * 4 <= 2 * 8 * TC_ROWS * 16, "lists + staging must fit the X tile");
-    __shared__ __align__(8) uint64_t mma_done;
-    __shared__ unsigned tmem_base_s;
-    __shared__ float gmx[SPLIT == 1 ? 1 : TC_ROWS * 8];                               // SPLIT = 2: the row's eight group maxima
-    __shared__ int cnt_s[SPLIT == 1 ? 1 : 2 * TC_ROWS];                               // SPLIT = 2: candidates per half
+    constexpr int NTL = ND / 8;                          // 8-column n-tiles of the accumulator fragment
+    constexpr int NPG = NTL / 8;                         // n-tiles per maximum group: 8 groups per row
+    constexpr unsigned FULL = 0xffffffffu;
+    static_assert(2 * FL + 1 <= TC_K && (ND == 64 || ND == 128 || ND == 256), "shape");
+    extern __shared__ __align__(128) unsigned char wg_smem[];
+    const int tid = threadIdx.x, wg = tid >> 7, t = tid & 127, warp = t >> 5, lane = tid & 31;
+    float *sW = reinterpret_cast<float *>(wg_smem);                                   // [2][8][ND][4]
+    float *sX = sW + 2 * 8 * ND * 4 + wg * (2 * 8 * WG_ROWS * 4);                     // this warpgroup's [2][8][64][4]
+    unsigned char *ex = wg_smem + (size_t)2 * 8 * ND * 16 + 2 * (2 * 8 * WG_ROWS * 16) + (size_t)wg * WG_EXTRA;
+    float *Lv = reinterpret_cast<float *>(ex);                                        // [TC_CAP][64] candidate values
+    int *cnt = reinterpret_cast<int *>(Lv + TC_CAP * WG_ROWS);                        // [64] candidates per row
+    float *epsr = reinterpret_cast<float *>(cnt + WG_ROWS);                           // [64] error bound per row
+    unsigned char *Lc = reinterpret_cast<unsigned char *>(epsr + WG_ROWS);            // [TC_CAP][64] candidate columns
 
     // grid: x = pair (fastest), y = group of tiles: CTAs that run together read the SAME frames for different pairs, so
-    // the feature rows come out of L2 (with tiles fastest every pair re-read the whole feature matrix from HBM: 23 GB
-    // per 998 k frames in the first ncu capture) while the 126 W blocks (8 MB) stay L2-resident
+    // the feature rows come out of L2 while the W blocks of all pairs stay L2-resident
     const int k = klist[blockIdx.x];
     const int f = k % n_feat;
-    const int tid = threadIdx.x, warp = tid >> 5;
-    const int r = tid & (TC_ROWS - 1), half = tid / TC_ROWS;          // this thread's frame of the tile and its half of the columns
-
-    if (warp == 0) {                                     // 256 (or fewer) TMEM columns for the accumulator
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"((unsigned)__cvta_generic_to_shared(&tmem_base_s)),
-                     "n"(ND < 32 ? 32 : ND));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    if (tid == 0) {
-        mbar_init1(&mma_done);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
     {
         const float4 *src = reinterpret_cast<const float4 *>(wumma + (size_t)k * 2 * 8 * ND * 4);
         float4 *dst = reinterpret_cast<float4 *>(sW);
-        for (int i = tid; i < 2 * 8 * ND; i += NT_) dst[i] = src[i];
+        for (int i = tid; i < 2 * 8 * ND; i += 2 * 128) dst[i] = src[i];
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const unsigned tmem_d = tmem_base_s;
-    // instruction descriptor (cute::UMMA::InstrDescriptor): D fp32, A / B tf32, both K-major, N >> 3, M >> 4
-    constexpr unsigned IDESC = (1u << 4) | (2u << 7) | (2u << 10) | ((unsigned)(ND >> 3) << 17) | ((unsigned)(TC_ROWS >> 4) << 24);
     const float *m = cen + (size_t)k * 16, *bb = bnd + (size_t)k * 32;
     const float *rc = rec + rec_off[k];
+    const int r = t & (WG_ROWS - 1), half = t >> 6;     // the frame this thread prepares (and resolves if half == 0)
+    const int g = lane >> 2, q4 = lane & 3;
+    const int ra = warp * 16 + g, rb = ra + 8;           // the two accumulator rows this thread holds columns of
 
     // the next tile's feature row is fetched while this tile's GEMM runs
     float xn[FL];
     {
-        const long long r0 = (long long)blockIdx.y * tiles_per_cta * TC_ROWS + r;
+        const long long r0 = (long long)blockIdx.y * tiles_per_cta * TC_ROWS + wg * WG_ROWS + r;
         const float *p = feats + (r0 < total ? r0 : 0) * D + featoff[f];
 #pragma unroll
         for (int j = 0; j < FL; ++j) xn[j] = r0 < total ? p[j] : 0.f;
     }
     for (int tile = 0; tile < tiles_per_cta; ++tile) {
-        const long long row = ((long long)blockIdx.y * tiles_per_cta + tile) * TC_ROWS + r;
-        if (row - r >= total) break;                     // uniform: the whole tile lies past the end
+        const long long row0 = ((long long)blockIdx.y * tiles_per_cta + tile) * TC_ROWS + wg * WG_ROWS;
+        if (row0 >= total) break;                        // uniform in the warpgroup: its rows lie past the end
+        const long long row = row0 + r;
         const bool valid = row < total;
-        // ---- this thread's frame: X row (TF32 halves, canonical layout) and its error bound ----
+        // ---- this thread's frame: X row (TF32 halves, canonical layout; two threads share the stores) and its error bound ----
         float x[FL], ee;
         {
             float v[TC_K];
@@ -551,95 +516,62 @@ ptm_tc5_kernel(const float *__restrict__ feats, long long total, int D, const in
             ee = __fadd_ru(__fmul_ru(S, TC_ERR), 2.0f);
 #pragma unroll
             for (int kc = 0; kc < 8; ++kc) {
-                if (SPLIT == 2 && (kc & 1) != half) continue;         // the pair shares the conversions and stores
+                if ((kc & 1) != half) continue;
                 float4 h, l;
                 h.x = to_tf32(v[4 * kc]); h.y = to_tf32(v[4 * kc + 1]); h.z = to_tf32(v[4 * kc + 2]); h.w = to_tf32(v[4 * kc + 3]);
                 l.x = to_tf32(__fsub_rn(v[4 * kc], h.x)); l.y = to_tf32(__fsub_rn(v[4 * kc + 1], h.y));
                 l.z = to_tf32(__fsub_rn(v[4 * kc + 2], h.z)); l.w = to_tf32(__fsub_rn(v[4 * kc + 3], h.w));
-                reinterpret_cast<float4 *>(sX)[kc * TC_ROWS + r] = h;
-                reinterpret_cast<float4 *>(sX)[(8 + kc) * TC_ROWS + r] = l;
+                reinterpret_cast<float4 *>(sX)[kc * WG_ROWS + r] = h;
+                reinterpret_cast<float4 *>(sX)[(8 + kc) * WG_ROWS + r] = l;
             }
+            if (half == 0) { epsr[r] = ee; cnt[r] = 0; }
         }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic-proxy writes -> visible to the tensor core
-        __syncthreads();
-        if (tid == 0) {
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            // chunk kc of A at sX + kc * 2048 B (128 rows x 16 B), of B at sW + kc * ND * 16 B; core matrices 128 B apart
-            for (int pass = 0; pass < 3; ++pass) {        // lo*hi, hi*lo, hi*hi
-                const int ha = pass == 0 ? 1 : 0, hb = pass == 1 ? 1 : 0;
-                for (int ks = 0; ks < 4; ++ks) {
-                    const uint64_t ad = umma_smem_desc(sX + ((size_t)(ha * 8 + 2 * ks) * TC_ROWS) * 4, TC_ROWS * 16, 128);
-                    const uint64_t bd = umma_smem_desc(sW + ((size_t)(hb * 8 + 2 * ks) * ND) * 4, ND * 16, 128);
-                    umma_tf32(tmem_d, ad, bd, IDESC, (pass | ks) ? 1u : 0u);
-                }
+        warpgroup_bar(1 + wg);
+
+        // ---- 3 x TF32 GEMM of the warpgroup's 64 rows against all ND codewords ----
+        float acc[ND / 2];
+#pragma unroll
+        for (int i = 0; i < ND / 2; ++i) acc[i] = 0.f;
+        wgmma_fence_regs(acc);
+        asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+        // chunk kc of A at sX + kc * 1024 B (64 rows x 16 B), of B at sW + kc * ND * 16 B; core matrices 128 B apart
+#pragma unroll
+        for (int pass = 0; pass < 3; ++pass) {           // lo*hi, hi*lo, hi*hi
+            const int ha = pass == 0 ? 1 : 0, hb = pass == 1 ? 1 : 0;
+#pragma unroll
+            for (int ks = 0; ks < 4; ++ks) {
+                const uint64_t ad = wgmma_desc(sX + (size_t)(ha * 8 + 2 * ks) * WG_ROWS * 4, WG_ROWS * 16, 128);
+                const uint64_t bd = wgmma_desc(sW + (size_t)(hb * 8 + 2 * ks) * ND * 4, ND * 16, 128);
+                Wgmma<ND>::mma(acc, ad, bd, (pass | ks) ? 1 : 0);
             }
-            asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                             (unsigned)__cvta_generic_to_shared(&mma_done))
-                         : "memory");
         }
+        asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
         if (tile + 1 < tiles_per_cta) {
             const long long rn = row + TC_ROWS;
             const float *p = feats + (rn < total ? rn : 0) * D + featoff[f];
 #pragma unroll
             for (int j = 0; j < FL; ++j) xn[j] = rn < total ? p[j] : 0.f;
         }
-        mbar_wait_parity(&mma_done, (unsigned)tile & 1u);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+        asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+        wgmma_fence_regs(acc);
 
-        // ---- this thread's row of the accumulator: group maxima, threshold, the columns above it ----
-        const unsigned trow = tmem_d + ((unsigned)((warp & 3) * 32) << 16) + (unsigned)(half * NDH);
-        float gm[8];
+        // ---- rows ra / rb: group maxima (the quad's four lanes hold a row between them), threshold, the columns above it ----
+        float gma[8], gmb[8];
 #pragma unroll
-        for (int i = 0; i < 8; ++i) gm[i] = -INFINITY;
-        auto maxima = [&](int c0, const float (&v)[32]) {
-            if (GW >= 32) {
-                // a tree, not a chain: with two warps per scheduler the dependent-issue latency is what counts
-                float m8[8];
+        for (int q = 0; q < 8; ++q) {
+            float a = -INFINITY, b = -INFINITY;
 #pragma unroll
-                for (int i = 0; i < 8; ++i) m8[i] = fmaxf(fmaxf(v[i], v[i + 8]), fmaxf(v[i + 16], v[i + 24]));
-                const float mx = fmaxf(fmaxf(fmaxf(m8[0], m8[1]), fmaxf(m8[2], m8[3])), fmaxf(fmaxf(m8[4], m8[5]), fmaxf(m8[6], m8[7])));
-                const int gi = (half * NDH + c0) / GW;
-#pragma unroll
-                for (int q = 0; q < 8; ++q)
-                    if (q == gi) gm[q] = fmaxf(gm[q], mx);
+            for (int i = q * NPG; i < (q + 1) * NPG; ++i) {
+                a = fmaxf(a, fmaxf(acc[4 * i], acc[4 * i + 1]));
+                b = fmaxf(b, fmaxf(acc[4 * i + 2], acc[4 * i + 3]));
             }
-            else {
-                constexpr int PER = 32 / (GW < 32 ? GW : 32);       // groups inside one 32-column slab
-#pragma unroll
-                for (int s2 = 0; s2 < PER; ++s2) {
-                    float mx = v[s2 * GW];
-#pragma unroll
-                    for (int i = 1; i < GW; ++i) mx = fmaxf(mx, v[s2 * GW + i]);
-                    const int gi = (half * NDH + c0) / GW + s2;
-#pragma unroll
-                    for (int q = 0; q < 8; ++q)
-                        if (q == gi) gm[q] = fmaxf(gm[q], mx);
-                }
-            }
-        };
-        {   // two slabs in flight: the load of the next one runs while this one is reduced
-            float va[32], vb[32];
-            tmem_ld32_issue(trow, va);
-#pragma unroll 1
-            for (int c0 = 0; c0 < NDH; c0 += 64) {
-                tmem_wait_ld_dep(va);
-                tmem_ld32_issue(trow + c0 + 32, vb);
-                maxima(c0, va);
-                tmem_wait_ld_dep(vb);
-                if (c0 + 64 < NDH) tmem_ld32_issue(trow + c0 + 64, va);
-                maxima(c0 + 32, vb);
-            }
-        }
-        if (SPLIT == 2) {                                 // the other half's group maxima
-#pragma unroll
-            for (int q = 0; q < 4; ++q) gmx[r * 8 + half * 4 + q] = gm[half * 4 + q];
-            __syncthreads();
-#pragma unroll
-            for (int q = 0; q < 8; ++q) gm[q] = gmx[r * 8 + q];
+            a = fmaxf(a, __shfl_xor_sync(FULL, a, 1)); a = fmaxf(a, __shfl_xor_sync(FULL, a, 2));
+            b = fmaxf(b, __shfl_xor_sync(FULL, b, 1)); b = fmaxf(b, __shfl_xor_sync(FULL, b, 2));
+            gma[q] = a; gmb[q] = b;
         }
         // five distinct columns >= L0: the fifth largest of the eight group maxima
-        float L0;
-        {
+        auto fifth = [](const float (&gm)[8]) {
             float a5[5] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY, -INFINITY};
 #pragma unroll
             for (int q = 0; q < 8; ++q) {
@@ -647,80 +579,62 @@ ptm_tc5_kernel(const float *__restrict__ feats, long long total, int D, const in
 #pragma unroll
                 for (int j = 0; j < 5; ++j) { const float hi = fmaxf(a5[j], v); v = fminf(a5[j], v); a5[j] = hi; }
             }
-            L0 = a5[4];
-        }
-        // L' = floor(L0 - eps) - 1, candidates: a_c >= L' - eps; every step rounded towards -inf
-        const float thr = __fsub_rd(__fsub_rd(floorf(__fsub_rd(L0, ee)), 1.0f), ee);
-        // no block barrier here: any thread that saw the mbarrier flip knows the GEMM is complete, so the X tile is dead for
-        // everybody; lists and staging slab are thread-private
-        int n = 0;
-        float worst = 0.f;
-        auto collect = [&](int c0, const float (&v)[32]) {
-            unsigned h4[4] = {0u, 0u, 0u, 0u};            // branch-free: one compare and one predicated OR per column, four chains
-#pragma unroll
-            for (int i = 0; i < 32; ++i) h4[i & 3] |= v[i] >= thr ? (1u << i) : 0u;
-            const unsigned hit_all = (h4[0] | h4[1]) | (h4[2] | h4[3]);
-            if (__any_sync(0xffffffffu, hit_all != 0u)) {    // registers cannot be indexed by a run-time column: through shared memory
-#pragma unroll
-                for (int part = 0; part < SPLIT; ++part) {
-#pragma unroll
-                    for (int i = 0; i < SD; ++i) stage[i * NT_ + tid] = v[part * SD + i];
-                    unsigned hit = (hit_all >> (part * SD)) & (SD == 32 ? 0xffffffffu : ((1u << SD) - 1u));
-                    while (hit) {
-                        const int i = __ffs(hit) - 1;
-                        hit &= hit - 1;
-                        if (n < CAPH) {
-                            Lv[n * NT_ + tid] = stage[i * NT_ + tid];
-                            Lc[n * NT_ + tid] = (unsigned char)(half * NDH + c0 + part * SD + i);
-                        }
-                        ++n;
-                    }
-                }
-            }
-            if (CHECK && valid) {
-                for (int i = 0; i < 32; ++i) {
-                    const float *rp = rc + (size_t)(half * NDH + c0 + i) * RF;
-                    float d = rp[0];
-                    for (int j = 0; j < FL; ++j) {
-                        const float df = __fsub_rn(x[j], rp[1 + 2 * j]);
-                        d = __fsub_rn(d, __fmul_rn(__fmul_rn(df, df), rp[2 + 2 * j]));
-                    }
-                    worst = fmaxf(worst, __fdividef(fabsf(v[i] - d), ee));
-                }
-            }
+            return a5[4];
         };
-        {
-            float va[32], vb[32];
-            tmem_ld32_issue(trow, va);
-#pragma unroll 1
-            for (int c0 = 0; c0 < NDH; c0 += 64) {
-                tmem_wait_ld_dep(va);
-                tmem_ld32_issue(trow + c0 + 32, vb);
-                collect(c0, va);
-                tmem_wait_ld_dep(vb);
-                if (c0 + 64 < NDH) tmem_ld32_issue(trow + c0 + 64, va);
-                collect(c0 + 32, vb);
+        const float e_a = epsr[ra], e_b = epsr[rb];
+        // L' = floor(L0 - eps) - 1, candidates: a_c >= L' - eps; every step rounded towards -inf
+        const float thra = __fsub_rd(__fsub_rd(floorf(__fsub_rd(fifth(gma), e_a)), 1.0f), e_a);
+        const float thrb = __fsub_rd(__fsub_rd(floorf(__fsub_rd(fifth(gmb), e_b)), 1.0f), e_b);
+        const float thr_min = fminf(thra, thrb);
+#pragma unroll
+        for (int i = 0; i < NTL; ++i) {
+            if (fmaxf(fmaxf(acc[4 * i], acc[4 * i + 1]), fmaxf(acc[4 * i + 2], acc[4 * i + 3])) < thr_min) continue;
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const float a = acc[4 * i + e];
+                const int rr = (e & 2) ? rb : ra;
+                if (a >= ((e & 2) ? thrb : thra)) {
+                    const int slot = atomicAdd(&cnt[rr], 1);
+                    if (slot < TC_CAP) {
+                        Lv[slot * WG_ROWS + rr] = a;
+                        Lc[slot * WG_ROWS + rr] = (unsigned char)(8 * i + 2 * q4 + (e & 1));
+                    }
+                }
             }
         }
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        // SPLIT = 2: thread 0 of the pair takes over with both sub-lists (own slots, then the partner's)
-        int n0 = n, n1 = 0;
-        if (SPLIT == 2) {
-            cnt_s[half * TC_ROWS + r] = n;
-            __syncthreads();
-            n0 = cnt_s[r]; n1 = cnt_s[TC_ROWS + r];
-        }
-        const bool listed = n0 <= CAPH && n1 <= CAPH && n0 + n1 >= 5 && n0 + n1 <= 20;
-        n = n0 + n1;
-        auto cand_v = [&](int i) { return i < n0 ? Lv[i * NT_ + r] : Lv[(i - n0) * NT_ + TC_ROWS + r]; };
-        auto cand_c = [&](int i) { return (int)(i < n0 ? Lc[i * NT_ + r] : Lc[(i - n0) * NT_ + TC_ROWS + r]); };
         if (CHECK) {
-            atomicMax(reinterpret_cast<int *>(check), __float_as_int(worst));
-            if (valid && half == 0) atomicMax(reinterpret_cast<int *>(check) + 1, n);
+            // exact distances of every column this lane holds (debug only): |a - d| / eps
+            float worst = 0.f;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int rr = h ? rb : ra;
+                if (row0 + rr >= total) continue;
+                const float *px = feats + (row0 + rr) * D + featoff[f];
+                const float er = epsr[rr];
+#pragma unroll
+                for (int i = 0; i < NTL; ++i)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const float *rp = rc + (size_t)(8 * i + 2 * q4 + e) * RF;
+                        float d = rp[0];
+                        for (int j = 0; j < FL; ++j) {
+                            const float df = __fsub_rn(px[j], rp[1 + 2 * j]);
+                            d = __fsub_rn(d, __fmul_rn(__fmul_rn(df, df), rp[2 + 2 * j]));
+                        }
+                        worst = fmaxf(worst, __fdividef(fabsf(acc[4 * i + 2 * h + e] - d), er));
+                    }
+            }
+            atomicMax(reinterpret_cast<int *>(check), __float_as_int(worst));     // non-negative floats order like ints
         }
+        warpgroup_bar(1 + wg);                           // every row's list is complete
 
         // ---- the record straight from the filter values when they leave no doubt ----
         if (valid && half == 0) {
+            const int n = cnt[r];
+            const bool listed = n >= 5 && n <= TC_CAP;
+            auto cand_v = [&](int i) { return Lv[i * WG_ROWS + r]; };
+            auto cand_c = [&](int i) { return (int)Lc[i * WG_ROWS + r]; };
+            if (CHECK) atomicMax(reinterpret_cast<int *>(check) + 1, n);
             bool certain = listed;
             if (certain) {
                 float a[5] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY, -INFINITY};
@@ -803,15 +717,11 @@ ptm_tc5_kernel(const float *__restrict__ feats, long long total, int D, const in
                 if (CHECK) { atomicAdd(stats, 1ull); atomicAdd(stats + 2, (unsigned long long)n_exact); if (!distinct) atomicAdd(stats + 3, 1ull); }
             }
         }
-        __syncthreads();                                  // lists consumed, accumulator read: the next tile may overwrite both
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+        warpgroup_bar(1 + wg);                           // lists consumed: the next tile may overwrite X, lists and counts
     }
-    __syncthreads();
-    if (warp == 0)
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_d), "n"(ND < 32 ? 32 : ND));
 }
 
-// Rows the filter values left in doubt (work list of ptm_tc5_kernel): one thread per row, the reference's exact
+// Rows the filter values left in doubt (work list of ptm_wgmma_kernel): one thread per row, the reference's exact
 // arithmetic for its candidate codewords (all codewords when its list had overflowed), the five best, the record;
 // exact ties go on to the fix-up.  Item: {row low, pair | n << 16, 18 codeword bytes, row high}.
 template <int FL>
@@ -935,8 +845,8 @@ ptm_fixup_kernel(const float *__restrict__ feats, int D, const int32_t *__restri
 // chain in order.  All distances of a frame in parallel, the four seeds fetched by shuffle, then the scan only visits --
 // in ascending codeword order -- the codewords whose distance reaches the seeds' worst score (ballots), each re-tested
 // against the list as it stands: eval_topn + eval_cb literally, like semi_scan_kernel does for semi-continuous models.
-// The thread-per-chain kernel above serialises 260 distances per flagged frame inside one lane (15 ms per 10^6 frames
-// at a 0.04 % tie rate); this one costs a few hundred warp instructions per flagged frame.
+// The thread-per-chain kernel above serialises 260 distances per flagged frame inside one lane; this one costs a few
+// hundred warp instructions per flagged frame.
 template <int FL, int NDW>
 __global__ void __launch_bounds__(128)
 ptm_fixup_warp_kernel(const float *__restrict__ feats, int D, const int32_t *__restrict__ featoff, const int32_t *__restrict__ utt_off,
@@ -1076,31 +986,35 @@ int launch_tc(psb_batch_t *b, const float *d_feats, long long total, const int32
     return PSB_OK;
 }
 
-template <int FL, int ND, int SPLIT>
-int launch_tc5(psb_batch_t *b, const float *d_feats, long long total, const int32_t *d_klist, int n_k, const int32_t *d_featoff,
+template <int FL, int ND>
+int launch_wgmma(psb_batch_t *b, const float *d_feats, long long total, const int32_t *d_klist, int n_k, const int32_t *d_featoff,
                bool check)
 {
     psb_model_t *m = b->m;
-    const size_t smem = (size_t)2 * 8 * ND * 16 + (size_t)2 * 8 * TC_ROWS * 16;
+    const size_t smem = (size_t)2 * 8 * ND * 16 + 2 * ((size_t)2 * 8 * WG_ROWS * 16 + WG_EXTRA);
     const long long tiles = (total + TC_ROWS - 1) / TC_ROWS;
-    // W (64 KB at 256 densities) is staged once per CTA: a few tiles per CTA, but still >= 4 waves of 2 CTAs per SM
+    const int n_sm = psb_sm_count(m->device);
+    int per_sm = 1;                                      // sm_90: 147-255 registers x 256 threads, one CTA per SM
+    PSB_CUDA(cudaFuncSetAttribute(ptm_wgmma_kernel<FL, ND, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    PSB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ptm_wgmma_kernel<FL, ND, false>, TC_ROWS * 2, smem));
+    // W (64 KB at 256 densities) is staged once per CTA: a few tiles per CTA, but still >= 4 waves of the resident CTAs
     int tpc = 1;
-    while (tpc < 8 && (tiles / (tpc * 2)) * n_k >= 148LL * 2 * 4) tpc *= 2;
+    while (tpc < 8 && (tiles / (tpc * 2)) * n_k >= (long long)n_sm * std::max(per_sm, 1) * 4) tpc *= 2;
     PSB_REQUIRE((tiles + tpc - 1) / tpc <= 65535, "too many frames for one launch of the tensor-core filter");
     const dim3 grid((unsigned)n_k, (unsigned)((tiles + tpc - 1) / tpc));
     float *chk = b->d_tc_check;
     unsigned long long *stats = reinterpret_cast<unsigned long long *>(b->d_tc_check + 4);
     if (check) {
-        auto kern = ptm_tc5_kernel<FL, ND, SPLIT, true>;
+        auto kern = ptm_wgmma_kernel<FL, ND, true>;
         PSB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        kern<<<grid, TC_ROWS * SPLIT, smem, b->stream>>>(d_feats, total, m->sumlen, d_featoff, d_klist, m->d_tc_wumma, m->d_tc_cen, m->d_tc_bnd,
+        kern<<<grid, TC_ROWS * 2, smem, b->stream>>>(d_feats, total, m->sumlen, d_featoff, d_klist, m->d_tc_wumma, m->d_tc_cen, m->d_tc_bnd,
                                                 m->d_rec, m->d_rec_off, b->d_topn, b->d_tc_flags, (long long)b->tc_flag_words, m->K,
                                                 m->n_feat, tpc, b->d_tc_items, b->d_tc_nitems, b->tc_item_cap, chk, stats);
     }
     else {
-        auto kern = ptm_tc5_kernel<FL, ND, SPLIT, false>;
+        auto kern = ptm_wgmma_kernel<FL, ND, false>;
         PSB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        kern<<<grid, TC_ROWS * SPLIT, smem, b->stream>>>(d_feats, total, m->sumlen, d_featoff, d_klist, m->d_tc_wumma, m->d_tc_cen, m->d_tc_bnd,
+        kern<<<grid, TC_ROWS * 2, smem, b->stream>>>(d_feats, total, m->sumlen, d_featoff, d_klist, m->d_tc_wumma, m->d_tc_cen, m->d_tc_bnd,
                                                 m->d_rec, m->d_rec_off, b->d_topn, b->d_tc_flags, (long long)b->tc_flag_words, m->K,
                                                 m->n_feat, tpc, b->d_tc_items, b->d_tc_nitems, b->tc_item_cap, nullptr, nullptr);
     }
@@ -1108,7 +1022,7 @@ int launch_tc5(psb_batch_t *b, const float *d_feats, long long total, const int3
     if (b->d_tc_items) {
         // the rows in doubt: the count lives on the device, so the grid covers the list's capacity (grid-stride loop, idle
         // blocks leave at once)
-        const unsigned blocks = (unsigned)std::min<size_t>(((size_t)b->tc_item_cap + 127) / 128, 148 * 64);
+        const unsigned blocks = (unsigned)std::min<size_t>(((size_t)b->tc_item_cap + 127) / 128, (size_t)n_sm * 64);
         ptm_tc_exact_kernel<FL><<<blocks, 128, 0, b->stream>>>(d_feats, m->sumlen, d_featoff, b->d_tc_items, b->d_tc_nitems, b->tc_item_cap,
                                                               m->d_rec, m->d_rec_off, b->d_topn, b->d_tc_flags, (long long)b->tc_flag_words,
                                                               m->K, m->n_feat, ND, check ? stats : nullptr);
@@ -1130,7 +1044,7 @@ int psb_tc_prepare(psb_model_t *m, const float *hm, const float *hv, const float
         if (m->featlen[f] != 13) return PSB_OK;              // the kernels are instantiated for 13-dimensional streams
     const int nd = m->n_density, NT = nd / 8, FL = 13, K = m->K;
     std::vector<float> wf((size_t)K * 2 * NT * 4 * 32 * 2, 0.f), cen((size_t)K * 16, 0.f), bnd((size_t)K * 32, 0.f);
-    std::vector<float> wu((size_t)K * 2 * 8 * nd * 4, 0.f);     // canonical K-major layout of the tcgen05 path: [half][chunk][n][4]
+    std::vector<float> wu((size_t)K * 2 * 8 * nd * 4, 0.f);     // canonical K-major layout of the wgmma path: [half][chunk][n][4]
     std::vector<double> W((size_t)TC_K * nd);
     for (int cb = 0; cb < m->n_mgau; ++cb)
         for (int f = 0; f < m->n_feat; ++f) {
@@ -1243,7 +1157,7 @@ int psb_launch_ptm_tc(psb_batch_t *b, const float *d_feats, const int32_t *utt_o
     PSB_CUDA(cudaMemsetAsync(b->d_tc_flags, 0, fw * m->K * 4, b->stream));
     PSB_CUDA(cudaMemcpyAsync(b->d_uttoff, utt_off, ((size_t)n_utt + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, b->stream));
     static const bool check = [] { const char *v = getenv("PSB_TC_CHECK"); return v && atoi(v) != 0; }();
-    static const bool legacy_mma = [] { const char *v = getenv("PSB_TC_IMPL"); return v && !strcmp(v, "mma"); }();   // default: tcgen05
+    static const bool legacy_mma = [] { const char *v = getenv("PSB_TC_IMPL"); return v && !strcmp(v, "mma"); }();   // default: wgmma
     int rc;
     if (legacy_mma)
         switch (m->n_density) {
@@ -1252,16 +1166,11 @@ int psb_launch_ptm_tc(psb_batch_t *b, const float *d_feats, const int32_t *utt_o
         default: rc = launch_tc<13, 8>(b, d_feats, total, d_klist, m->K, d_featoff, check); break;
         }
     else
-    {
-        static const bool one_thread = [] { const char *v = getenv("PSB_TC_SPLIT"); return !(v && atoi(v) == 2); }();   // two threads per frame measured slower (DESIGN 4.15): 37.2 vs 30.7 ms
         switch (m->n_density) {
-        case 256: rc = one_thread ? launch_tc5<13, 256, 1>(b, d_feats, total, d_klist, m->K, d_featoff, check)
-                                  : launch_tc5<13, 256, 2>(b, d_feats, total, d_klist, m->K, d_featoff, check); break;
-        case 128: rc = one_thread ? launch_tc5<13, 128, 1>(b, d_feats, total, d_klist, m->K, d_featoff, check)
-                                  : launch_tc5<13, 128, 2>(b, d_feats, total, d_klist, m->K, d_featoff, check); break;
-        default: rc = launch_tc5<13, 64, 1>(b, d_feats, total, d_klist, m->K, d_featoff, check); break;
+        case 256: rc = launch_wgmma<13, 256>(b, d_feats, total, d_klist, m->K, d_featoff, check); break;
+        case 128: rc = launch_wgmma<13, 128>(b, d_feats, total, d_klist, m->K, d_featoff, check); break;
+        default: rc = launch_wgmma<13, 64>(b, d_feats, total, d_klist, m->K, d_featoff, check); break;
         }
-    }
     if (rc) return rc;
     const long long chains = (long long)n_utt * m->K;
     static const bool thread_fixup = [] { const char *v = getenv("PSB_TC_FIXUP"); return v && !strcmp(v, "thread"); }();

@@ -112,7 +112,7 @@ static bool search_warp_mode()
 }
 
 // Grow-only device workspace kept in the context: repeated calls (one per batch) do not pay
-// cudaMalloc / cudaFree again (the alignment entry point lost 220 ms per call that way, DESIGN 4.7).
+// cudaMalloc / cudaFree again (DESIGN 4.7).
 template <class T>
 static cudaError_t srch_reserve(psb_hmmctx_t *c, int slot, size_t count, T **out)
 {

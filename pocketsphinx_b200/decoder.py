@@ -4,7 +4,7 @@ loop -> first pass -> second pass on the GPU, hypothesis and segments read from 
 (ps_decode_raw + ps_get_hyp / ps_seg_iter with -bestpath no, pocketsphinx.c:1073-1345).  Everything the
 reference loads from files is read here by the package itself (s3io, lmio, dict2pid, lextree).
 
-STATUS: GPU-verified end to end (tests/test_gpu_zz_decoder.py, first hardware run in round 2).  Out of the
+STATUS: GPU-verified end to end (tests/test_gpu_zz_decoder.py).  Out of the
 hot-path scope (SURVEY 8): kept small, not extended.
 """
 import math

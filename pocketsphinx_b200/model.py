@@ -115,8 +115,30 @@ class PackedModel:
 
     @classmethod
     def load(cls, path):
-        with np.load(path, allow_pickle=False) as z:
-            return cls.from_dict({k: z[k] for k in z.files})
+        return cls.from_dict(load_npz(path))
+
+
+class NpzArrays(dict):
+    """The arrays of an .npz file by name; `.files` lists the names like np.load's result."""
+
+    @property
+    def files(self):
+        return list(self)
+
+
+def load_npz(path):
+    """All arrays of `path`.  A large file is stored in parts (name.npz, name.part1.npz, ...) so that each part stays
+    under 1 MB: an array found in several parts is their concatenation along axis 0, in part order."""
+    import glob
+    import re
+    stem = path[:-len(".npz")]
+    parts = sorted(glob.glob(glob.escape(stem) + ".part*.npz"), key=lambda p: int(re.search(r"\.part(\d+)\.npz$", p).group(1)))
+    out = NpzArrays()
+    for p in [path] + parts:
+        with np.load(p, allow_pickle=False) as z:
+            for k in z.files:
+                out[k] = np.concatenate([out[k], z[k]]) if k in out else z[k]
+    return out
 
 
 def make_logadd8(base=1.0001, shift=10):

@@ -12,11 +12,12 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on a B200)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run with -m gpu on an H100)")
 
 
 def golden(name):
-    return np.load(os.path.join(GOLDEN, name), allow_pickle=False)
+    from pocketsphinx_b200.model import load_npz
+    return load_npz(os.path.join(GOLDEN, name))
 
 
 @pytest.fixture(scope="session")

@@ -54,10 +54,10 @@ def test_no_fused_multiply_add_in_distance_kernels():
     for line in sass.splitlines():
         if "Function :" in line:
             fn = line.split("Function :")[1].strip()
-        elif fn and any(k in fn for k in ("topn", "ms_dist", "semi_dist", "ptm_tc", "ptm_fixup")) and "FFMA" in line:
+        elif fn and any(k in fn for k in ("topn", "ms_dist", "semi_dist", "ptm_tc", "ptm_wgmma", "ptm_fixup")) and "FFMA" in line:
             bad.append((fn[:60], line.strip()[:80]))
     assert not bad, bad[:5]
-    assert "FMUL2" in sass and "FADD2" in sass, "packed FP32 path missing from the build"
+    assert "HGMMA" in sass, "warpgroup tensor-core filter missing from the build"
 
 
 def test_header_is_plain_c_and_the_example_compiles(tmp_path):

@@ -1,26 +1,16 @@
 """CPU: the numpy restatement of the front end (oracle/fe_port.py, structured like psb_fe.cu)
 against the compiled reference on real and synthetic PCM -- bit-exact (same libm)."""
-import os
-
 import numpy as np
 import pytest
 
-from oracle import fe_port, refdrv
-
-pytestmark = pytest.mark.skipif(not refdrv.available(), reason="oracle/_ref/libpsref.so not built")
-REF = os.path.dirname(refdrv.LIB_PATH)
-EN_US = os.path.join(REF, "model", "en-us")
+from oracle import fe_golden, fe_port
 
 
-@pytest.mark.parametrize("kv", [dict(), dict(transform="legacy", remove_noise="no", lifter="0"),
-                                dict(transform="htk", remove_dc="yes"), dict(cmn="none")])
+@pytest.mark.parametrize("kv", fe_golden.PORT_CONFIGS)
 def test_fe_port_matches_reference(kv):
-    ref = refdrv.RefModel(EN_US, **kv)
+    ref = fe_golden.Recorded(**kv)
     d = ref.fe_desc()
-    go = np.fromfile(os.path.join(REF, "data", "goforward.raw"), np.int16)
-    rng = np.random.default_rng(3)
-    noise = np.clip(rng.normal(0, 3000, 5000), -32768, 32767).astype(np.int16)
-    for pcm in (go[:6000], go[20000:23000], noise, go[:411], go[:100], np.zeros(1500, np.int16)):
+    for pcm in fe_golden.port_inputs(fe_golden.goforward()):
         want_c = ref.mfcc(pcm)
         got_c = fe_port.cepstra(d, fe_port.mfspec(d, pcm))
         assert got_c.shape == want_c.shape

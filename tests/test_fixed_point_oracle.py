@@ -12,7 +12,7 @@ import pytest
 
 from oracle import refdrv
 
-from conftest import fx_case
+from conftest import fx_case, golden
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
@@ -83,5 +83,5 @@ def test_fixed_point_ptm_oracle_matches_fixed_point_reference(tmp_path):
         np.argwhere((topn != fx["topn"]).reshape(len(topn), -1).any(1))[0, 0])
     assert np.array_equal(got, fx["senscr"])
     # and the two builds really differ (otherwise this test would prove nothing)
-    flt = np.load(os.path.join(HERE, "golden", "en_us_goforward.npz"))["senscr"]
+    flt = golden("en_us_goforward.npz")["senscr"]
     assert (got != flt).mean() > 0.2

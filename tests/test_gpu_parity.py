@@ -417,13 +417,13 @@ print(json.dumps(out))
 """
 
 
-@pytest.mark.parametrize("impl", ["tcgen05", "mma"])
+@pytest.mark.parametrize("impl", ["wgmma", "mma"])
 def test_tensor_core_filter_error_bound_holds_on_the_device(impl):
     """PSB_TC_CHECK=1: the filter kernel compares every 3 x TF32 GEMM value it produced with the exact float
     distance and reports the worst |a - d| / eps (the bound the candidate selection relies on must hold
     with room to spare: the analysis in psb_ptm_tc.cu allows 0.8 of eps), on the shipped model with real
     features, the BASELINE shape, features scaled far outside the model's range and tie-stress data; for the
-    tcgen05 / tensor-memory kernel (the default) and for the legacy mma.sync variant (PSB_TC_IMPL=mma)."""
+    warpgroup-MMA kernel (wgmma, the default) and for the legacy mma.sync variant (PSB_TC_IMPL=mma)."""
     import json
     import os
     import subprocess

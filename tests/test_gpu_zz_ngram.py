@@ -1,8 +1,7 @@
 """GPU (-m gpu): psb_ngram_fwdtree_batch_device (the first pass of the n-gram search on the device)
 against the reference's golden backpointer tables and against the oracle on ragged batches.
 
-First hardware run: round 2, first GPU call (profiles/r02_first_hw_run/): all cases green in both
-bindings of the phase code, compute-sanitizer memcheck + racecheck clean.  The phase code is also
+PSB_SEARCH_WARP=1 runs the same cases on the warp binding of the phase code.  The phase code is also
 checked on the host against the reference (tests/test_ngs_emul.py, tests/test_ngf_emul.py)."""
 
 import os

@@ -19,10 +19,10 @@ sys.path.insert(0, ROOT)
 
 def main():
     from pocketsphinx_b200 import _lib, api
-    from pocketsphinx_b200.model import PackedModel
+    from pocketsphinx_b200.model import PackedModel, load_npz
     gd = os.path.join(ROOT, "tests", "golden")
     pm = PackedModel.load(os.path.join(gd, "en_us_ptm_model.npz"))
-    g = np.load(os.path.join(gd, "en_us_goforward.npz"))
+    g = load_npz(os.path.join(gd, "en_us_goforward.npz"))
     feats = g["feats"]
     out = {"model": "en-us PTM 42x3x128x13, 5126 senones", "frames": int(len(feats))}
     m = api.Model(pm)

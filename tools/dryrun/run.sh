@@ -11,6 +11,7 @@ python -c "from oracle import oracle; oracle.build()" 2>/dev/null || (cd "$ROOT"
 for h in fsg ngs ngf; do
     g++ -O1 -fPIC -shared -ffp-contract=off -o /tmp/lib${h}emul.so "$ROOT/tests/emul/${h}_emul.cpp" -L"$ROOT/oracle/_build" -lpsoracle -Wl,-rpath,"$ROOT/oracle/_build"
 done
+export PSB_ROOT="$ROOT"
 cp "$ROOT/tools/dryrun/conftest_dry.py" "$D/conftest.py"
 for f in test_gpu_zz_fsg.py test_gpu_zz_ngram.py; do
     python - "$ROOT/tests/$f" "$D/$f" <<'P'

@@ -9,7 +9,7 @@ import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from oracle import oracle  # noqa: E402
-from pocketsphinx_b200.model import PackedModel, quantize_for_ties, synth_feats, synth_ptm  # noqa: E402
+from pocketsphinx_b200.model import PackedModel, load_npz, quantize_for_ties, synth_feats, synth_ptm  # noqa: E402
 
 L = oracle.lib()
 L.pso_filter_experiment.restype = C.c_int32
@@ -35,7 +35,7 @@ fq = gen(6, 200, s=9)
 for lag in (1, 3, 10):
     tot = sum(run(pmq, fq[u], lag) for u in range(6))
     print("tie stress, lag", lag, "lists", tot[0], "differ", tot[1], "scanned %.3f" % (tot[3] / tot[4]), flush=True)
-g = np.load(os.path.join(os.path.dirname(__file__), "..", "tests", "golden", "en_us_goforward.npz"))
+g = load_npz(os.path.join(os.path.dirname(__file__), "..", "tests", "golden", "en_us_goforward.npz"))
 en = PackedModel.load(os.path.join(os.path.dirname(__file__), "..", "tests", "golden", "en_us_ptm_model.npz"))
 for lag in (1, 5, 30):
     st = run(en, g["feats"], lag)
