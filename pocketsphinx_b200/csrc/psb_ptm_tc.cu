@@ -21,23 +21,21 @@
 //  (2) The five best can be found without computing 256 exact distances.  With y = x - m (m = the
 //      codebook's mean centre) the exponent d = det - sum_j v_j (y_j - mu'_j)^2 is the inner product
 //      of X = (y_j^2, y_j, 1) with W_c = (-v_cj, 2 v_cj mu'_cj, det_c - sum_j v_cj mu'_cj^2): one
-//      [frames x 32] x [32 x n_density] TF32 GEMM per pair on the tensor cores (mma.sync m16n8k8;
-//      the operands are rounded to TF32 once, on the host for W).  Its result a_c differs from the
+//      [frames x 32] x [32 x n_density] GEMM per pair on the tensor cores, as 3 x TF32 (lo*hi + hi*lo
+//      + hi*hi; W is split into TF32 halves on the host): warpgroup MMA (ptm_wgmma_kernel, the
+//      default) or mma.sync m16n8k8 (ptm_tc_kernel, PSB_TC_IMPL=mma).  Its result a_c differs from the
 //      reference's float d_c by at most eps = ERR * (sum_j Amax_j y_j^2 + Bmax_j |y_j| + Cmax), a
 //      bound every row computes for itself (Amax/Bmax/Cmax: per-pair maxima of |W| entries).  Five
-//      distinct codewords with a_c >= L0 (the four per-lane row maxima of the accumulator fragment
-//      and the best of the four runner-up half maxima) give the integer L' = floor(L0 - eps) - 1
-//      <= s(5) - 1, and every codeword with s_c >= s(5) has d_c > L', hence a_c >= L' - eps: the
-//      candidate set C (about a dozen of 256 on the BASELINE shape).  Among them, with a(4) the
-//      fourth largest a_c, only E = {c : a_c >= a(4) - 2 eps - 1} can reach the four best or tie with
-//      them (anything else has d_c < d(4) - 1, i.e. a strictly smaller integer score): E (five to
-//      seven codewords) is what gets the reference's exact float arithmetic.
+//      distinct codewords with a_c >= L0 (wgmma: the fifth largest of eight group maxima of the row;
+//      mma.sync: the four per-lane row maxima and the best runner-up half maximum) give the integer
+//      L' = floor(L0 - eps) - 1 <= s(5) - 1, and every codeword with s_c >= s(5) has d_c > L', hence
+//      a_c >= L' - eps: the candidate set C (about seven of 256 on the BASELINE shape).
 //
-// The exact stage keeps the warp-uniform record stream of the old kernels: lane = frame (32
-// consecutive frames of the batch per warp), the warp walks the UNION of its lanes' E sets pair by
-// pair with the codeword-pair distance (gau_dist2) and each lane keeps the five best of its
-// own set.  A row whose candidate list overflows its shared-memory slots falls back to E = C; a warp
-// whose rows agree on nothing degrades towards the dense scan, never below it.
+// A row is then decided from the filter values alone when its five largest a_c are more than 2 eps + 1
+// apart and the `>> 10` of the four best is the same at both ends of [a - eps, a + eps]: the record
+// is certain without one exact distance.  Otherwise the row's candidate codewords (all of them when
+// C has more than TC_CAP members) get the reference's exact float arithmetic, one thread per row:
+// in ptm_wgmma_kernel's work list served by ptm_tc_exact_kernel, in ptm_tc_kernel itself.
 //
 // Nothing here is approximate in its output: tests/test_gpu_parity.py compares every record with the
 // oracle's lists, PSB_TC_CHECK=1 makes the filter kernel measure max |a_c - d_c| / eps on the device.
@@ -372,11 +370,15 @@ ptm_tc_kernel(const float *__restrict__ feats, long long total, int D, const int
 // The same filter on Hopper's warpgroup MMA: each warpgroup issues twelve wgmma.mma_async m64nNDk8 TF32 (lo*hi, hi*lo,
 // hi*hi over four K steps) per 64 frames, A (X rows split into TF32 halves) and B (W, both halves) straight from shared
 // memory in the canonical K-major no-swizzle layout, the fp32 accumulator in registers.  A frame's row is spread over the
-// four lanes of a quad: group maxima meet by shuffles, candidates go to the row's shared-memory list, one thread per row
-// resolves it.  The two warpgroups of a CTA share W and run their 64-frame halves independently (named barriers), so the
-// GEMM of one overlaps the selection of the other; a CTA walks `tiles_per_cta` consecutive tiles of its pair.
+// four lanes of a quad: group maxima meet by shuffles; each lane then stores, without a branch or an atomic, the column
+// pairs of its rows whose larger value passes the threshold (predicated stores to its own slots, one mask bit per pair),
+// and two threads per row -- all four warps -- pick the five largest candidates and decide the row.  The two warpgroups of
+// a CTA share W and run their 64-frame halves independently (named barriers), so the GEMM of one overlaps the selection
+// of the other, and each issues its next tile's GEMM before it resolves the rows of the current one; a CTA walks
+// `tiles_per_cta` consecutive tiles of its pair.
 constexpr int WG_ROWS = 64;                                                   // frames per warpgroup and tile
-constexpr int WG_EXTRA = TC_CAP * WG_ROWS * 4 + WG_ROWS * 4 + WG_ROWS * 4 + TC_CAP * WG_ROWS;   // lists, counts, bounds
+constexpr int WG_SLOTS = (TC_CAP + 1) * WG_ROWS * 4;                         // candidate pairs: [slot][row][quad lane], slot TC_CAP absorbs overflow
+constexpr int WG_EXTRA = WG_SLOTS * 8 + WG_ROWS * 4 * 4 + WG_ROWS * 4 + 2 * WG_ROWS * 4 + WG_ROWS * 20;   // pairs, masks, thresholds, bounds, codewords
 
 __device__ __forceinline__ uint64_t wgmma_desc(const void *p, unsigned lbo_bytes, unsigned sbo_bytes)
 {
@@ -461,10 +463,11 @@ ptm_wgmma_kernel(const float *__restrict__ feats, long long total, int D, const 
     float *sW = reinterpret_cast<float *>(wg_smem);                                   // [2][8][ND][4]
     float *sX = sW + 2 * 8 * ND * 4 + wg * (2 * 8 * WG_ROWS * 4);                     // this warpgroup's [2][8][64][4]
     unsigned char *ex = wg_smem + (size_t)2 * 8 * ND * 16 + 2 * (2 * 8 * WG_ROWS * 16) + (size_t)wg * WG_EXTRA;
-    float *Lv = reinterpret_cast<float *>(ex);                                        // [TC_CAP][64] candidate values
-    int *cnt = reinterpret_cast<int *>(Lv + TC_CAP * WG_ROWS);                        // [64] candidates per row
-    float *epsr = reinterpret_cast<float *>(cnt + WG_ROWS);                           // [64] error bound per row
-    unsigned char *Lc = reinterpret_cast<unsigned char *>(epsr + WG_ROWS);            // [TC_CAP][64] candidate columns
+    float2 *Pv = reinterpret_cast<float2 *>(ex);                                      // [TC_CAP + 1][64][4] candidate column pairs
+    unsigned *Pm = reinterpret_cast<unsigned *>(Pv + WG_SLOTS);                       // [64][4] n-tiles of the stored pairs
+    float *thrs = reinterpret_cast<float *>(Pm + WG_ROWS * 4);                        // [64] candidate threshold per row
+    float *epsr = thrs + WG_ROWS;                                                     // [2][64] error bound per row (two tiles)
+    unsigned *Lc = reinterpret_cast<unsigned *>(epsr + 2 * WG_ROWS);                  // [64][5] candidate codewords (bytes)
 
     // grid: x = pair (fastest), y = group of tiles: CTAs that run together read the SAME frames for different pairs, so
     // the feature rows come out of L2 while the W blocks of all pairs stay L2-resident
@@ -478,59 +481,51 @@ ptm_wgmma_kernel(const float *__restrict__ feats, long long total, int D, const 
     __syncthreads();
     const float *m = cen + (size_t)k * 16, *bb = bnd + (size_t)k * 32;
     const float *rc = rec + rec_off[k];
-    const int r = t & (WG_ROWS - 1), half = t >> 6;     // the frame this thread prepares (and resolves if half == 0)
+    const int r = t & (WG_ROWS - 1), half = t >> 6;     // the frame whose X row this thread prepares (half of its chunks)
     const int g = lane >> 2, q4 = lane & 3;
     const int ra = warp * 16 + g, rb = ra + 8;           // the two accumulator rows this thread holds columns of
 
-    // the next tile's feature row is fetched while this tile's GEMM runs
-    float xn[FL];
-    {
-        const long long r0 = (long long)blockIdx.y * tiles_per_cta * TC_ROWS + wg * WG_ROWS + r;
-        const float *p = feats + (r0 < total ? r0 : 0) * D + featoff[f];
+    // ---- a tile's frames: X rows (TF32 halves, canonical layout; two threads share the stores of a row) and error bounds ----
+    float xn[FL];                                        // the feature row of the frame this thread prepares next
+    auto fetch = [&](long long row) {
+        const float *p = feats + (row < total ? row : 0) * D + featoff[f];
 #pragma unroll
-        for (int j = 0; j < FL; ++j) xn[j] = r0 < total ? p[j] : 0.f;
-    }
-    for (int tile = 0; tile < tiles_per_cta; ++tile) {
-        const long long row0 = ((long long)blockIdx.y * tiles_per_cta + tile) * TC_ROWS + wg * WG_ROWS;
-        if (row0 >= total) break;                        // uniform in the warpgroup: its rows lie past the end
-        const long long row = row0 + r;
-        const bool valid = row < total;
-        // ---- this thread's frame: X row (TF32 halves, canonical layout; two threads share the stores) and its error bound ----
-        float x[FL], ee;
-        {
-            float v[TC_K];
-            float S = bb[2 * FL];
+        for (int j = 0; j < FL; ++j) xn[j] = row < total ? p[j] : 0.f;
+    };
+    auto prepare = [&](float *eps) {
+        float v[TC_K];
+        float S = bb[2 * FL];
 #pragma unroll
-            for (int j = 0; j < FL; ++j) {
-                x[j] = xn[j];
-                const float y = __fsub_rn(x[j], m[j]);
-                const float y2 = __fmul_rn(y, y);
-                v[j] = y2;
-                v[FL + j] = y;
-                S = __fadd_ru(S, __fmul_ru(bb[j], y2));               // no FMA anywhere in these kernels: tests/test_abi.py greps for it
+        for (int j = 0; j < FL; ++j) {
+            const float y = __fsub_rn(xn[j], m[j]);
+            const float y2 = __fmul_rn(y, y);
+            v[j] = y2;
+            v[FL + j] = y;
+            if (half == 0) {                                      // the thread that stores the bound (warp-uniform)
+                S = __fadd_ru(S, __fmul_ru(bb[j], y2));           // no FMA anywhere in these kernels: tests/test_abi.py greps for it
                 S = __fadd_ru(S, __fmul_ru(bb[FL + j], fabsf(y)));
             }
-            v[2 * FL] = 1.0f;
-#pragma unroll
-            for (int j = 2 * FL + 1; j < TC_K; ++j) v[j] = 0.f;
-            ee = __fadd_ru(__fmul_ru(S, TC_ERR), 2.0f);
-#pragma unroll
-            for (int kc = 0; kc < 8; ++kc) {
-                if ((kc & 1) != half) continue;
-                float4 h, l;
-                h.x = to_tf32(v[4 * kc]); h.y = to_tf32(v[4 * kc + 1]); h.z = to_tf32(v[4 * kc + 2]); h.w = to_tf32(v[4 * kc + 3]);
-                l.x = to_tf32(__fsub_rn(v[4 * kc], h.x)); l.y = to_tf32(__fsub_rn(v[4 * kc + 1], h.y));
-                l.z = to_tf32(__fsub_rn(v[4 * kc + 2], h.z)); l.w = to_tf32(__fsub_rn(v[4 * kc + 3], h.w));
-                reinterpret_cast<float4 *>(sX)[kc * WG_ROWS + r] = h;
-                reinterpret_cast<float4 *>(sX)[(8 + kc) * WG_ROWS + r] = l;
-            }
-            if (half == 0) { epsr[r] = ee; cnt[r] = 0; }
         }
+        v[2 * FL] = 1.0f;
+#pragma unroll
+        for (int j = 2 * FL + 1; j < TC_K; ++j) v[j] = 0.f;
+#pragma unroll
+        for (int kc = 0; kc < 8; ++kc) {
+            if ((kc & 1) != half) continue;
+            float4 h, l;
+            h.x = to_tf32(v[4 * kc]); h.y = to_tf32(v[4 * kc + 1]); h.z = to_tf32(v[4 * kc + 2]); h.w = to_tf32(v[4 * kc + 3]);
+            l.x = to_tf32(__fsub_rn(v[4 * kc], h.x)); l.y = to_tf32(__fsub_rn(v[4 * kc + 1], h.y));
+            l.z = to_tf32(__fsub_rn(v[4 * kc + 2], h.z)); l.w = to_tf32(__fsub_rn(v[4 * kc + 3], h.w));
+            reinterpret_cast<float4 *>(sX)[kc * WG_ROWS + r] = h;
+            reinterpret_cast<float4 *>(sX)[(8 + kc) * WG_ROWS + r] = l;
+        }
+        if (half == 0) eps[r] = __fadd_ru(__fmul_ru(S, TC_ERR), 2.0f);
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic-proxy writes -> visible to the tensor core
         warpgroup_bar(1 + wg);
-
-        // ---- 3 x TF32 GEMM of the warpgroup's 64 rows against all ND codewords ----
-        float acc[ND / 2];
+    };
+    // ---- 3 x TF32 GEMM of the warpgroup's 64 rows against all ND codewords, issued asynchronously ----
+    float acc[ND / 2];
+    auto gemm = [&]() {
 #pragma unroll
         for (int i = 0; i < ND / 2; ++i) acc[i] = 0.f;
         wgmma_fence_regs(acc);
@@ -547,12 +542,173 @@ ptm_wgmma_kernel(const float *__restrict__ feats, long long total, int D, const 
             }
         }
         asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
-        if (tile + 1 < tiles_per_cta) {
-            const long long rn = row + TC_ROWS;
-            const float *p = feats + (rn < total ? rn : 0) * D + featoff[f];
+    };
+
+    // ---- the rows of a tile whose candidates are stored: two threads per row; thread h takes the pairs of quad lanes 2 h
+    // and 2 h + 1, keeps its five largest candidates and writes its candidate codewords to the row's byte list (h = 0 from
+    // the front, h = 1 from byte TC_CAP - 1 down: they meet only if the row has more than TC_CAP candidates); the halves
+    // meet by shuffles ----
+    auto resolve = [&](const long long row0, const float *eps) {
+        const int rr = t >> 1, h = t & 1;
+        const long long row = row0 + rr;
+        const bool valid = row < total;
+        unsigned char *lb = reinterpret_cast<unsigned char *>(Lc + rr * 5);
+        float a[5] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY, -INFINITY};
+        int c[5] = {0, 0, 0, 0, 0};
+        int nl = 0;
+        bool over = false;                               // a lane of the row kept more than TC_CAP pairs
+        {
+            const float thr = thrs[rr];
+            auto cand = [&](float v, int col) {
+                const bool p = v >= thr;
+                if (p && nl < TC_CAP) lb[h ? TC_CAP - 1 - nl : nl] = (unsigned char)col;
+                nl += p ? 1 : 0;
+                v = p ? v : -INFINITY;
 #pragma unroll
-            for (int j = 0; j < FL; ++j) xn[j] = rn < total ? p[j] : 0.f;
+                for (int j = 0; j < 5; ++j) {
+                    const bool s = v > a[j];
+                    const float tv = a[j];
+                    const int tc = c[j];
+                    a[j] = s ? v : tv; c[j] = s ? col : tc;
+                    v = s ? tv : v; col = s ? tc : col;
+                }
+            };
+            // one loop over the stored pairs of both lanes (the first TC_CAP of each): a warp runs as many iterations as
+            // its busiest thread has pairs
+            unsigned m0 = Pm[rr * 4 + 2 * h], m1 = Pm[rr * 4 + 2 * h + 1];
+            over = __popc(m0) > TC_CAP || __popc(m1) > TC_CAP;
+            int j0 = 0, j1 = 0;
+            while ((m0 | m1) != 0u) {
+                const bool first = m0 != 0u;
+                const unsigned msk = first ? m0 : m1;
+                const int i = __ffs(msk) - 1, q = 2 * h + (first ? 0 : 1), j = first ? j0 : j1;
+                const float2 v = Pv[j * WG_ROWS * 4 + rr * 4 + q];
+                cand(v.x, 8 * i + 2 * q);
+                cand(v.y, 8 * i + 2 * q + 1);
+                if (first) { m0 = ++j0 < TC_CAP ? m0 & (m0 - 1u) : 0u; }
+                else { m1 = ++j1 < TC_CAP ? m1 & (m1 - 1u) : 0u; }
+            }
         }
+        const int n1 = __shfl_xor_sync(FULL, nl, 1), n = nl + n1;
+        over = __shfl_xor_sync(FULL, (int)over, 1) != 0 || over;
+        {
+            // the five largest of the row: max(a[j], b[4 - j]) over the two sorted halves, then a sorting network
+            float b[5];
+            int bc[5];
+#pragma unroll
+            for (int j = 0; j < 5; ++j) { b[j] = __shfl_xor_sync(FULL, a[j], 1); bc[j] = __shfl_xor_sync(FULL, c[j], 1); }
+#pragma unroll
+            for (int j = 0; j < 5; ++j)
+                if (b[4 - j] > a[j]) { a[j] = b[4 - j]; c[j] = bc[4 - j]; }
+            auto cmpx = [&](int i, int j) {
+                if (a[j] > a[i]) { const float tv = a[i]; const int tc = c[i]; a[i] = a[j]; c[i] = c[j]; a[j] = tv; c[j] = tc; }
+            };
+            cmpx(0, 1); cmpx(3, 4); cmpx(2, 4); cmpx(2, 3); cmpx(1, 4); cmpx(0, 3); cmpx(0, 2); cmpx(1, 3); cmpx(1, 2);
+        }
+        const bool listed = n >= 5 && n <= TC_CAP && !over;
+        const float ee = eps[rr];
+
+        // ---- the record straight from the filter values when they leave no doubt ----
+        bool certain = listed;
+        {
+            // order and distinctness of the truncated scores: neighbours more than 2 eps + 1 apart, everything safely
+            // negative (truncation is towards zero); s >> 10 of the four best: the same at both ends of [a - eps, a + eps]
+            const float gap = __fadd_ru(__fadd_ru(ee, ee), 1.0f);
+            int qv[4];
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                certain &= __fsub_rd(a[j], a[j + 1]) > gap;
+                const int lo = __float2int_ru(__fsub_rd(a[j], ee)), hi = __float2int_ru(__fadd_ru(a[j], ee));
+                certain &= (lo >> PSB_SENSCR_SHIFT) == (hi >> PSB_SENSCR_SHIFT);
+                qv[j] = lo >> PSB_SENSCR_SHIFT;
+            }
+            certain &= __fadd_ru(a[0], ee) < -2.0f && a[4] > -2.0e9f;
+            if (valid && h == 0) {
+                if (CHECK) atomicMax(reinterpret_cast<int *>(check) + 1, n);
+                if (certain) {
+                    unsigned cb = 0, eb = 0;
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) {
+                        int ev = qv[0] - qv[j];
+                        ev = ev > 255 ? 255 : ev;
+                        cb |= (unsigned)c[j] << (8 * j);
+                        eb |= (unsigned)ev << (8 * j);
+                    }
+                    out[row * K + k] = make_int4(qv[0], (int)cb, (int)eb, 0);
+                    if (CHECK) { atomicAdd(stats, 1ull); atomicAdd(stats + 1, 1ull); }
+                }
+            }
+        }
+        // ---- doubt: the row goes to ptm_tc_exact_kernel's work list (one atomic per warp); only when that list is full
+        // is the exact arithmetic done here ----
+        __syncwarp();                                    // the partner's codeword bytes are in the row's list
+        const bool doubt = valid && h == 0 && !certain;
+        const int n0 = listed ? nl : 255, nb = listed ? n1 : 0;   // n0 = 255: all codewords
+        bool handled = false;
+        if (items) {
+            const unsigned need = __ballot_sync(FULL, doubt);
+            if (need) {
+                const int leader = __ffs(need) - 1;
+                unsigned base = 0;
+                if (lane == leader) base = atomicAdd(n_items, (unsigned)__popc(need));
+                base = __shfl_sync(FULL, base, leader);
+                const unsigned slot = base + (unsigned)__popc(need & ((1u << lane) - 1u));
+                if (doubt && slot < item_cap) {
+                    const unsigned *w = Lc + rr * 5;
+                    items[2 * (size_t)slot] = make_uint4((unsigned)row, (unsigned)k | ((unsigned)n0 << 16) | ((unsigned)nb << 24), w[0], w[1]);
+                    items[2 * (size_t)slot + 1] = make_uint4(w[2], w[3], w[4], (unsigned)(row >> 32));
+                    handled = true;
+                    if (CHECK) atomicAdd(stats, 1ull);
+                }
+            }
+        }
+        if (doubt && !handled) {
+            // the reference's exact arithmetic for this row's candidates (all codewords if the list overflowed)
+            float x[FL];
+            const float *px = feats + row * D + featoff[f];
+#pragma unroll
+            for (int j = 0; j < FL; ++j) x[j] = px[j];
+            Top5 top;
+            top.n = 0; top.c = 0u; top.c4 = 0;
+#pragma unroll
+            for (int j = 0; j < 5; ++j) top.s[j] = INT_MIN;
+            const int cnt_l = listed ? n : ND;
+            for (int i = 0; i < cnt_l; ++i) {
+                const int cw = listed ? (int)lb[i < n0 ? i : i - n0 + TC_CAP - nb] : i;
+                const float d = gau_dist<FL>(reinterpret_cast<const float4 *>(rc + (size_t)cw * RF), x);
+                top5_insert(top, f2i_clamped(d), cw);
+            }
+            const bool distinct = top.n >= 5 && top.s[0] > top.s[1] && top.s[1] > top.s[2] && top.s[2] > top.s[3] && top.s[3] > top.s[4];
+            const int tp = top.s[0] >> PSB_SENSCR_SHIFT;
+            unsigned eb = 0;
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                int ev = tp - (top.s[j] >> PSB_SENSCR_SHIFT);
+                ev = ev > 255 ? 255 : ev;
+                eb |= (unsigned)ev << (8 * j);
+            }
+            out[row * K + k] = make_int4(tp, (int)top.c, (int)eb, 0);
+            if (!distinct) atomicOr(&flags[(size_t)k * flag_words + (row >> 5)], 1u << (row & 31));
+            if (CHECK) { atomicAdd(stats, 1ull); atomicAdd(stats + 2, (unsigned long long)cnt_l); if (!distinct) atomicAdd(stats + 3, 1ull); }
+        }
+    };
+
+    // the next tile's GEMM runs on the tensor core while this tile's rows are resolved: X and its bounds are written as
+    // soon as this tile's candidates are stored (its GEMM is complete then), the bounds alternate between two buffers
+    long long row0 = (long long)blockIdx.y * tiles_per_cta * TC_ROWS + wg * WG_ROWS;
+    if (row0 >= total) return;                           // uniform in the warpgroup: its rows lie past the end
+    fetch(row0 + r);
+    prepare(epsr);
+    int buf = 0;                                         // the bounds buffer of the current tile
+    for (int tile = 0;; ++tile, buf ^= 1, row0 += TC_ROWS) {
+        gemm();
+        const bool more = tile + 1 < tiles_per_cta && row0 + TC_ROWS < total;
+        if (more) fetch(row0 + TC_ROWS + r);
+        if (tile > 0) {
+            resolve(row0 - TC_ROWS, epsr + (buf ^ 1) * WG_ROWS);
+            warpgroup_bar(1 + wg);                       // lists consumed: this tile may overwrite pairs and lists
+        }
+        const float *eps = epsr + buf * WG_ROWS;
         asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
         wgmma_fence_regs(acc);
 
@@ -562,45 +718,48 @@ ptm_wgmma_kernel(const float *__restrict__ feats, long long total, int D, const 
         for (int q = 0; q < 8; ++q) {
             float a = -INFINITY, b = -INFINITY;
 #pragma unroll
-            for (int i = q * NPG; i < (q + 1) * NPG; ++i) {
-                a = fmaxf(a, fmaxf(acc[4 * i], acc[4 * i + 1]));
-                b = fmaxf(b, fmaxf(acc[4 * i + 2], acc[4 * i + 3]));
+            for (int i = q * NPG; i < (q + 1) * NPG; ++i) {     // a chain: the pair maxima below are not kept live
+                a = fmaxf(fmaxf(a, acc[4 * i]), acc[4 * i + 1]);
+                b = fmaxf(fmaxf(b, acc[4 * i + 2]), acc[4 * i + 3]);
             }
             a = fmaxf(a, __shfl_xor_sync(FULL, a, 1)); a = fmaxf(a, __shfl_xor_sync(FULL, a, 2));
             b = fmaxf(b, __shfl_xor_sync(FULL, b, 1)); b = fmaxf(b, __shfl_xor_sync(FULL, b, 2));
             gma[q] = a; gmb[q] = b;
         }
-        // five distinct columns >= L0: the fifth largest of the eight group maxima
-        auto fifth = [](const float (&gm)[8]) {
-            float a5[5] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY, -INFINITY};
+        // five distinct columns >= L0: the fifth largest of the eight group maxima.  With both halves sorted (descending)
+        // it is max_i min(first[i], second[3 - i])
+        auto fifth = [](float (&gm)[8]) {
+            auto cmpx = [&](int i, int j) { const float hi = fmaxf(gm[i], gm[j]); gm[j] = fminf(gm[i], gm[j]); gm[i] = hi; };
 #pragma unroll
-            for (int q = 0; q < 8; ++q) {
-                float v = gm[q];
-#pragma unroll
-                for (int j = 0; j < 5; ++j) { const float hi = fmaxf(a5[j], v); v = fminf(a5[j], v); a5[j] = hi; }
-            }
-            return a5[4];
+            for (int o = 0; o < 8; o += 4) { cmpx(o, o + 1); cmpx(o + 2, o + 3); cmpx(o, o + 2); cmpx(o + 1, o + 3); cmpx(o + 1, o + 2); }
+            return fmaxf(fmaxf(fminf(gm[0], gm[7]), fminf(gm[1], gm[6])), fmaxf(fminf(gm[2], gm[5]), fminf(gm[3], gm[4])));
         };
-        const float e_a = epsr[ra], e_b = epsr[rb];
+        const float e_a = eps[ra], e_b = eps[rb];
         // L' = floor(L0 - eps) - 1, candidates: a_c >= L' - eps; every step rounded towards -inf
         const float thra = __fsub_rd(__fsub_rd(floorf(__fsub_rd(fifth(gma), e_a)), 1.0f), e_a);
         const float thrb = __fsub_rd(__fsub_rd(floorf(__fsub_rd(fifth(gmb), e_b)), 1.0f), e_b);
-        const float thr_min = fminf(thra, thrb);
+        {
+            // the lane's pair (8 i + 2 q4, + 1) of a row is kept when its larger value passes: predicated stores to the
+            // lane's next slot and a mask bit, no branch; past TC_CAP pairs the lane writes the overflow slot again (the row
+            // then has more than TC_CAP candidates, and its mask says so)
+            constexpr int SS = WG_ROWS * 4;                  // slot stride in pairs
+            int oa = ra * 4 + q4, ob = rb * 4 + q4;
+            const int lim_a = oa + TC_CAP * SS, lim_b = ob + TC_CAP * SS;
+            unsigned ma = 0u, mb = 0u;
 #pragma unroll
-        for (int i = 0; i < NTL; ++i) {
-            if (fmaxf(fmaxf(acc[4 * i], acc[4 * i + 1]), fmaxf(acc[4 * i + 2], acc[4 * i + 3])) < thr_min) continue;
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                const float a = acc[4 * i + e];
-                const int rr = (e & 2) ? rb : ra;
-                if (a >= ((e & 2) ? thrb : thra)) {
-                    const int slot = atomicAdd(&cnt[rr], 1);
-                    if (slot < TC_CAP) {
-                        Lv[slot * WG_ROWS + rr] = a;
-                        Lc[slot * WG_ROWS + rr] = (unsigned char)(8 * i + 2 * q4 + (e & 1));
-                    }
-                }
+            for (int i = 0; i < NTL; ++i) {
+                const bool pa = fmaxf(acc[4 * i], acc[4 * i + 1]) >= thra;
+                const bool pb = fmaxf(acc[4 * i + 2], acc[4 * i + 3]) >= thrb;
+                if (pa) Pv[oa] = make_float2(acc[4 * i], acc[4 * i + 1]);
+                if (pb) Pv[ob] = make_float2(acc[4 * i + 2], acc[4 * i + 3]);
+                oa = pa ? min(oa + SS, lim_a) : oa;
+                ob = pb ? min(ob + SS, lim_b) : ob;
+                ma |= pa ? 1u << i : 0u;
+                mb |= pb ? 1u << i : 0u;
             }
+            Pm[ra * 4 + q4] = ma;
+            Pm[rb * 4 + q4] = mb;
+            if (q4 == 0) { thrs[ra] = thra; thrs[rb] = thrb; }
         }
         if (CHECK) {
             // exact distances of every column this lane holds (debug only): |a - d| / eps
@@ -610,7 +769,7 @@ ptm_wgmma_kernel(const float *__restrict__ feats, long long total, int D, const 
                 const int rr = h ? rb : ra;
                 if (row0 + rr >= total) continue;
                 const float *px = feats + (row0 + rr) * D + featoff[f];
-                const float er = epsr[rr];
+                const float er = eps[rr];
 #pragma unroll
                 for (int i = 0; i < NTL; ++i)
 #pragma unroll
@@ -626,104 +785,17 @@ ptm_wgmma_kernel(const float *__restrict__ feats, long long total, int D, const 
             }
             atomicMax(reinterpret_cast<int *>(check), __float_as_int(worst));     // non-negative floats order like ints
         }
-        warpgroup_bar(1 + wg);                           // every row's list is complete
-
-        // ---- the record straight from the filter values when they leave no doubt ----
-        if (valid && half == 0) {
-            const int n = cnt[r];
-            const bool listed = n >= 5 && n <= TC_CAP;
-            auto cand_v = [&](int i) { return Lv[i * WG_ROWS + r]; };
-            auto cand_c = [&](int i) { return (int)Lc[i * WG_ROWS + r]; };
-            if (CHECK) atomicMax(reinterpret_cast<int *>(check) + 1, n);
-            bool certain = listed;
-            if (certain) {
-                float a[5] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY, -INFINITY};
-                int c[5] = {0, 0, 0, 0, 0};
-                for (int i = 0; i < n; ++i) {
-                    float v = cand_v(i);
-                    int cv = cand_c(i);
-#pragma unroll
-                    for (int j = 0; j < 5; ++j)
-                        if (v > a[j]) { const float tv = a[j]; const int tc = c[j]; a[j] = v; c[j] = cv; v = tv; cv = tc; }
-                }
-                const float gap = __fadd_ru(__fadd_ru(ee, ee), 1.0f);
-                int qv[4];
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    certain &= __fsub_rd(a[j], a[j + 1]) > gap;
-                    const int lo = __float2int_ru(__fsub_rd(a[j], ee)), hi = __float2int_ru(__fadd_ru(a[j], ee));
-                    certain &= (lo >> PSB_SENSCR_SHIFT) == (hi >> PSB_SENSCR_SHIFT);
-                    qv[j] = lo >> PSB_SENSCR_SHIFT;
-                }
-                certain &= __fadd_ru(a[0], ee) < -2.0f && a[4] > -2.0e9f;
-                if (certain) {
-                    unsigned cb = 0, eb = 0;
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        int ev = qv[0] - qv[j];
-                        ev = ev > 255 ? 255 : ev;
-                        cb |= (unsigned)c[j] << (8 * j);
-                        eb |= (unsigned)ev << (8 * j);
-                    }
-                    out[row * K + k] = make_int4(qv[0], (int)cb, (int)eb, 0);
-                    if (CHECK) { atomicAdd(stats, 1ull); atomicAdd(stats + 1, 1ull); }
-                }
-            }
-            // doubt: the row goes to ptm_tc_exact_kernel's work list (one atomic per warp); only when that list is full
-            // is the exact arithmetic done here
-            if (!certain && items) {
-                const unsigned who = __activemask();
-                const unsigned need = __ballot_sync(who, true);
-                const int leader = __ffs(need) - 1;
-                unsigned base = 0;
-                if ((tid & 31) == leader) base = atomicAdd(n_items, (unsigned)__popc(need));
-                base = __shfl_sync(need, base, leader);
-                const unsigned slot = base + (unsigned)__popc(need & ((1u << (tid & 31)) - 1u));
-                if (slot < item_cap) {
-                    unsigned wv[5] = {0u, 0u, 0u, 0u, 0u};
-                    if (listed)
-                        for (int i = 0; i < n; ++i) wv[i >> 2] |= (unsigned)cand_c(i) << (8 * (i & 3));
-                    items[2 * (size_t)slot] = make_uint4((unsigned)row, (unsigned)k | ((listed ? (unsigned)n : 255u) << 16), wv[0], wv[1]);
-                    items[2 * (size_t)slot + 1] = make_uint4(wv[2], wv[3], wv[4], (unsigned)(row >> 32));
-                    certain = true;                       // handled
-                    if (CHECK) atomicAdd(stats, 1ull);
-                }
-            }
-            if (!certain) {
-                // the reference's exact arithmetic for this row's candidates (all codewords if the list overflowed)
-                Top5 top;
-                top.n = 0; top.c = 0u; top.c4 = 0;
-#pragma unroll
-                for (int j = 0; j < 5; ++j) top.s[j] = INT_MIN;
-                int n_exact = 0;
-                const int cnt_l = listed ? n : ND;
-                for (int i = 0; i < cnt_l; ++i) {
-                    const int cw = listed ? cand_c(i) : i;
-                    const float d = gau_dist<FL>(reinterpret_cast<const float4 *>(rc + (size_t)cw * RF), x);
-                    top5_insert(top, f2i_clamped(d), cw);
-                    ++n_exact;
-                }
-                const bool distinct = top.n >= 5 && top.s[0] > top.s[1] && top.s[1] > top.s[2] && top.s[2] > top.s[3] && top.s[3] > top.s[4];
-                const int tp = top.s[0] >> PSB_SENSCR_SHIFT;
-                unsigned eb = 0;
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                    int ev = tp - (top.s[j] >> PSB_SENSCR_SHIFT);
-                    ev = ev > 255 ? 255 : ev;
-                    eb |= (unsigned)ev << (8 * j);
-                }
-                out[row * K + k] = make_int4(tp, (int)top.c, (int)eb, 0);
-                if (!distinct) atomicOr(&flags[(size_t)k * flag_words + (row >> 5)], 1u << (row & 31));
-                if (CHECK) { atomicAdd(stats, 1ull); atomicAdd(stats + 2, (unsigned long long)n_exact); if (!distinct) atomicAdd(stats + 3, 1ull); }
-            }
-        }
-        warpgroup_bar(1 + wg);                           // lists consumed: the next tile may overwrite X, lists and counts
+        warpgroup_bar(1 + wg);                           // every row's pairs are stored, the GEMM's X may be overwritten
+        if (!more) break;
+        prepare(epsr + (buf ^ 1) * WG_ROWS);
     }
+    resolve(row0, epsr + buf * WG_ROWS);
 }
 
 // Rows the filter values left in doubt (work list of ptm_wgmma_kernel): one thread per row, the reference's exact
 // arithmetic for its candidate codewords (all codewords when its list had overflowed), the five best, the record;
-// exact ties go on to the fix-up.  Item: {row low, pair | n << 16, 18 codeword bytes, row high}.
+// exact ties go on to the fix-up.  Item: {row low, pair | n0 << 16 | n1 << 24, 18 codeword bytes, row high}: the
+// candidates are bytes 0 .. n0 - 1 and TC_CAP - n1 .. TC_CAP - 1 (n0 = 255: all codewords).
 template <int FL>
 __global__ void __launch_bounds__(128)
 ptm_tc_exact_kernel(const float *__restrict__ feats, int D, const int32_t *__restrict__ featoff, const uint4 *__restrict__ items,
@@ -736,7 +808,7 @@ ptm_tc_exact_kernel(const float *__restrict__ feats, int D, const int32_t *__res
     for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < count; i += gridDim.x * blockDim.x) {
         const uint4 a = items[2 * (size_t)i], b = items[2 * (size_t)i + 1];
         const long long row = (long long)a.x | ((long long)b.w << 32);
-        const int k = (int)(a.y & 0xffffu), n = (int)(a.y >> 16);
+        const int k = (int)(a.y & 0xffffu), n0 = (int)((a.y >> 16) & 0xffu), n1 = (int)(a.y >> 24);
         const unsigned wv[5] = {a.z, a.w, b.x, b.y, b.z};
         const float *px = feats + row * D + featoff[k % n_feat];
         const float *rc = rec + rec_off[k];
@@ -747,9 +819,10 @@ ptm_tc_exact_kernel(const float *__restrict__ feats, int D, const int32_t *__res
         top.n = 0; top.c = 0u; top.c4 = 0;
 #pragma unroll
         for (int j = 0; j < 5; ++j) top.s[j] = INT_MIN;
-        const int cnt = n == 255 ? nd : n;
+        const int cnt = n0 == 255 ? nd : n0 + n1;
         for (int q = 0; q < cnt; ++q) {
-            const int cw = n == 255 ? q : (int)((wv[q >> 2] >> (8 * (q & 3))) & 0xffu);
+            const int pos = q < n0 ? q : q - n0 + TC_CAP - n1;
+            const int cw = n0 == 255 ? q : (int)((wv[pos >> 2] >> (8 * (pos & 3))) & 0xffu);
             const float d = gau_dist<FL>(reinterpret_cast<const float4 *>(rc + (size_t)cw * RF), x);
             top5_insert(top, f2i_clamped(d), cw);
         }
@@ -994,12 +1067,13 @@ int launch_wgmma(psb_batch_t *b, const float *d_feats, long long total, const in
     const size_t smem = (size_t)2 * 8 * ND * 16 + 2 * ((size_t)2 * 8 * WG_ROWS * 16 + WG_EXTRA);
     const long long tiles = (total + TC_ROWS - 1) / TC_ROWS;
     const int n_sm = psb_sm_count(m->device);
-    int per_sm = 1;                                      // sm_90: 147-255 registers x 256 threads, one CTA per SM
+    int per_sm = 1;                                      // sm_90: 151-255 registers x 256 threads, one CTA per SM
     PSB_CUDA(cudaFuncSetAttribute(ptm_wgmma_kernel<FL, ND, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     PSB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ptm_wgmma_kernel<FL, ND, false>, TC_ROWS * 2, smem));
-    // W (64 KB at 256 densities) is staged once per CTA: a few tiles per CTA, but still >= 4 waves of the resident CTAs
+    // W (64 KB at 256 densities) is staged once per CTA, and a CTA's first GEMM and last rows do not overlap: many tiles
+    // per CTA, but still >= 4 waves of the resident CTAs
     int tpc = 1;
-    while (tpc < 8 && (tiles / (tpc * 2)) * n_k >= (long long)n_sm * std::max(per_sm, 1) * 4) tpc *= 2;
+    while (tpc < 32 && (tiles / (tpc * 2)) * n_k >= (long long)n_sm * std::max(per_sm, 1) * 4) tpc *= 2;
     PSB_REQUIRE((tiles + tpc - 1) / tpc <= 65535, "too many frames for one launch of the tensor-core filter");
     const dim3 grid((unsigned)n_k, (unsigned)((tiles + tpc - 1) / tpc));
     float *chk = b->d_tc_check;
