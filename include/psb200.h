@@ -141,6 +141,16 @@ int psb_batch_event_elapsed_ms(psb_batch_t *b, float *ms);
  * below 1) and the largest candidate count per (frame, codebook-stream pair); stats4 (may be NULL) = rows seen,
  * rows whose record came from the filter values alone, exact distances computed, rows handed to the tie fix-up. */
 int psb_batch_tc_check(psb_batch_t *b, float *ratio, int32_t *max_candidates, int64_t *stats4);
+/* debugging (PSB_TC_CHECK=1): which decisions the tensor-core filter took over everything this batch has scored.
+ * out[0..n-1] receives the first n of, in order: the four stats4 values; rows with more than 18 candidates
+ * (the filter kernel's per-row list capacity); rows where one lane of the wgmma filter stored more than 18 column
+ * pairs; rows in doubt rescored inside the wgmma filter kernel because its work list was full, with a candidate
+ * list and over all codewords; rows in doubt whose candidate list the wgmma filter's two threads per row both
+ * wrote; rows with a candidate list that failed the gap test, the >> 10 agreement test, the sign guard and the
+ * saturation guard (one row can fail several); then, without PSB_TC_CHECK too, the last filter launch's tiles per
+ * CTA and its CTAs per codebook-stream pair. */
+#define PSB_TC_N_COUNTERS 15
+int psb_batch_tc_counters(psb_batch_t *b, int64_t *out, int32_t n);
 /* debugging/parity: copy the per-frame top-N records of the last call to the host:
  * rec int32 [total_frames][n_mgau*n_feat][4] = {top>>10, cw[4] bytes, e[4] bytes, 0} */
 int psb_batch_get_topn(psb_batch_t *b, int32_t *rec, int64_t n_frames);

@@ -63,7 +63,7 @@ def lib():
         L.pso_gmm_reset.argtypes = [C.c_void_p]
         L.pso_frame_eval.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
                                      C.c_int32, C.c_int32]
-        L.pso_score_utt.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
+        L.pso_score_utt.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
         L.pso_flags2list.restype = C.c_int32
         L.pso_flags2list.argtypes = [C.c_void_p, C.c_int32, C.c_void_p]
         L.pso_time_score_utt.restype = C.c_double
@@ -109,18 +109,24 @@ class OracleModel:
         m.fixed_point = int(getattr(pm, "fixed_point", 0))
         self.c = m
 
-    def score_utt(self, feats, want_topn=False):
+    def score_utt(self, feats, want_topn=False, want_raw=False):
+        """Scores [T][n_sen]; with want_topn the normalised top-N lists, with want_raw (ptm) the lists before
+        normalisation, [T][n_mgau][n_feat][topn]{codeword, integer distance} (see ptm_records)."""
         pm = self.pm
         feats = np.ascontiguousarray(feats, np.float32)
         T = feats.shape[0]
         scr = np.zeros((T, pm.n_sen), np.int16)
-        topn = None
+        topn = raw = None
         if want_topn and pm.kind == "ptm":
             topn = np.zeros((T, pm.n_mgau, pm.n_feat, pm.topn, 2), np.int32)
         elif want_topn and pm.kind == "s2_semi":
             topn = np.zeros((T, pm.n_feat, pm.topn, 2), np.int32)
-        lib().pso_score_utt(C.byref(self.c), _p(feats), T, _p(scr), _p(topn))
-        return (scr, topn) if want_topn else scr
+        if want_raw:
+            assert pm.kind == "ptm", "raw top-N lists exist for ptm models"
+            raw = np.zeros((T, pm.n_mgau, pm.n_feat, pm.topn, 2), np.int32)
+        lib().pso_score_utt(C.byref(self.c), _p(feats), T, _p(scr), _p(topn), _p(raw))
+        out = (scr,) + ((topn,) if want_topn else ()) + ((raw,) if want_raw else ())
+        return out if len(out) > 1 else scr
 
     def time_score_utt(self, feats, reps=1):
         feats = np.ascontiguousarray(feats, np.float32)
@@ -176,6 +182,50 @@ def flags2list(flags):
     out = np.zeros(len(flags), np.uint8)
     n = lib().pso_flags2list(_p(flags), len(flags), _p(out))
     return out[:n].copy()
+
+
+SENSCR_SHIFT, MAX_NEG_ASCR = 10, 96
+
+
+def ptm_records(raw):
+    """Raw PTM lists [T][n_mgau][n_feat][4]{codeword, score} (score_utt(want_raw=True)) -> the device's top-N
+    records int32 [T][n_mgau * n_feat][4] (psb_batch_get_topn): {s0 >> 10, the four codewords as bytes,
+    min(255, (s0 >> 10) - (sj >> 10)) as bytes, 0}."""
+    raw = np.asarray(raw)
+    assert raw.shape[-2:] == (4, 2), "records hold four list entries"
+    T = raw.shape[0]
+    cw = raw[..., 0].reshape(T, -1, 4).astype(np.uint32)
+    q = raw[..., 1].reshape(T, -1, 4) >> SENSCR_SHIFT
+    e = np.minimum(255, q[..., :1] - q).astype(np.uint32)
+    rec = np.zeros(cw.shape[:2] + (4,), np.int32)
+    rec[..., 0] = q[..., 0]
+    rec[..., 1] = (cw[..., 0] | cw[..., 1] << 8 | cw[..., 2] << 16 | cw[..., 3] << 24).view(np.int32)
+    rec[..., 2] = (e[..., 0] | e[..., 1] << 8 | e[..., 2] << 16 | e[..., 3] << 24).view(np.int32)
+    return rec
+
+
+def ptm_norm_raw(raw):
+    """ptm_mgau_codebook_norm (every codebook active) applied to raw lists: what score_utt(want_topn=True) returns."""
+    out = np.array(raw, np.int32, copy=True)
+    q = out[..., 1] >> SENSCR_SHIFT                               # [T][cb][f][topn]
+    norm = q[:, :, :, 0].max(axis=1)                              # per frame and stream
+    out[..., 1] = np.minimum(MAX_NEG_ASCR, norm[:, None, :, None] - q)
+    return out
+
+
+def assert_records_equal(got, want, what=""):
+    """Top-N records [T][K][4]: equal, or an error naming the first differing (frame, pair) and field."""
+    got, want = np.asarray(got, np.int32), np.asarray(want, np.int32)
+    assert got.shape == want.shape, "%s: record shapes %s vs %s" % (what, got.shape, want.shape)
+    g, w = got.view(np.uint32), want.view(np.uint32)          # codeword bytes compare as uint32
+    bad = np.argwhere((g != w).any(-1))
+    if bad.size:
+        t, k = bad[0]
+        names = ("top score >> 10", "codewords", "score offsets", "padding")
+        fld = int(np.argmax(g[t, k] != w[t, k]))
+        raise AssertionError("%s: %d records differ; first at frame %d, pair %d: field %s got 0x%08x want 0x%08x "
+                             "(got %s, want %s)" % (what, len(bad), t, k, names[fld], g[t, k, fld], w[t, k, fld],
+                                                    g[t, k].tolist(), w[t, k].tolist()))
 
 
 class OracleHmmCtx:

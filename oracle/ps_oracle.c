@@ -474,6 +474,8 @@ ptm_frame_eval(pso_gmm_t *g, int16_t *senscr, const uint8_t *list, int32_t n_lis
                     else
                         scan_cb_ptm(m, slot + ((size_t)cb * m->n_feat + f) * m->topn, cb, f, feat + off);
             }
+        if (g->raw)
+            memcpy(g->raw, slot, per * sizeof(*slot));
         ptm_norm(m, slot, active);
     }
     ptm_senones(m, slot, active, senscr, list, n_list, compall);
@@ -715,11 +717,13 @@ pso_frame_eval(pso_gmm_t *g, int16_t *senscr, const uint8_t *senone_active,
 
 int
 pso_score_utt(const pso_model_t *m, const float *feats, int32_t T, int16_t *senscr,
-              int32_t *topn_out)
+              int32_t *topn_out, int32_t *raw_out)
 {
     pso_gmm_t *g = pso_gmm_new(m, 2);
+    size_t per_ptm = (size_t)m->n_mgau * m->n_feat * m->topn;
     int32_t t;
     for (t = 0; t < T; ++t) {
+        g->raw = raw_out && m->kind == PSO_KIND_PTM ? (pso_topn_t *)raw_out + (size_t)t * per_ptm : NULL;
         pso_frame_eval(g, senscr + (size_t)t * m->n_sen, NULL, 0, feats + (size_t)t * g->sumlen, t, 1);
         g->frame_idx = t + 1;       /* acmod_advance (acmod.c:868-877) */
         if (topn_out && m->kind != PSO_KIND_MS) {
@@ -758,10 +762,10 @@ pso_time_score_utt(const pso_model_t *m, const float *feats, int32_t T, int32_t 
     int16_t *scr = malloc((size_t)T * m->n_sen * sizeof(*scr));
     struct timespec a, b;
     int r;
-    pso_score_utt(m, feats, T < 16 ? T : 16, scr, NULL);
+    pso_score_utt(m, feats, T < 16 ? T : 16, scr, NULL, NULL);
     clock_gettime(CLOCK_MONOTONIC, &a);
     for (r = 0; r < reps; ++r)
-        pso_score_utt(m, feats, T, scr, NULL);
+        pso_score_utt(m, feats, T, scr, NULL, NULL);
     clock_gettime(CLOCK_MONOTONIC, &b);
     free(scr);
     return (b.tv_sec - a.tv_sec) + 1e-9 * (b.tv_nsec - a.tv_nsec);

@@ -65,6 +65,7 @@ typedef struct pso_gmm_s {
     uint8_t *cb_active;    /* ptm: [n_hist][n_mgau] */
     uint8_t *hist_n;       /* semi: [n_hist][n_feat] */
     pso_topn_t *ms_dist;   /* ms scratch: [n_mgau][n_feat][topn], score field holds float bits */
+    pso_topn_t *raw;       /* ptm, optional: receives each evaluated frame's lists before ptm_norm */
     int32_t sumlen;
 } pso_gmm_t;
 
@@ -77,9 +78,11 @@ int pso_frame_eval(pso_gmm_t *g, int16_t *senscr, const uint8_t *senone_active,
                    int32_t n_senone_active, const float *feat, int32_t frame, int32_t compallsen);
 
 /* Fresh state, compallsen, frames 0..T-1, frame_idx advanced like acmod_advance.
- * topn_out optional: ptm [T][n_mgau][n_feat][topn]{cw,score}, semi [T][n_feat][topn]. */
+ * topn_out optional: ptm [T][n_mgau][n_feat][topn]{cw,score}, semi [T][n_feat][topn].
+ * raw_out optional (ptm): the same lists before ptm_norm, with the integer distances that
+ * decide their order (what the device's top-N records hold). */
 int pso_score_utt(const pso_model_t *m, const float *feats, int32_t T, int16_t *senscr,
-                  int32_t *topn_out);
+                  int32_t *topn_out, int32_t *raw_out);
 
 /* acmod_flags2list (acmod.c:1224-1275): flags[n_sen] bytes -> delta list; returns count. */
 int32_t pso_flags2list(const uint8_t *flags, int32_t n_sen, uint8_t *list);

@@ -200,12 +200,18 @@ class Batch:
         check(lib().psb_batch_get_topn(self.h, _p(rec), n_frames), "psb_batch_get_topn")
         return rec
 
+    TC_COUNTERS = ("rows", "from_filter_alone", "exact_distances", "tie_fixups", "over_cap", "lane_over",
+                   "fallback_listed", "fallback_all", "split_lists", "fail_gap", "fail_straddle", "fail_sign",
+                   "fail_saturation", "tiles_per_cta", "ctas_per_pair")
+
     def tc_check(self):
-        """(max |filter value - exact distance| / bound, max candidates) of the tensor-core filter (PSB_TC_CHECK=1)."""
+        """(max |filter value - exact distance| / bound, max candidates) of the tensor-core filter (PSB_TC_CHECK=1);
+        tc_stats gets its decision-path counters by name (psb_batch_tc_counters)."""
         r, n = C.c_float(), C.c_int32()
-        st = np.zeros(4, np.int64)
-        check(lib().psb_batch_tc_check(self.h, C.byref(r), C.byref(n), _p(st)), "psb_batch_tc_check")
-        self.tc_stats = dict(rows=int(st[0]), from_filter_alone=int(st[1]), exact_distances=int(st[2]), tie_fixups=int(st[3]))
+        check(lib().psb_batch_tc_check(self.h, C.byref(r), C.byref(n), None), "psb_batch_tc_check")
+        st = np.zeros(len(self.TC_COUNTERS), np.int64)
+        check(lib().psb_batch_tc_counters(self.h, _p(st), len(st)), "psb_batch_tc_counters")
+        self.tc_stats = {k: int(v) for k, v in zip(self.TC_COUNTERS, st)}
         return r.value, n.value
 
     def decode_host(self, phoneloop, feats, utt_off, want_senscr=False, best=None, pen=None, senscr=None):

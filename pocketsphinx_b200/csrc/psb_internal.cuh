@@ -134,7 +134,9 @@ struct psb_batch_s {
                                   // 4/5 pairs + deferred insertion (2 / 1 utterances per lane),
                                   // 6 (default) tensor-core filter + exact rescoring where the model allows, else 5
     unsigned *d_tc_flags; size_t tc_flag_cap, tc_flag_words;   // [K][words]: frames the tie fix-up redoes
-    float *d_tc_check;            // debug (PSB_TC_CHECK=1): max |a - d| / eps, max candidates
+    float *d_tc_check;            // debug (PSB_TC_CHECK=1): max |a - d| / eps, max candidates, decision-path counters
+    int tc_last_tpc;              // the last filter launch: tiles per CTA (wgmma; 1 for mma.sync) and CTAs per pair
+    long long tc_last_ctas;
     uint4 *d_tc_items; unsigned *d_tc_nitems; unsigned tc_item_cap;   // rows the filter left in doubt (ptm_tc_exact_kernel)
     // phone-loop outputs for psb_decode_batch_host
     int32_t *d_best, *d_pen;

@@ -16,7 +16,7 @@
 //      `d >= (float)worst` holds -- and can never be evicted.  The list is then exactly those four
 //      in descending order, whatever the seeds were.  Only when two of the five best integer scores
 //      coincide do the order-dependent rules (`>=` shifting, strict `>` in eval_topn,
-//      skip-if-listed) matter; those frames are flagged and redone by ptm_fixup_kernel, which
+//      skip-if-listed) matter; those frames are flagged and redone by ptm_fixup_warp_kernel, which
 //      replays the reference's loop literally with the previous frame's list as seeds.
 //  (2) The five best can be found without computing 256 exact distances.  With y = x - m (m = the
 //      codebook's mean centre) the exponent d = det - sum_j v_j (y_j - mu'_j)^2 is the inner product
@@ -55,6 +55,18 @@ constexpr int TC_CAP = 18;            // candidate slots per row: the row's X st
 constexpr float TC_ERR = 1.0f / 262144.f;  // 2^-18 of the magnitude sum S: 3 x TF32 leaves 3 * 2^-22 per product, the rest is
                                            // room for the tensor core's fp32 accumulation (<= 2^-23 per step assumed, 12 steps per
                                            // chain) and the reference's own 52 roundings; PSB_TC_CHECK=1 measures what is used of it
+
+// PSB_TC_CHECK builds only: 64-bit counters at byte 16 of the batch's debug block (psb_batch_tc_counters)
+enum {
+    ST_ROWS, ST_FILTER_ALONE, ST_EXACT_DIST, ST_TIE_FLAGS,
+    ST_OVER_CAP,                                   // rows with more than TC_CAP candidates
+    ST_LANE_OVER,                                  // wgmma: rows where one quad lane stored more than TC_CAP pairs
+    ST_FALLBACK_LISTED, ST_FALLBACK_ALL,           // wgmma: rows in doubt rescored in the filter kernel (work list full)
+    ST_SPLIT,                                      // wgmma: rows in doubt whose candidate bytes came from both threads
+    ST_FAIL_GAP, ST_FAIL_STRADDLE, ST_FAIL_SIGN, ST_FAIL_SAT,   // listed rows failing each certainty test
+    ST_N
+};
+constexpr size_t TC_CHECK_BYTES = 16 + 8 * ST_N;
 
 __device__ __forceinline__ float to_tf32(float x)
 {
@@ -287,6 +299,7 @@ ptm_tc_kernel(const float *__restrict__ feats, long long total, int D, const int
 #pragma unroll
     for (int j = 0; j < 5; ++j) top.s[j] = INT_MIN;
     bool certain = n <= TC_CAP;
+    if (CHECK && !certain) atomicAdd(stats + ST_OVER_CAP, 1ull);
     if (certain) {
         // the five largest a_c with their codewords (the list holds every a_c >= thr, at least five)
         const uint2 *L = lists + (size_t)tid * (TC_XS / 2);
@@ -304,14 +317,22 @@ ptm_tc_kernel(const float *__restrict__ feats, long long total, int D, const int
         // [a - eps, a + eps]
         const float gap = __fadd_ru(__fadd_ru(ee, ee), 1.0f);
         int qv[4];
+        bool gap_ok = true, straddle_ok = true;
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
-            certain &= __fsub_rd(a[j], a[j + 1]) > gap;
+            gap_ok &= __fsub_rd(a[j], a[j + 1]) > gap;
             const int lo = __float2int_ru(__fsub_rd(a[j], ee)), hi = __float2int_ru(__fadd_ru(a[j], ee));
-            certain &= (lo >> PSB_SENSCR_SHIFT) == (hi >> PSB_SENSCR_SHIFT);
+            straddle_ok &= (lo >> PSB_SENSCR_SHIFT) == (hi >> PSB_SENSCR_SHIFT);
             qv[j] = lo >> PSB_SENSCR_SHIFT;
         }
-        certain &= __fadd_ru(a[0], ee) < -2.0f && a[4] > -2.0e9f;
+        const bool sign_ok = __fadd_ru(a[0], ee) < -2.0f, sat_ok = a[4] > -2.0e9f;
+        certain &= gap_ok && straddle_ok && sign_ok && sat_ok;
+        if (CHECK) {
+            if (!gap_ok) atomicAdd(stats + ST_FAIL_GAP, 1ull);
+            if (!straddle_ok) atomicAdd(stats + ST_FAIL_STRADDLE, 1ull);
+            if (!sign_ok) atomicAdd(stats + ST_FAIL_SIGN, 1ull);
+            if (!sat_ok) atomicAdd(stats + ST_FAIL_SAT, 1ull);
+        }
         if (certain) {
             unsigned cb = 0, eb = 0;
 #pragma unroll
@@ -615,16 +636,28 @@ ptm_wgmma_kernel(const float *__restrict__ feats, long long total, int D, const 
             // negative (truncation is towards zero); s >> 10 of the four best: the same at both ends of [a - eps, a + eps]
             const float gap = __fadd_ru(__fadd_ru(ee, ee), 1.0f);
             int qv[4];
+            bool gap_ok = true, straddle_ok = true;
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
-                certain &= __fsub_rd(a[j], a[j + 1]) > gap;
+                gap_ok &= __fsub_rd(a[j], a[j + 1]) > gap;
                 const int lo = __float2int_ru(__fsub_rd(a[j], ee)), hi = __float2int_ru(__fadd_ru(a[j], ee));
-                certain &= (lo >> PSB_SENSCR_SHIFT) == (hi >> PSB_SENSCR_SHIFT);
+                straddle_ok &= (lo >> PSB_SENSCR_SHIFT) == (hi >> PSB_SENSCR_SHIFT);
                 qv[j] = lo >> PSB_SENSCR_SHIFT;
             }
-            certain &= __fadd_ru(a[0], ee) < -2.0f && a[4] > -2.0e9f;
+            const bool sign_ok = __fadd_ru(a[0], ee) < -2.0f, sat_ok = a[4] > -2.0e9f;
+            certain &= gap_ok && straddle_ok && sign_ok && sat_ok;
             if (valid && h == 0) {
-                if (CHECK) atomicMax(reinterpret_cast<int *>(check) + 1, n);
+                if (CHECK) {
+                    atomicMax(reinterpret_cast<int *>(check) + 1, n);
+                    if (n > TC_CAP) atomicAdd(stats + ST_OVER_CAP, 1ull);
+                    if (over) atomicAdd(stats + ST_LANE_OVER, 1ull);
+                    if (listed) {
+                        if (!gap_ok) atomicAdd(stats + ST_FAIL_GAP, 1ull);
+                        if (!straddle_ok) atomicAdd(stats + ST_FAIL_STRADDLE, 1ull);
+                        if (!sign_ok) atomicAdd(stats + ST_FAIL_SIGN, 1ull);
+                        if (!sat_ok) atomicAdd(stats + ST_FAIL_SAT, 1ull);
+                    }
+                }
                 if (certain) {
                     unsigned cb = 0, eb = 0;
 #pragma unroll
@@ -644,6 +677,7 @@ ptm_wgmma_kernel(const float *__restrict__ feats, long long total, int D, const 
         __syncwarp();                                    // the partner's codeword bytes are in the row's list
         const bool doubt = valid && h == 0 && !certain;
         const int n0 = listed ? nl : 255, nb = listed ? n1 : 0;   // n0 = 255: all codewords
+        if (CHECK && doubt && listed && nl > 0 && n1 > 0) atomicAdd(stats + ST_SPLIT, 1ull);
         bool handled = false;
         if (items) {
             const unsigned need = __ballot_sync(FULL, doubt);
@@ -673,6 +707,7 @@ ptm_wgmma_kernel(const float *__restrict__ feats, long long total, int D, const 
 #pragma unroll
             for (int j = 0; j < 5; ++j) top.s[j] = INT_MIN;
             const int cnt_l = listed ? n : ND;
+            if (CHECK) atomicAdd(stats + (listed ? ST_FALLBACK_LISTED : ST_FALLBACK_ALL), 1ull);
             for (int i = 0; i < cnt_l; ++i) {
                 const int cw = listed ? (int)lb[i < n0 ? i : i - n0 + TC_CAP - nb] : i;
                 const float d = gau_dist<FL>(reinterpret_cast<const float4 *>(rc + (size_t)cw * RF), x);
@@ -841,85 +876,13 @@ ptm_tc_exact_kernel(const float *__restrict__ feats, int D, const int32_t *__res
     }
 }
 
-// Frames whose five best scores tie: the reference's loop, literally (eval_topn ptm_mgau.c:88-136,
-// eval_cb :152-226), seeded with the previous frame's list -- the record the filter kernel (or this
-// thread, one frame earlier) wrote -- or with codewords 0..3 at the start of an utterance (:791-792).
-// One thread per (utterance, pair); flagged frames of a chain are visited in order.
-template <int FL>
-__global__ void __launch_bounds__(128)
-ptm_fixup_kernel(const float *__restrict__ feats, int D, const int32_t *__restrict__ featoff, const int32_t *__restrict__ utt_off,
-                 int n_utt, const float *__restrict__ rec, const size_t *__restrict__ rec_off, int4 *__restrict__ out,
-                 const unsigned *__restrict__ flags, long long flag_words, int K, int n_feat, int nd)
-{
-    constexpr int RF = (1 + 2 * FL + 3) / 4 * 4;
-    const long long id = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (id >= (long long)n_utt * K) return;
-    const int u = (int)(id / K), k = (int)(id % K);
-    const int f = k % n_feat;
-    const long long f0 = utt_off[u], f1 = utt_off[u + 1];
-    const unsigned *fl = flags + (size_t)k * flag_words;
-    const float *rc = rec + rec_off[k];
-    for (long long wd = f0 >> 5; wd <= (f1 - 1) >> 5 && f1 > f0; ++wd) {
-        unsigned bits = fl[wd];
-        while (bits) {
-            const int b = __ffs(bits) - 1;
-            bits &= bits - 1;
-            const long long row = wd * 32 + b;
-            if (row < f0 || row >= f1) continue;
-            const float *px = feats + row * D + featoff[f];
-            float x[FL];
-#pragma unroll
-            for (int j = 0; j < FL; ++j) x[j] = px[j];
-            const unsigned seeds = row == f0 ? 0x03020100u : (unsigned)out[(row - 1) * K + k].y;
-            int cw[4], sc[4];
-            for (int i = 0; i < 4; ++i) {                                   // eval_topn: stable, strict >
-                const int c = (seeds >> (8 * i)) & 0xff;
-                const float *r = rc + (size_t)c * RF;
-                float d = r[0];
-#pragma unroll
-                for (int j = 0; j < FL; ++j) {
-                    const float df = __fsub_rn(x[j], r[1 + 2 * j]);
-                    d = __fsub_rn(d, __fmul_rn(__fmul_rn(df, df), r[2 + 2 * j]));
-                }
-                const int s = f2i_clamped(d);
-                int j = i - 1;
-                while (j >= 0 && s > sc[j]) { sc[j + 1] = sc[j]; cw[j + 1] = cw[j]; --j; }
-                sc[j + 1] = s; cw[j + 1] = c;
-            }
-            for (int c = 0; c < nd; ++c) {                                  // eval_cb (early exit is result-neutral)
-                const float *r = rc + (size_t)c * RF;
-                float d = r[0];
-#pragma unroll
-                for (int j = 0; j < FL; ++j) {
-                    const float df = __fsub_rn(x[j], r[1 + 2 * j]);
-                    d = __fsub_rn(d, __fmul_rn(__fmul_rn(df, df), r[2 + 2 * j]));
-                }
-                if (!(d >= (float)sc[3])) continue;
-                if (cw[0] == c || cw[1] == c || cw[2] == c || cw[3] == c) continue;
-                const int s = f2i_clamped(d);
-                int kk = 3;
-                while (kk > 0 && s >= sc[kk - 1]) { sc[kk] = sc[kk - 1]; cw[kk] = cw[kk - 1]; --kk; }
-                sc[kk] = s; cw[kk] = c;
-            }
-            const int tp = sc[0] >> PSB_SENSCR_SHIFT;
-            unsigned cb = 0, eb = 0;
-            for (int j = 0; j < 4; ++j) {
-                int ev = tp - (sc[j] >> PSB_SENSCR_SHIFT);
-                ev = ev > 255 ? 255 : ev;
-                cb |= (unsigned)cw[j] << (8 * j);
-                eb |= (unsigned)ev << (8 * j);
-            }
-            out[row * K + k] = make_int4(tp, (int)cb, (int)eb, 0);
-        }
-    }
-}
-
-// The same fix-up with a WARP per (utterance, pair) chain: lanes = codewords (ND / 32 each), the flagged frames of the
-// chain in order.  All distances of a frame in parallel, the four seeds fetched by shuffle, then the scan only visits --
-// in ascending codeword order -- the codewords whose distance reaches the seeds' worst score (ballots), each re-tested
-// against the list as it stands: eval_topn + eval_cb literally, like semi_scan_kernel does for semi-continuous models.
-// The thread-per-chain kernel above serialises 260 distances per flagged frame inside one lane; this one costs a few
-// hundred warp instructions per flagged frame.
+// Frames whose five best scores tie: the reference's loop, literally (eval_topn ptm_mgau.c:88-136, eval_cb :152-226),
+// seeded with the previous frame's list -- the record the filter kernel (or this warp, one frame earlier) wrote -- or
+// with codewords 0..3 at the start of an utterance (:791-792).  One WARP per (utterance, pair) chain: lanes = codewords
+// (ND / 32 each), the flagged frames of the chain in order.  All distances of a frame in parallel, the four seeds
+// fetched by shuffle, then the scan only visits -- in ascending codeword order -- the codewords whose distance reaches
+// the seeds' worst score (ballots), each re-tested against the list as it stands: eval_topn + eval_cb literally, like
+// semi_scan_kernel does for semi-continuous models.
 template <int FL, int NDW>
 __global__ void __launch_bounds__(128)
 ptm_fixup_warp_kernel(const float *__restrict__ feats, int D, const int32_t *__restrict__ featoff, const int32_t *__restrict__ utt_off,
@@ -1039,6 +1002,8 @@ int launch_tc(psb_batch_t *b, const float *d_feats, long long total, const int32
     psb_model_t *m = b->m;
     const size_t smem = (size_t)NT * 4 * 32 * 8 + (size_t)TC_ROWS * TC_XS * 4 + (size_t)TC_ROWS * 8 * 4 + TC_ROWS * 4 + TC_ROWS * 4;
     const dim3 grid((unsigned)((total + TC_ROWS - 1) / TC_ROWS), (unsigned)n_k);
+    b->tc_last_tpc = 1;
+    b->tc_last_ctas = grid.x;
     float *chk = b->d_tc_check;
     unsigned long long *stats = reinterpret_cast<unsigned long long *>(b->d_tc_check + 4);
     if (check) {
@@ -1076,6 +1041,8 @@ int launch_wgmma(psb_batch_t *b, const float *d_feats, long long total, const in
     while (tpc < 32 && (tiles / (tpc * 2)) * n_k >= (long long)n_sm * std::max(per_sm, 1) * 4) tpc *= 2;
     PSB_REQUIRE((tiles + tpc - 1) / tpc <= 65535, "too many frames for one launch of the tensor-core filter");
     const dim3 grid((unsigned)n_k, (unsigned)((tiles + tpc - 1) / tpc));
+    b->tc_last_tpc = tpc;
+    b->tc_last_ctas = grid.y;
     float *chk = b->d_tc_check;
     unsigned long long *stats = reinterpret_cast<unsigned long long *>(b->d_tc_check + 4);
     if (check) {
@@ -1211,9 +1178,9 @@ int psb_launch_ptm_tc(psb_batch_t *b, const float *d_feats, const int32_t *utt_o
         b->uttoff_cap = (size_t)n_utt + 1 + 64;
         PSB_CUDA(cudaMalloc(&b->d_uttoff, b->uttoff_cap * sizeof(int32_t)));
     }
-    if (!b->d_tc_check) {                                     // float[2] check values, then (16-byte offset) four 64-bit counters
-        PSB_CUDA(cudaMalloc(&b->d_tc_check, 64));
-        PSB_CUDA(cudaMemsetAsync(b->d_tc_check, 0, 64, b->stream));
+    if (!b->d_tc_check) {                                     // float[2] check values, then (16-byte offset) ST_N 64-bit counters
+        PSB_CUDA(cudaMalloc(&b->d_tc_check, TC_CHECK_BYTES));
+        PSB_CUDA(cudaMemsetAsync(b->d_tc_check, 0, TC_CHECK_BYTES, b->stream));
     }
     {
         // work list of the rows the filter leaves in doubt: room for a quarter of all (frame, pair) rows, 32 bytes each
@@ -1247,20 +1214,13 @@ int psb_launch_ptm_tc(psb_batch_t *b, const float *d_feats, const int32_t *utt_o
         }
     if (rc) return rc;
     const long long chains = (long long)n_utt * m->K;
-    static const bool thread_fixup = [] { const char *v = getenv("PSB_TC_FIXUP"); return v && !strcmp(v, "thread"); }();
-    if (thread_fixup)
-        ptm_fixup_kernel<13><<<(unsigned)((chains + 127) / 128), 128, 0, b->stream>>>(
-            d_feats, m->sumlen, d_featoff, b->d_uttoff, n_utt, m->d_rec, m->d_rec_off, b->d_topn, b->d_tc_flags, (long long)fw, m->K,
-            m->n_feat, m->n_density);
-    else {
-        const unsigned blocks = (unsigned)((chains * 32 + 127) / 128);
+    const unsigned blocks = (unsigned)((chains * 32 + 127) / 128);
 #define PSB_FIXW(NDW) ptm_fixup_warp_kernel<13, NDW><<<blocks, 128, 0, b->stream>>>(d_feats, m->sumlen, d_featoff, b->d_uttoff, n_utt, \
-            m->d_rec, m->d_rec_off, b->d_topn, b->d_tc_flags, (long long)fw, m->K, m->n_feat)
-        if (m->n_density == 256) PSB_FIXW(8);
-        else if (m->n_density == 128) PSB_FIXW(4);
-        else PSB_FIXW(2);
+        m->d_rec, m->d_rec_off, b->d_topn, b->d_tc_flags, (long long)fw, m->K, m->n_feat)
+    if (m->n_density == 256) PSB_FIXW(8);
+    else if (m->n_density == 128) PSB_FIXW(4);
+    else PSB_FIXW(2);
 #undef PSB_FIXW
-    }
     PSB_LAUNCH_CHECK();
     return PSB_OK;
 }
@@ -1280,5 +1240,23 @@ extern "C" int psb_batch_tc_check(psb_batch_t *b, float *ratio, int32_t *max_can
     memcpy(ratio, h, 4);
     memcpy(max_candidates, h + 4, 4);
     if (stats4) memcpy(stats4, h + 16, 32);
+    return PSB_OK;
+}
+
+// debug (PSB_TC_CHECK=1): the filter's decision-path counters (include/psb200.h lists them), then the last launch's
+// tiles per CTA and CTAs per pair; the first min(n, PSB_TC_N_COUNTERS) values go to out
+extern "C" int psb_batch_tc_counters(psb_batch_t *b, int64_t *out, int32_t n)
+{
+    PSB_REQUIRE(b && (out || n == 0) && n >= 0, "psb_batch_tc_counters: bad argument");
+    static_assert(ST_N + 2 == PSB_TC_N_COUNTERS, "psb200.h lists every counter");
+    int64_t v[PSB_TC_N_COUNTERS] = {0};
+    if (b->d_tc_check) {
+        PSB_CUDA(cudaSetDevice(b->m->device));
+        PSB_CUDA(cudaStreamSynchronize(b->stream));
+        PSB_CUDA(cudaMemcpy(v, reinterpret_cast<unsigned char *>(b->d_tc_check) + 16, 8 * ST_N, cudaMemcpyDeviceToHost));
+    }
+    v[ST_N] = b->tc_last_tpc;
+    v[ST_N + 1] = b->tc_last_ctas;
+    memcpy(out, v, sizeof(int64_t) * (size_t)std::min<int32_t>(n, PSB_TC_N_COUNTERS));
     return PSB_OK;
 }

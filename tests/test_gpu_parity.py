@@ -197,9 +197,14 @@ def _batch_vs_oracle(api, pm, feats_by_utt):
     b = api.Batch(m, len(lens) + 1, sum(lens) + 8)
     off = api.Batch.offsets(lens)
     scr = b.score_host(np.concatenate(feats_by_utt), off)
+    rec = b.get_topn(int(off[-1])) if pm.kind == "ptm" else None
     om = oracle.OracleModel(pm)
     for u, f in enumerate(feats_by_utt):
-        want = om.score_utt(f)
+        if rec is not None and len(f):
+            want, raw = om.score_utt(f, want_raw=True)
+            oracle.assert_records_equal(rec[off[u]:off[u + 1]], oracle.ptm_records(raw), "utt %d" % u)
+        else:
+            want = om.score_utt(f)
         got = scr[off[u]:off[u + 1]]
         bad = np.argwhere(got != want)
         assert bad.size == 0, "utt %d: first mismatch (frame, senone) %s: got %s want %s" % (
@@ -370,6 +375,8 @@ def test_topn_kernel_variants(api, en_us_dev, variant, monkeypatch):
     g = golden("en_us_goforward.npz")
     b = api.Batch(en_us_dev, 4, 1024)
     assert np.array_equal(b.score_host(g["feats"], np.array([0, 278], np.int32)), g["senscr"])
+    _, raw = oracle.OracleModel(en_us_dev.pm).score_utt(g["feats"], want_raw=True)
+    oracle.assert_records_equal(b.get_topn(278), oracle.ptm_records(raw), "en-us")
     b.close()
     # (2) BASELINE shape, ragged batch of 70 utterances (3 lane groups: an odd group count, padding
     #     lanes, zero-length utterances)
@@ -389,22 +396,18 @@ def test_topn_kernel_variants(api, en_us_dev, variant, monkeypatch):
 
 
 TC_CHECK = r"""
-import sys, json, numpy as np
-sys.path.insert(0, %r)
-sys.path.insert(0, %r)
+import json, numpy as np
+import tc_cases as tc
 from conftest import golden
 from oracle import oracle
 from pocketsphinx_b200 import api
 from pocketsphinx_b200.model import PackedModel, quantize_for_ties, synth_feats, synth_ptm
 out = {}
 def run(name, pm, chunks):
-    m = api.Model(pm); lens = [len(c) for c in chunks]; off = api.Batch.offsets(lens)
-    b = api.Batch(m, len(chunks) + 1, int(off[-1]) + 1)
-    scr = b.score_host(np.concatenate(chunks), off)
-    om = oracle.OracleModel(pm)
-    ok = all(np.array_equal(scr[off[u]:off[u + 1]], om.score_utt(c)) for u, c in enumerate(chunks) if len(c))
+    m = api.Model(pm); b = api.Batch(m, len(chunks) + 1, sum(len(c) for c in chunks) + 1)
+    tc.score_vs_oracle(api, oracle, pm, chunks, batch=b)          # scores and top-N records, or an AssertionError
     r, n = b.tc_check()
-    out[name] = {"identical": bool(ok), "ratio": float(r), "max_candidates": int(n), "stats": b.tc_stats}
+    out[name] = {"ratio": float(r), "max_candidates": int(n), "stats": b.tc_stats}
     b.close(); m.close()
 g = golden("en_us_goforward.npz")
 run("en_us", PackedModel.load(%r), [g["feats"]])
@@ -423,20 +426,14 @@ def test_tensor_core_filter_error_bound_holds_on_the_device(impl):
     distance and reports the worst |a - d| / eps (the bound the candidate selection relies on must hold
     with room to spare: the analysis in psb_ptm_tc.cu allows 0.8 of eps), on the shipped model with real
     features, the BASELINE shape, features scaled far outside the model's range and tie-stress data; for the
-    warpgroup-MMA kernel (wgmma, the default) and for the legacy mma.sync variant (PSB_TC_IMPL=mma)."""
-    import json
+    warpgroup-MMA kernel (wgmma, the default) and for the legacy mma.sync variant (PSB_TC_IMPL=mma).  Scores and
+    top-N records match the oracle in the same runs."""
     import os
-    import subprocess
-    import sys
-    from conftest import GOLDEN, ROOT
-    code = TC_CHECK % (ROOT, os.path.join(ROOT, "tests"), os.path.join(GOLDEN, "en_us_ptm_model.npz"))
-    r = subprocess.run([sys.executable, "-c", code], env=dict(os.environ, PSB_TC_CHECK="1", PSB_TOPN_VARIANT="6", PSB_TC_IMPL=impl),
-                       capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stderr[-3000:]
-    out = json.loads(r.stdout.strip().splitlines()[-1])
+    import tc_cases as tc
+    from conftest import GOLDEN
+    out = tc.child(TC_CHECK % os.path.join(GOLDEN, "en_us_ptm_model.npz"), impl)
     print(out)
     for name, v in out.items():
-        assert v["identical"], name
         assert 0.0 <= v["ratio"] < 0.8, (name, v)
         assert v["max_candidates"] >= 5, (name, v)
 

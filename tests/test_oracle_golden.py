@@ -15,6 +15,47 @@ def test_ptm_goforward_bit_exact(en_us):
     assert np.array_equal(topn[0], g["topn_first"]) and np.array_equal(topn[-1], g["topn_last"])
 
 
+def test_ptm_raw_lists_normalise_to_the_reference_lists(en_us):
+    """The lists before ptm_norm (what the device's records hold) give, normalised, exactly the lists the
+    reference hands out -- the en-us golden's first and last frame included -- and the same scores."""
+    from pocketsphinx_b200.model import synth_feats, synth_ptm
+    g = golden("en_us_goforward.npz")
+    om = oracle.OracleModel(en_us)
+    scr, topn, raw = om.score_utt(g["feats"], want_topn=True, want_raw=True)
+    assert np.array_equal(scr, g["senscr"])
+    norm = oracle.ptm_norm_raw(raw)
+    assert np.array_equal(norm, topn)
+    assert np.array_equal(norm[0], g["topn_first"]) and np.array_equal(norm[-1], g["topn_last"])
+    assert np.array_equal(raw[..., 0], topn[..., 0])
+    s = raw[..., 1]
+    assert (s[..., :-1] >= s[..., 1:]).all() and (s < 0).all()            # descending integer distances
+    for ds in (1, 2):
+        pm = synth_ptm(seed=4, n_density=64, n_sen=300)
+        pm.ds_ratio = ds
+        f = synth_feats(pm, 1, 30, seed=1)[0]
+        om = oracle.OracleModel(pm)
+        scr, topn, raw = om.score_utt(f, want_topn=True, want_raw=True)
+        assert np.array_equal(oracle.ptm_norm_raw(raw), topn) and np.array_equal(scr, om.score_utt(f))
+
+
+def test_ptm_records_layout():
+    """ptm_records packs {s0 >> 10, codeword bytes, min(255, offsets) bytes, 0}; assert_records_equal names the
+    first differing (frame, pair) and field."""
+    raw = np.zeros((2, 1, 2, 4, 2), np.int32)
+    raw[0, 0, 0] = [[7, -1025], [255, -2047], [0, -2048], [9, -400000]]
+    raw[0, 0, 1] = [[1, -1], [2, -2], [3, -3], [4, -1025]]
+    raw[1] = raw[0]
+    rec = oracle.ptm_records(raw)
+    assert rec.shape == (2, 2, 4)
+    assert rec[0, 0].view(np.uint32).tolist() == [(-2) & 0xffffffff, 0x0900ff07, 0xff000000, 0]
+    assert rec[0, 1].view(np.uint32).tolist() == [(-1) & 0xffffffff, 0x04030201, 0x01000000, 0]
+    oracle.assert_records_equal(rec, rec.copy())
+    bad = rec.copy()
+    bad[1, 1, 1] ^= np.int32(-0x80000000)                       # top codeword byte: compared as uint32
+    with pytest.raises(AssertionError, match="frame 1, pair 1: field codewords"):
+        oracle.assert_records_equal(bad, rec)
+
+
 def test_ptm_active_lists(en_us):
     g = golden("en_us_active.npz")
     gf = golden("en_us_goforward.npz")
