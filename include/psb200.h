@@ -143,9 +143,9 @@ int psb_batch_event_elapsed_ms(psb_batch_t *b, float *ms);
 int psb_batch_tc_check(psb_batch_t *b, float *ratio, int32_t *max_candidates, int64_t *stats4);
 /* debugging (PSB_TC_CHECK=1): which decisions the tensor-core filter took over everything this batch has scored.
  * out[0..n-1] receives the first n of, in order: the four stats4 values; rows with more than 18 candidates
- * (the filter kernel's per-row list capacity); rows where one lane of the wgmma filter stored more than 18 column
- * pairs; rows in doubt rescored inside the wgmma filter kernel because its work list was full, with a candidate
- * list and over all codewords; rows in doubt whose candidate list the wgmma filter's two threads per row both
+ * (the filter kernel's per-row list capacity); rows where one lane of the filter stored more than 18 column
+ * pairs; rows in doubt rescored inside the filter kernel because its work list was full, with a candidate
+ * list and over all codewords; rows in doubt whose candidate list the filter's two threads per row both
  * wrote; rows with a candidate list that failed the gap test, the >> 10 agreement test, the sign guard and the
  * saturation guard (one row can fail several); then, without PSB_TC_CHECK too, the last filter launch's tiles per
  * CTA and its CTAs per codebook-stream pair. */

@@ -182,7 +182,7 @@ extern "C" int psb_model_create(const psb_model_desc_t *d, int device, psb_model
     m->has_topn_beam = false;
     m->d_topn_beam = nullptr;
     m->tc_ok = false;
-    m->d_tc_wfrag = m->d_tc_wumma = m->d_tc_cen = m->d_tc_bnd = nullptr;
+    m->d_tc_wumma = m->d_tc_cen = m->d_tc_bnd = nullptr;
     m->d_msT = m->d_msdetT = nullptr; m->d_featlen = m->d_featoff = nullptr;
     for (int f = 0; f < PSB_MAX_FEAT; ++f) m->topn_beam[f] = 0;
     const bool dev = d->on_device != 0;
@@ -270,8 +270,6 @@ extern "C" int psb_model_create(const psb_model_desc_t *d, int device, psb_model
             uint8_t t[256];
             if (cudaMemcpy(t, m->d_logadd8, 256, cudaMemcpyDeviceToHost) == cudaSuccess)
                 for (int i = 0; i < 256; ++i) m->logadd8_max = std::max<int>(m->logadd8_max, t[i]);
-                m->logadd8_zero_from = 256;
-                while (m->logadd8_zero_from > 0 && t[m->logadd8_zero_from - 1] == 0) --m->logadd8_zero_from;
         }
     }
     if (!rc && m->kind != PSB_KIND_MS && !d->logadd8) {
@@ -312,7 +310,7 @@ extern "C" void psb_model_free(psb_model_t *m)
     cudaFree(m->d_rec); cudaFree(m->d_rec_off); cudaFree(m->d_rec2); cudaFree(m->d_rec2_off); cudaFree(m->d_mixw); cudaFree(m->d_mixw_cb);
     cudaFree(m->d_sen2cb); cudaFree(m->d_sen2cb32); cudaFree(m->d_quadcb); cudaFree(m->d_bsen); cudaFree(m->d_logadd8); cudaFree(m->d_logadd_ms);
     cudaFree(m->d_topn_beam); cudaFree(m->d_msT); cudaFree(m->d_msdetT); cudaFree(m->d_featlen); cudaFree(m->d_featoff);
-    cudaFree(m->d_tc_wfrag); cudaFree(m->d_tc_wumma); cudaFree(m->d_tc_cen); cudaFree(m->d_tc_bnd);
+    cudaFree(m->d_tc_wumma); cudaFree(m->d_tc_cen); cudaFree(m->d_tc_bnd);
     delete m;
 }
 
@@ -333,15 +331,20 @@ extern "C" int psb_model_device(const psb_model_t *m) { return m ? m->device : -
 extern "C" int psb_batch_create(psb_model_t *m, int32_t max_utts, int64_t max_frames, psb_batch_t **out)
 {
     PSB_REQUIRE(m && out && max_utts > 0 && max_frames > 0, "psb_batch_create: bad argument");
+    // top-N path (see psb_internal.cuh): a value that selects no kernel is an error rather than the default, so that a
+    // run never times the default under another kernel's name
+    const char *v = getenv("PSB_TOPN_VARIANT"), *impl = getenv("PSB_TC_IMPL");
+    PSB_REQUIRE(!v || (strlen(v) == 1 && strchr("023456", v[0])),
+                "psb_batch_create: PSB_TOPN_VARIANT=%s; accepted values are 0, 2, 3, 4, 5 and 6 (default)", v);
+    PSB_REQUIRE(!impl || !strcmp(impl, "wgmma"), "psb_batch_create: PSB_TC_IMPL=%s; the only accepted value is wgmma", impl);
     PSB_CUDA(cudaSetDevice(m->device));
     psb_batch_t *b = new psb_batch_t();      // value-initialised: all pointers null, counters zero
     b->m = m;
     b->max_utts = max_utts;
     b->max_frames = max_frames;
     {
-        // tuning knob; default = tensor-core filter + exact rescoring (psb_ptm_tc.cu) where the model allows it,
+        // default 6 = tensor-core filter + exact rescoring (psb_ptm_tc.cu) where the model allows it,
         // else codeword pairs with deferred insertion (ptm_topnq_kernel, variant 5)
-        const char *v = getenv("PSB_TOPN_VARIANT");
         b->topn_variant = v ? atoi(v) : 6;
         const char *p = getenv("PSB_PIPELINE");         // sub-batches in flight for psb_decode_batch_*
         b->n_pipe = p ? atoi(p) : 0;                   // 0 = auto (see decode_common)

@@ -283,8 +283,8 @@ ptm_topn_kernel(const float *__restrict__ rec, const size_t *__restrict__ rec_of
     }
 }
 
-template <int FL, bool SEMI, int WARPS, int MINB>
-__global__ void __launch_bounds__(WARPS * 32, MINB)
+template <int FL, bool SEMI>
+__global__ void __launch_bounds__(TOPN_WARPS * 32, 7)
 ptm_topn2_kernel(const float *__restrict__ rec2, const size_t *__restrict__ rec2_off,
                  const int32_t *__restrict__ klist, const float *__restrict__ featT, GroupTabs tabs,
                  int4 *__restrict__ out, int n_groups, int nd, int n_feat, int D,
@@ -302,7 +302,7 @@ ptm_topn2_kernel(const float *__restrict__ rec2, const size_t *__restrict__ rec2
             srec[i] = src[i];
     }
     __syncthreads();
-    const int g = blockIdx.y * WARPS + warp;
+    const int g = blockIdx.y * TOPN_WARPS + warp;
     if (g >= n_groups) return;
     const int len = tabs.lane_len[g * 32 + lane];
     const long long off = tabs.lane_off[g * 32 + lane];
@@ -1167,10 +1167,6 @@ semi_senone_kernel(const int4 *__restrict__ topn, const uint8_t *__restrict__ mi
 // owns senones 4q..4q+3 fetches each weight row with ONE aligned 32-bit load (four senones'
 // bytes) and reads the codebook's offsets/scores once; quads that straddle a codebook boundary
 // (a few per cent) take the per-senone path.
-// TAB2: the add table is zero from entry 31 on (every logbase-1.0001 >> 10 table is), so the two look-ups of a packed
-// log-add -- tab[d_lo] and tab[d_hi] -- become ONE 32-bit read of a 32 x 32 table of ready-made halfword pairs indexed
-// by the two differences clamped to 31: half the shared-memory instructions of the loop (its limit: LSU data pipe 84 %).
-template <bool TAB2>
 __global__ void __launch_bounds__(512)
 ptm_senone4_kernel(const int4 *__restrict__ topn, const uint8_t *__restrict__ mixw,
                    const uint16_t *__restrict__ sen2cb, const int16_t *__restrict__ quadcb,
@@ -1187,13 +1183,10 @@ ptm_senone4_kernel(const int4 *__restrict__ topn, const uint8_t *__restrict__ mi
     int *red = norm + 8;                                            // [32]
     uint8_t *tab = reinterpret_cast<uint8_t *>(red + 32);           // [PSB_LOGADD8_N]
     int16_t *asc = reinterpret_cast<int16_t *>(tab + PSB_LOGADD8_N + 16);     // [n_sen rounded up to 4]
-    unsigned *tab2 = reinterpret_cast<unsigned *>(asc + ((n_sen + 7) & ~7));  // [32 * 32] (TAB2 only)
     const long long frame = blockIdx.x;
     const int tid = threadIdx.x;
 
     for (int i = tid; i < PSB_LOGADD8_N; i += blockDim.x) tab[i] = logadd_tab[i];
-    if (TAB2)
-        for (int i = tid; i < 1024; i += blockDim.x) tab2[i] = (unsigned)logadd_tab[i & 31] | ((unsigned)logadd_tab[i >> 5] << 16);
     if (tid < n_feat) norm[tid] = PSB_WORST_SCORE;
     __syncthreads();
     int4 r = make_int4(0, 0, 0, 0);
@@ -1245,13 +1238,7 @@ ptm_senone4_kernel(const int4 *__restrict__ topn, const uint8_t *__restrict__ mi
                 const unsigned mn = __viaddmin_u16x2(y, nvj, x);                                \
                 const unsigned mx = __viaddmax_u16x2(y, nvj, x);                                \
                 const unsigned d = mx - mn;                                                     \
-                unsigned t;                                                                     \
-                if (TAB2) {                                                                     \
-                    const unsigned dc = __vminu2(d, 0x001f001fu);                               \
-                    t = tab2[(dc & 0x1fu) | (dc >> 11)];                                        \
-                }                                                                               \
-                else                                                                            \
-                    t = (unsigned)tab[d & 0xffffu] | ((unsigned)tab[d >> 16] << 16);            \
+                const unsigned t = (unsigned)tab[d & 0xffffu] | ((unsigned)tab[d >> 16] << 16); \
                 x = mn - t;                                                                     \
             }
             PSB_LADD2(x01, w1, 0x4140, nv.y) PSB_LADD2(x23, w1, 0x4342, nv.y)
@@ -1298,19 +1285,19 @@ ptm_senone4_kernel(const int4 *__restrict__ topn, const uint8_t *__restrict__ mi
         dst[s] = (int16_t)(asc[s] - best);                       // ptm_mgau.c:398-400
 }
 
-template <int FL, bool SEMI, int WARPS, int MINB>
+template <int FL, bool SEMI>
 int launch_topn2(psb_batch_t *b, const int32_t *d_klist, int n_k, const GroupTabs &tabs, int n_groups,
                  const int32_t *d_featoff)
 {
     psb_model_t *m = b->m;
     constexpr int RECF2 = (2 + 4 * FL + 3) / 4 * 4;
     size_t smem = (size_t)(m->n_density / 2) * RECF2 * sizeof(float);
-    auto kern = ptm_topn2_kernel<FL, SEMI, WARPS, MINB>;
+    auto kern = ptm_topn2_kernel<FL, SEMI>;
     PSB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    dim3 grid(n_k, (n_groups + WARPS - 1) / WARPS);
-    kern<<<grid, WARPS * 32, smem, b->stream>>>(m->d_rec2, m->d_rec2_off, d_klist, b->d_featT, tabs, b->d_topn, n_groups,
-                                               m->n_density, m->n_feat, m->sumlen, d_featoff, m->K, m->ds_ratio,
-                                               m->d_topn_beam);
+    dim3 grid(n_k, (n_groups + TOPN_WARPS - 1) / TOPN_WARPS);
+    kern<<<grid, TOPN_WARPS * 32, smem, b->stream>>>(m->d_rec2, m->d_rec2_off, d_klist, b->d_featT, tabs, b->d_topn, n_groups,
+                                                    m->n_density, m->n_feat, m->sumlen, d_featoff, m->K, m->ds_ratio,
+                                                    m->d_topn_beam);
     PSB_LAUNCH_CHECK();
     return PSB_OK;
 }
@@ -1372,12 +1359,8 @@ int launch_topn(psb_batch_t *b, const int32_t *d_klist, int n_k, const GroupTabs
         PSB_LAUNCH_CHECK();
         return PSB_OK;
     }
-    if (FL <= 16 && m->d_rec2 && b->topn_variant != 0) {
-        // codeword-pair kernels (FL <= 16 keeps the register budget): variant 1 = 2 warps/CTA with a
-        // large register budget (two balanced waves), variant 2 = 4 warps/CTA at 72 registers
-        if (b->topn_variant != 1) return launch_topn2<FL <= 16 ? FL : 1, SEMI, 4, 7>(b, d_klist, n_k, tabs, n_groups, d_featoff);
-        return launch_topn2<FL <= 16 ? FL : 1, SEMI, 2, 7>(b, d_klist, n_k, tabs, n_groups, d_featoff);
-    }
+    if (FL <= 16 && m->d_rec2 && b->topn_variant != 0)      // codeword pairs, 4 warps/CTA (FL <= 16 keeps the register budget)
+        return launch_topn2<FL <= 16 ? FL : 1, SEMI>(b, d_klist, n_k, tabs, n_groups, d_featoff);
     size_t smem = (size_t)m->n_density * rec_floats(FL) * sizeof(float);
     PSB_CUDA(cudaFuncSetAttribute(ptm_topn_kernel<FL, SEMI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     // few (pair, group) items (semi-continuous models, small batches): one warp per CTA spreads
@@ -1693,21 +1676,8 @@ int psb_launch_ptm_batch(psb_batch_t *b, const float *d_feats, const int32_t *ut
             // at least 256 threads (log-add table staging) and one thread per (codebook, stream) pair
             const int threads = std::min(512, std::max(std::max(256, roundup(K, 32)), roundup((n_quads + iters - 1) / iters, 32)));
             const size_t smem4 = smem + 8 + (size_t)K * 16;
-            // experiment, off by default: the 4 KB two-index table trades two mostly-broadcast byte reads for one read
-            // that bank-conflicts across 1024 words (bit-identical either way)
-            static const bool use_tab2 = getenv("PSB_SENONE_TAB2") && atoi(getenv("PSB_SENONE_TAB2")) == 1;
-            if (m->logadd8_zero_from <= 31 && use_tab2) {
-                const size_t smem5 = smem4 + 16 + 4096;
-                PSB_CUDA(cudaFuncSetAttribute(ptm_senone4_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem5));
-                ptm_senone4_kernel<true><<<(unsigned)total, threads, smem5, b->stream>>>(
-                    b->d_topn, m->d_mixw, m->d_sen2cb, m->d_quadcb, m->d_bsen, m->n_bsen, m->d_logadd8, d_senscr, m->n_sen,
-                    m->n_feat, m->n_density, K, m->mixw_stride);
-                PSB_LAUNCH_CHECK();
-                if (b->have_ev) PSB_CUDA(cudaEventRecord(b->ev[3], b->stream));
-                return PSB_OK;
-            }
-            PSB_CUDA(cudaFuncSetAttribute(ptm_senone4_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem4));
-            ptm_senone4_kernel<false><<<(unsigned)total, threads, smem4, b->stream>>>(
+            PSB_CUDA(cudaFuncSetAttribute(ptm_senone4_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem4));
+            ptm_senone4_kernel<<<(unsigned)total, threads, smem4, b->stream>>>(
                 b->d_topn, m->d_mixw, m->d_sen2cb, m->d_quadcb, m->d_bsen, m->n_bsen, m->d_logadd8, d_senscr, m->n_sen,
                 m->n_feat, m->n_density, K, m->mixw_stride);
         }

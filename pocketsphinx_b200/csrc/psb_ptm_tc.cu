@@ -22,20 +22,19 @@
 //      codebook's mean centre) the exponent d = det - sum_j v_j (y_j - mu'_j)^2 is the inner product
 //      of X = (y_j^2, y_j, 1) with W_c = (-v_cj, 2 v_cj mu'_cj, det_c - sum_j v_cj mu'_cj^2): one
 //      [frames x 32] x [32 x n_density] GEMM per pair on the tensor cores, as 3 x TF32 (lo*hi + hi*lo
-//      + hi*hi; W is split into TF32 halves on the host): warpgroup MMA (ptm_wgmma_kernel, the
-//      default) or mma.sync m16n8k8 (ptm_tc_kernel, PSB_TC_IMPL=mma).  Its result a_c differs from the
-//      reference's float d_c by at most eps = ERR * (sum_j Amax_j y_j^2 + Bmax_j |y_j| + Cmax), a
-//      bound every row computes for itself (Amax/Bmax/Cmax: per-pair maxima of |W| entries).  Five
-//      distinct codewords with a_c >= L0 (wgmma: the fifth largest of eight group maxima of the row;
-//      mma.sync: the four per-lane row maxima and the best runner-up half maximum) give the integer
-//      L' = floor(L0 - eps) - 1 <= s(5) - 1, and every codeword with s_c >= s(5) has d_c > L', hence
-//      a_c >= L' - eps: the candidate set C (about seven of 256 on the BASELINE shape).
+//      + hi*hi; W is split into TF32 halves on the host) with warpgroup MMA (ptm_wgmma_kernel).
+//      Its result a_c differs from the reference's float d_c by at most
+//      eps = ERR * (sum_j Amax_j y_j^2 + Bmax_j |y_j| + Cmax), a bound every row computes for itself
+//      (Amax/Bmax/Cmax: per-pair maxima of |W| entries).  Five distinct codewords with a_c >= L0 (the
+//      fifth largest of eight group maxima of the row) give the integer L' = floor(L0 - eps) - 1 <= s(5) - 1,
+//      and every codeword with s_c >= s(5) has d_c > L', hence a_c >= L' - eps: the candidate set C
+//      (about seven of 256 on the BASELINE shape).
 //
 // A row is then decided from the filter values alone when its five largest a_c are more than 2 eps + 1
 // apart and the `>> 10` of the four best is the same at both ends of [a - eps, a + eps]: the record
 // is certain without one exact distance.  Otherwise the row's candidate codewords (all of them when
-// C has more than TC_CAP members) get the reference's exact float arithmetic, one thread per row:
-// in ptm_wgmma_kernel's work list served by ptm_tc_exact_kernel, in ptm_tc_kernel itself.
+// C has more than TC_CAP members) get the reference's exact float arithmetic, one thread per row, from
+// ptm_wgmma_kernel's work list served by ptm_tc_exact_kernel.
 //
 // Nothing here is approximate in its output: tests/test_gpu_parity.py compares every record with the
 // oracle's lists, PSB_TC_CHECK=1 makes the filter kernel measure max |a_c - d_c| / eps on the device.
@@ -48,10 +47,9 @@
 
 namespace {
 
-constexpr int TC_ROWS = 128;          // frames per CTA (4 warps x 2 m-tiles x 16 rows)
+constexpr int TC_ROWS = 128;          // frames per CTA and tile (2 warpgroups x 64 rows)
 constexpr int TC_K = 32;              // GEMM depth: 2 * FL + 1 <= 32
-constexpr int TC_XS = 36;             // row pitch of the X tile in floats (conflict-free fragment loads)
-constexpr int TC_CAP = 18;            // candidate slots per row: the row's X storage, 144 B / 8 B
+constexpr int TC_CAP = 18;            // candidate codewords per row: the byte list a work-list item carries
 constexpr float TC_ERR = 1.0f / 262144.f;  // 2^-18 of the magnitude sum S: 3 x TF32 leaves 3 * 2^-22 per product, the rest is
                                            // room for the tensor core's fp32 accumulation (<= 2^-23 per step assumed, 12 steps per
                                            // chain) and the reference's own 52 roundings; PSB_TC_CHECK=1 measures what is used of it
@@ -60,9 +58,9 @@ constexpr float TC_ERR = 1.0f / 262144.f;  // 2^-18 of the magnitude sum S: 3 x 
 enum {
     ST_ROWS, ST_FILTER_ALONE, ST_EXACT_DIST, ST_TIE_FLAGS,
     ST_OVER_CAP,                                   // rows with more than TC_CAP candidates
-    ST_LANE_OVER,                                  // wgmma: rows where one quad lane stored more than TC_CAP pairs
-    ST_FALLBACK_LISTED, ST_FALLBACK_ALL,           // wgmma: rows in doubt rescored in the filter kernel (work list full)
-    ST_SPLIT,                                      // wgmma: rows in doubt whose candidate bytes came from both threads
+    ST_LANE_OVER,                                  // rows where one quad lane stored more than TC_CAP pairs
+    ST_FALLBACK_LISTED, ST_FALLBACK_ALL,           // rows in doubt rescored in the filter kernel (work list full)
+    ST_SPLIT,                                      // rows in doubt whose candidate bytes came from both threads
     ST_FAIL_GAP, ST_FAIL_STRADDLE, ST_FAIL_SIGN, ST_FAIL_SAT,   // listed rows failing each certainty test
     ST_N
 };
@@ -73,13 +71,6 @@ __device__ __forceinline__ float to_tf32(float x)
     unsigned r;
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
     return __uint_as_float(r);
-}
-
-__device__ __forceinline__ void mma_tf32(float (&d)[4], const unsigned (&a)[4], float b0, float b1)
-{
-    asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(__float_as_uint(b0)), "r"(__float_as_uint(b1)));
 }
 
 struct Top5 {
@@ -113,282 +104,8 @@ __device__ __forceinline__ void top5_insert(Top5 &t, int s, int c)
     if (t.n < 5) ++t.n;
 }
 
-// Filter + resolution for one (pair, 128-frame tile).
-//   wfrag   [K][2][NT][4][32] float2   W (high, then low TF32 halves) in mma B-fragment order:
-//                                      b0 = W[8 ks + t][8 n + g], b1 = W[8 ks + t + 4][8 n + g]
-//   cen     [K][16]                    centre m
-//   bnd     [K][32]                    Amax[FL], Bmax[FL], Cmax at [2 FL]
-//   rec     scalar records {det, mu0, v0, ...} of the model (exact distances of ambiguous rows, read through L1/L2)
-//   flags   [K][flag_words]            bit (row & 31) of word row >> 5: frame must be redone by the fix-up
-//   check   (debug) float[2]: max over everything of |a_c - d_c| / eps, and of the candidate count
-//   stats   (debug) unsigned long long[4]: rows, rows resolved from the filter alone, exact distances, tie flags
-template <int FL, int NT, bool CHECK>
-__global__ void __launch_bounds__(TC_ROWS, 4)
-ptm_tc_kernel(const float *__restrict__ feats, long long total, int D, const int32_t *__restrict__ featoff,
-              const int32_t *__restrict__ klist, const float2 *__restrict__ wfrag, const float *__restrict__ cen,
-              const float *__restrict__ bnd, const float *__restrict__ rec, const size_t *__restrict__ rec_off,
-              int4 *__restrict__ out, unsigned *__restrict__ flags, long long flag_words, int K, int n_feat,
-              float *__restrict__ check, unsigned long long *__restrict__ stats)
-{
-    constexpr int ND = NT * 8;
-    constexpr int RF = (1 + 2 * FL + 3) / 4 * 4;
-    constexpr unsigned FULL = 0xffffffffu;
-    static_assert(2 * FL + 1 <= TC_K, "stream too long for one 32-deep GEMM");
-    extern __shared__ __align__(16) unsigned char tc_smem[];
-    float2 *wf = reinterpret_cast<float2 *>(tc_smem);                                   // [NT][4][32]: high halves of W
-    float *xs = reinterpret_cast<float *>(tc_smem + (size_t)NT * 4 * 32 * 8);           // [128][36]; later the candidate lists
-    unsigned *masks = reinterpret_cast<unsigned *>(xs + TC_ROWS * TC_XS);               // [128][8]
-    int *cnt = reinterpret_cast<int *>(masks + TC_ROWS * 8);                            // [128]
-    float *epsr = reinterpret_cast<float *>(cnt + TC_ROWS);                             // [128]
-
-    const int k = klist[blockIdx.y];
-    const int f = k % n_feat;
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const long long row = (long long)blockIdx.x * TC_ROWS + tid;
-    const bool valid = row < total;
-
-    // ---- stage W (both halves), build this thread's X row (fp32: split into TF32 halves at fragment load) ----
-    {
-        const float4 *src = reinterpret_cast<const float4 *>(wfrag + (size_t)k * 2 * NT * 4 * 32);
-        float4 *dst = reinterpret_cast<float4 *>(wf);
-        for (int i = tid; i < NT * 4 * 32 / 2; i += TC_ROWS) dst[i] = src[i];
-    }
-    float x[FL];
-    {
-        const float *p = feats + (valid ? row : 0) * D + featoff[f];
-        const float *m = cen + (size_t)k * 16, *bb = bnd + (size_t)k * 32;
-        float S = bb[2 * FL];
-        float *xr = xs + tid * TC_XS;
-#pragma unroll
-        for (int j = 0; j < FL; ++j) {
-            x[j] = valid ? p[j] : 0.f;
-            const float y = __fsub_rn(x[j], m[j]);
-            const float y2 = __fmul_rn(y, y);
-            xr[j] = y2;
-            xr[FL + j] = y;
-            S = __fadd_ru(S, __fmul_ru(bb[j], y2));
-            S = __fadd_ru(S, __fmul_ru(bb[FL + j], fabsf(y)));
-        }
-        xr[2 * FL] = 1.0f;
-#pragma unroll
-        for (int j = 2 * FL + 1; j < TC_K; ++j) xr[j] = 0.f;
-        epsr[tid] = __fadd_ru(__fmul_ru(S, TC_ERR), 2.0f);
-        cnt[tid] = 0;
-#pragma unroll
-        for (int w = 0; w < 8; ++w) masks[tid * 8 + w] = 0u;
-    }
-    __syncthreads();
-
-    // ---- 3 x TF32 GEMM (lo*hi + hi*lo + hi*hi) of this warp's 32 rows against all codewords, 16 rows at a time.
-    // The accumulators are never held for all codewords at once: a first sweep over chunks of CH n-tiles keeps only
-    // the row maxima that give the threshold, a second sweep recomputes the same chunks (bit-identical: same
-    // instructions, same order) and extracts the few columns above it.  The tensor pipe has the room (< 10 % busy
-    // with one sweep); 40 accumulator registers instead of 128 double the resident warps. ----
-    constexpr int CH = NT <= 8 ? NT / 2 : 8;             // at least two chunks: the two half maxima per lane come from different chunks
-    const int g = lane >> 2, t = lane & 3;
-    uint2 *lists = reinterpret_cast<uint2 *>(xs);            // row r: slots at (r * TC_XS floats) .. + TC_CAP
-    const float2 *wlo = wfrag + ((size_t)k * 2 + 1) * NT * 4 * 32;      // low halves of W: from L1 / L2, same fragment order
-#pragma unroll 1
-    for (int mt = 0; mt < 2; ++mt) {
-        unsigned ah[4][4], al[4][4];
-        {
-            const float *xa = xs + (warp * 32 + mt * 16 + g) * TC_XS, *xb = xa + 8 * TC_XS;
-#pragma unroll
-            for (int ks = 0; ks < 4; ++ks) {
-                const float v[4] = {xa[8 * ks + t], xb[8 * ks + t], xa[8 * ks + t + 4], xb[8 * ks + t + 4]};
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    const float h = to_tf32(v[q]);
-                    ah[ks][q] = __float_as_uint(h);
-                    al[ks][q] = __float_as_uint(to_tf32(__fsub_rn(v[q], h)));
-                }
-            }
-        }
-        __syncwarp();                                        // this m-tile's X rows now become their candidate lists
-        auto chunk = [&](int n0, float (&acc)[CH][4]) {
-#pragma unroll
-            for (int i = 0; i < CH; ++i) {
-                const int n = n0 + i;
-                acc[i][0] = acc[i][1] = acc[i][2] = acc[i][3] = 0.f;
-#pragma unroll
-                for (int ks = 0; ks < 4; ++ks) {             // the small cross terms first
-                    const float2 bh = wf[(n * 4 + ks) * 32 + lane], bl = __ldg(wlo + (n * 4 + ks) * 32 + lane);
-                    mma_tf32(acc[i], al[ks], bh.x, bh.y);
-                    mma_tf32(acc[i], ah[ks], bl.x, bl.y);
-                }
-#pragma unroll
-                for (int ks = 0; ks < 4; ++ks) {
-                    const float2 bh = wf[(n * 4 + ks) * 32 + lane];
-                    mma_tf32(acc[i], ah[ks], bh.x, bh.y);
-                }
-            }
-        };
-        // rows g (acc[.][0..1]) and g + 8 (acc[.][2..3]) of this m-tile: the lane's two half maxima each
-        const int r0 = warp * 32 + mt * 16 + g, r1 = r0 + 8;
-        float h00 = -INFINITY, h01 = -INFINITY, h10 = -INFINITY, h11 = -INFINITY;
-#pragma unroll 1
-        for (int n0 = 0; n0 < NT; n0 += CH) {
-            float acc[CH][4];
-            chunk(n0, acc);
-            float a = -INFINITY, b = -INFINITY;
-#pragma unroll
-            for (int i = 0; i < CH; ++i) { a = fmaxf(a, fmaxf(acc[i][0], acc[i][1])); b = fmaxf(b, fmaxf(acc[i][2], acc[i][3])); }
-            if (n0 < NT / 2) { h00 = fmaxf(h00, a); h10 = fmaxf(h10, b); }
-            else { h01 = fmaxf(h01, a); h11 = fmaxf(h11, b); }
-        }
-        float hi0 = fmaxf(h00, h01), lo0 = fminf(h00, h01), hi1 = fmaxf(h10, h11), lo1 = fminf(h10, h11);
-        // five distinct columns >= L0: the quad's four lane maxima and the best runner-up half maximum
-        hi0 = fminf(hi0, __shfl_xor_sync(FULL, hi0, 1)); hi0 = fminf(hi0, __shfl_xor_sync(FULL, hi0, 2));
-        lo0 = fmaxf(lo0, __shfl_xor_sync(FULL, lo0, 1)); lo0 = fmaxf(lo0, __shfl_xor_sync(FULL, lo0, 2));
-        hi1 = fminf(hi1, __shfl_xor_sync(FULL, hi1, 1)); hi1 = fminf(hi1, __shfl_xor_sync(FULL, hi1, 2));
-        lo1 = fmaxf(lo1, __shfl_xor_sync(FULL, lo1, 1)); lo1 = fmaxf(lo1, __shfl_xor_sync(FULL, lo1, 2));
-        const float e0 = epsr[r0], e1 = epsr[r1];
-        // L' = floor(L0 - eps) - 1, candidates: a_c >= L' - eps; every step rounded towards -inf
-        const float thr0 = __fsub_rd(__fsub_rd(floorf(__fsub_rd(fminf(hi0, lo0), e0)), 1.0f), e0);
-        const float thr1 = __fsub_rd(__fsub_rd(floorf(__fsub_rd(fminf(hi1, lo1), e1)), 1.0f), e1);
-        const float thr_min = fminf(thr0, thr1);
-        float worst = 0.f;
-#pragma unroll 1
-        for (int n0 = 0; n0 < NT; n0 += CH) {
-            float acc[CH][4];
-            chunk(n0, acc);
-#pragma unroll
-            for (int i = 0; i < CH; ++i) {
-                if (fmaxf(fmaxf(acc[i][0], acc[i][1]), fmaxf(acc[i][2], acc[i][3])) < thr_min) continue;
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    const float a = acc[i][q];
-                    if (a >= ((q & 2) ? thr1 : thr0)) {
-                        const int rr = (q & 2) ? r1 : r0, col = 8 * (n0 + i) + 2 * t + (q & 1);
-                        const int slot = atomicAdd(&cnt[rr], 1);
-                        if (slot < TC_CAP) lists[(size_t)rr * (TC_XS / 2) + slot] = make_uint2(__float_as_uint(a), (unsigned)col);
-                        atomicOr(&masks[rr * 8 + (col >> 5)], 1u << (col & 31));
-                    }
-                }
-            }
-            if (CHECK) {
-                // exact distances of every column this lane holds (debug only): |a - d| / eps
-                const float *rc = rec + rec_off[k];
-                for (int i = 0; i < CH; ++i)
-                    for (int q = 0; q < 4; ++q) {
-                        const int rr = (q & 2) ? r1 : r0, col = 8 * (n0 + i) + 2 * t + (q & 1);
-                        const long long grow = (long long)blockIdx.x * TC_ROWS + rr;
-                        if (grow >= total) continue;
-                        const float *px = feats + grow * D + featoff[f];
-                        const float *r = rc + (size_t)col * RF;
-                        float d = r[0];
-                        for (int j = 0; j < FL; ++j) {
-                            const float df = __fsub_rn(px[j], r[1 + 2 * j]);
-                            d = __fsub_rn(d, __fmul_rn(__fmul_rn(df, df), r[2 + 2 * j]));
-                        }
-                        worst = fmaxf(worst, __fdividef(fabsf(acc[i][q] - d), epsr[rr]));
-                    }
-            }
-        }
-        if (CHECK) atomicMax(reinterpret_cast<int *>(check), __float_as_int(worst));     // non-negative floats order like ints
-    }
-    __syncthreads();
-    if (!valid) return;
-
-    // ---- one thread per row: the record straight from the filter values when they leave no doubt ----
-    const int n = cnt[tid];
-    const float ee = epsr[tid];
-    if (CHECK) atomicMax(reinterpret_cast<int *>(check) + 1, n);
-    Top5 top;
-    top.n = 0; top.c = 0u; top.c4 = 0;
-#pragma unroll
-    for (int j = 0; j < 5; ++j) top.s[j] = INT_MIN;
-    bool certain = n <= TC_CAP;
-    if (CHECK && !certain) atomicAdd(stats + ST_OVER_CAP, 1ull);
-    if (certain) {
-        // the five largest a_c with their codewords (the list holds every a_c >= thr, at least five)
-        const uint2 *L = lists + (size_t)tid * (TC_XS / 2);
-        float a[5] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY, -INFINITY};
-        int c[5] = {0, 0, 0, 0, 0};
-        for (int i = 0; i < n; ++i) {
-            float v = __uint_as_float(L[i].x);
-            int cv = (int)L[i].y;
-#pragma unroll
-            for (int j = 0; j < 5; ++j)
-                if (v > a[j]) { const float tv = a[j]; const int tc = c[j]; a[j] = v; c[j] = cv; v = tv; cv = tc; }
-        }
-        // order and distinctness of the truncated scores: neighbours more than 2 eps + 1 apart, everything
-        // safely negative (truncation is towards zero); s >> 10 of the four best: the same at both ends of
-        // [a - eps, a + eps]
-        const float gap = __fadd_ru(__fadd_ru(ee, ee), 1.0f);
-        int qv[4];
-        bool gap_ok = true, straddle_ok = true;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            gap_ok &= __fsub_rd(a[j], a[j + 1]) > gap;
-            const int lo = __float2int_ru(__fsub_rd(a[j], ee)), hi = __float2int_ru(__fadd_ru(a[j], ee));
-            straddle_ok &= (lo >> PSB_SENSCR_SHIFT) == (hi >> PSB_SENSCR_SHIFT);
-            qv[j] = lo >> PSB_SENSCR_SHIFT;
-        }
-        const bool sign_ok = __fadd_ru(a[0], ee) < -2.0f, sat_ok = a[4] > -2.0e9f;
-        certain &= gap_ok && straddle_ok && sign_ok && sat_ok;
-        if (CHECK) {
-            if (!gap_ok) atomicAdd(stats + ST_FAIL_GAP, 1ull);
-            if (!straddle_ok) atomicAdd(stats + ST_FAIL_STRADDLE, 1ull);
-            if (!sign_ok) atomicAdd(stats + ST_FAIL_SIGN, 1ull);
-            if (!sat_ok) atomicAdd(stats + ST_FAIL_SAT, 1ull);
-        }
-        if (certain) {
-            unsigned cb = 0, eb = 0;
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                int ev = qv[0] - qv[j];
-                ev = ev > 255 ? 255 : ev;
-                cb |= (unsigned)c[j] << (8 * j);
-                eb |= (unsigned)ev << (8 * j);
-            }
-            out[row * K + k] = make_int4(qv[0], (int)cb, (int)eb, 0);
-            if (CHECK) { atomicAdd(stats, 1ull); atomicAdd(stats + 1, 1ull); }
-            return;
-        }
-    }
-    // ---- doubt: the reference's exact arithmetic for this row's candidates (few rows, few codewords each) ----
-    {
-        const float *rc = rec + rec_off[k];
-        int n_exact = 0;
-        auto exact = [&](int cw) {
-            const float4 *r4 = reinterpret_cast<const float4 *>(rc + (size_t)cw * RF);
-            const float d = gau_dist<FL>(r4, x);
-            top5_insert(top, f2i_clamped(d), cw);
-            ++n_exact;
-        };
-        if (n <= TC_CAP) {
-            const uint2 *L = lists + (size_t)tid * (TC_XS / 2);
-            // ascending codeword order is not needed: ties are redone by the fix-up
-            for (int i = 0; i < n; ++i) exact((int)L[i].y);
-        }
-        else {
-            for (int w = 0; w < ND / 32; ++w) {
-                unsigned bits = masks[tid * 8 + w];
-                while (bits) {
-                    const int b = __ffs(bits) - 1;
-                    bits &= bits - 1;
-                    exact(w * 32 + b);
-                }
-            }
-        }
-        const bool distinct = top.n >= 5 && top.s[0] > top.s[1] && top.s[1] > top.s[2] && top.s[2] > top.s[3] && top.s[3] > top.s[4];
-        const int tp = top.s[0] >> PSB_SENSCR_SHIFT;
-        unsigned eb = 0;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            int ev = tp - (top.s[j] >> PSB_SENSCR_SHIFT);
-            ev = ev > 255 ? 255 : ev;
-            eb |= (unsigned)ev << (8 * j);
-        }
-        out[row * K + k] = make_int4(tp, (int)top.c, (int)eb, 0);
-        if (!distinct) atomicOr(&flags[(size_t)k * flag_words + (row >> 5)], 1u << (row & 31));
-        if (CHECK) { atomicAdd(stats, 1ull); atomicAdd(stats + 2, (unsigned long long)n_exact); if (!distinct) atomicAdd(stats + 3, 1ull); }
-    }
-}
-
 // ---------------------------------------------------------------------------------------
-// The same filter on Hopper's warpgroup MMA: each warpgroup issues twelve wgmma.mma_async m64nNDk8 TF32 (lo*hi, hi*lo,
+// The filter on Hopper's warpgroup MMA: each warpgroup issues twelve wgmma.mma_async m64nNDk8 TF32 (lo*hi, hi*lo,
 // hi*hi over four K steps) per 64 frames, A (X rows split into TF32 halves) and B (W, both halves) straight from shared
 // memory in the canonical K-major no-swizzle layout, the fp32 accumulator in registers.  A frame's row is spread over the
 // four lanes of a quad: group maxima meet by shuffles; each lane then stores, without a branch or an atomic, the column
@@ -995,35 +712,6 @@ float round_tf32_host(float x)
     return r;
 }
 
-template <int FL, int NT>
-int launch_tc(psb_batch_t *b, const float *d_feats, long long total, const int32_t *d_klist, int n_k, const int32_t *d_featoff,
-              bool check)
-{
-    psb_model_t *m = b->m;
-    const size_t smem = (size_t)NT * 4 * 32 * 8 + (size_t)TC_ROWS * TC_XS * 4 + (size_t)TC_ROWS * 8 * 4 + TC_ROWS * 4 + TC_ROWS * 4;
-    const dim3 grid((unsigned)((total + TC_ROWS - 1) / TC_ROWS), (unsigned)n_k);
-    b->tc_last_tpc = 1;
-    b->tc_last_ctas = grid.x;
-    float *chk = b->d_tc_check;
-    unsigned long long *stats = reinterpret_cast<unsigned long long *>(b->d_tc_check + 4);
-    if (check) {
-        auto kern = ptm_tc_kernel<FL, NT, true>;
-        PSB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        kern<<<grid, TC_ROWS, smem, b->stream>>>(d_feats, total, m->sumlen, d_featoff, d_klist, reinterpret_cast<const float2 *>(m->d_tc_wfrag),
-                                                m->d_tc_cen, m->d_tc_bnd, m->d_rec, m->d_rec_off, b->d_topn, b->d_tc_flags,
-                                                (long long)b->tc_flag_words, m->K, m->n_feat, chk, stats);
-    }
-    else {
-        auto kern = ptm_tc_kernel<FL, NT, false>;
-        PSB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        kern<<<grid, TC_ROWS, smem, b->stream>>>(d_feats, total, m->sumlen, d_featoff, d_klist, reinterpret_cast<const float2 *>(m->d_tc_wfrag),
-                                                m->d_tc_cen, m->d_tc_bnd, m->d_rec, m->d_rec_off, b->d_topn, b->d_tc_flags,
-                                                (long long)b->tc_flag_words, m->K, m->n_feat, nullptr, nullptr);
-    }
-    PSB_LAUNCH_CHECK();
-    return PSB_OK;
-}
-
 template <int FL, int ND>
 int launch_wgmma(psb_batch_t *b, const float *d_feats, long long total, const int32_t *d_klist, int n_k, const int32_t *d_featoff,
                bool check)
@@ -1083,9 +771,9 @@ int psb_tc_prepare(psb_model_t *m, const float *hm, const float *hv, const float
     if (m->n_density != 64 && m->n_density != 128 && m->n_density != 256) return PSB_OK;
     for (int f = 0; f < m->n_feat; ++f)
         if (m->featlen[f] != 13) return PSB_OK;              // the kernels are instantiated for 13-dimensional streams
-    const int nd = m->n_density, NT = nd / 8, FL = 13, K = m->K;
-    std::vector<float> wf((size_t)K * 2 * NT * 4 * 32 * 2, 0.f), cen((size_t)K * 16, 0.f), bnd((size_t)K * 32, 0.f);
-    std::vector<float> wu((size_t)K * 2 * 8 * nd * 4, 0.f);     // canonical K-major layout of the wgmma path: [half][chunk][n][4]
+    const int nd = m->n_density, FL = 13, K = m->K;
+    std::vector<float> cen((size_t)K * 16, 0.f), bnd((size_t)K * 32, 0.f);
+    std::vector<float> wu((size_t)K * 2 * 8 * nd * 4, 0.f);     // canonical K-major layout of wgmma's B operand: [half][chunk][n][4]
     std::vector<double> W((size_t)TC_K * nd);
     for (int cb = 0; cb < m->n_mgau; ++cb)
         for (int f = 0; f < m->n_feat; ++f) {
@@ -1117,18 +805,6 @@ int psb_tc_prepare(psb_model_t *m, const float *hm, const float *hv, const float
             bb[2 * FL] = (float)(cmax * 1.0001);
             for (int j = 0; j < 2 * FL; ++j) bb[j] = std::nextafter(bb[j] * 1.0001f, INFINITY);
             // high and low TF32 halves of the fp32 value of every W entry: w = hi + lo + O(2^-22 w)
-            float *w = wf.data() + (size_t)k * 2 * NT * 4 * 32 * 2;
-            for (int n = 0; n < NT; ++n)
-                for (int ks = 0; ks < 4; ++ks)
-                    for (int lane = 0; lane < 32; ++lane) {
-                        const int g = lane >> 2, t = lane & 3;
-                        float *oh = w + ((size_t)(n * 4 + ks) * 32 + lane) * 2, *ol = oh + (size_t)NT * 4 * 32 * 2;
-                        for (int h = 0; h < 2; ++h) {
-                            const float v = (float)W[(size_t)(8 * ks + t + 4 * h) * nd + 8 * n + g];
-                            oh[h] = round_tf32_host(v);
-                            ol[h] = round_tf32_host(v - oh[h]);
-                        }
-                    }
             float *u = wu.data() + (size_t)k * 2 * 8 * nd * 4;
             for (int kk = 0; kk < TC_K; ++kk)
                 for (int q = 0; q < nd; ++q) {
@@ -1139,14 +815,12 @@ int psb_tc_prepare(psb_model_t *m, const float *hm, const float *hv, const float
             for (int i = 0; i < 32; ++i)
                 if (!std::isfinite(bb[i])) return PSB_OK;    // degenerate model: keep the scan kernels
         }
-    if (!m->d_tc_wfrag) {
+    if (!m->d_tc_wumma) {
         PSB_CUDA(cudaMalloc(&m->d_tc_wumma, wu.size() * sizeof(float)));
-        PSB_CUDA(cudaMalloc(&m->d_tc_wfrag, wf.size() * sizeof(float)));
         PSB_CUDA(cudaMalloc(&m->d_tc_cen, cen.size() * sizeof(float)));
         PSB_CUDA(cudaMalloc(&m->d_tc_bnd, bnd.size() * sizeof(float)));
     }
     PSB_CUDA(cudaMemcpy(m->d_tc_wumma, wu.data(), wu.size() * sizeof(float), cudaMemcpyHostToDevice));
-    PSB_CUDA(cudaMemcpy(m->d_tc_wfrag, wf.data(), wf.size() * sizeof(float), cudaMemcpyHostToDevice));
     PSB_CUDA(cudaMemcpy(m->d_tc_cen, cen.data(), cen.size() * sizeof(float), cudaMemcpyHostToDevice));
     PSB_CUDA(cudaMemcpy(m->d_tc_bnd, bnd.data(), bnd.size() * sizeof(float), cudaMemcpyHostToDevice));
     m->tc_ok = true;
@@ -1198,20 +872,12 @@ int psb_launch_ptm_tc(psb_batch_t *b, const float *d_feats, const int32_t *utt_o
     PSB_CUDA(cudaMemsetAsync(b->d_tc_flags, 0, fw * m->K * 4, b->stream));
     PSB_CUDA(cudaMemcpyAsync(b->d_uttoff, utt_off, ((size_t)n_utt + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, b->stream));
     static const bool check = [] { const char *v = getenv("PSB_TC_CHECK"); return v && atoi(v) != 0; }();
-    static const bool legacy_mma = [] { const char *v = getenv("PSB_TC_IMPL"); return v && !strcmp(v, "mma"); }();   // default: wgmma
     int rc;
-    if (legacy_mma)
-        switch (m->n_density) {
-        case 256: rc = launch_tc<13, 32>(b, d_feats, total, d_klist, m->K, d_featoff, check); break;
-        case 128: rc = launch_tc<13, 16>(b, d_feats, total, d_klist, m->K, d_featoff, check); break;
-        default: rc = launch_tc<13, 8>(b, d_feats, total, d_klist, m->K, d_featoff, check); break;
-        }
-    else
-        switch (m->n_density) {
-        case 256: rc = launch_wgmma<13, 256>(b, d_feats, total, d_klist, m->K, d_featoff, check); break;
-        case 128: rc = launch_wgmma<13, 128>(b, d_feats, total, d_klist, m->K, d_featoff, check); break;
-        default: rc = launch_wgmma<13, 64>(b, d_feats, total, d_klist, m->K, d_featoff, check); break;
-        }
+    switch (m->n_density) {
+    case 256: rc = launch_wgmma<13, 256>(b, d_feats, total, d_klist, m->K, d_featoff, check); break;
+    case 128: rc = launch_wgmma<13, 128>(b, d_feats, total, d_klist, m->K, d_featoff, check); break;
+    default: rc = launch_wgmma<13, 64>(b, d_feats, total, d_klist, m->K, d_featoff, check); break;
+    }
     if (rc) return rc;
     const long long chains = (long long)n_utt * m->K;
     const unsigned blocks = (unsigned)((chains * 32 + 127) / 128);

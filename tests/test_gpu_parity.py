@@ -366,7 +366,7 @@ def test_phoneloop_large_and_5state_vs_oracle(api, n_emit, H, window, skip):
 # ---------------------------------------------------------------------------------------
 # every top-N kernel variant (PSB_TOPN_VARIANT, read at psb_batch_create) must give the same bits
 
-@pytest.mark.parametrize("variant", [0, 1, 2, 3, 4, 5, 6])
+@pytest.mark.parametrize("variant", [0, 2, 3, 4, 5, 6])
 def test_topn_kernel_variants(api, en_us_dev, variant, monkeypatch):
     from oracle import oracle
     from pocketsphinx_b200.model import quantize_for_ties, synth_feats, synth_ptm
@@ -395,6 +395,16 @@ def test_topn_kernel_variants(api, en_us_dev, variant, monkeypatch):
     _batch_vs_oracle(api, pm2, [f2[u].reshape(-1, pm2.sumlen) for u in range(33)])
 
 
+@pytest.mark.parametrize("var,value", [("PSB_TOPN_VARIANT", "1"), ("PSB_TOPN_VARIANT", "7"), ("PSB_TC_IMPL", "mma")])
+def test_batch_refuses_a_selector_without_a_kernel(api, en_us_dev, var, value, monkeypatch):
+    """A top-N selector value that names no kernel is an error at psb_batch_create, not a silent fall-back to the
+    default, and the error names the accepted values."""
+    from pocketsphinx_b200._lib import PsbError
+    monkeypatch.setenv(var, value)
+    with pytest.raises(PsbError, match=r"accepted value.*(0, 2, 3, 4, 5 and 6|wgmma)"):
+        api.Batch(en_us_dev, 4, 1024)
+
+
 TC_CHECK = r"""
 import json, numpy as np
 import tc_cases as tc
@@ -420,18 +430,16 @@ print(json.dumps(out))
 """
 
 
-@pytest.mark.parametrize("impl", ["wgmma", "mma"])
-def test_tensor_core_filter_error_bound_holds_on_the_device(impl):
+def test_tensor_core_filter_error_bound_holds_on_the_device():
     """PSB_TC_CHECK=1: the filter kernel compares every 3 x TF32 GEMM value it produced with the exact float
     distance and reports the worst |a - d| / eps (the bound the candidate selection relies on must hold
     with room to spare: the analysis in psb_ptm_tc.cu allows 0.8 of eps), on the shipped model with real
-    features, the BASELINE shape, features scaled far outside the model's range and tie-stress data; for the
-    warpgroup-MMA kernel (wgmma, the default) and for the legacy mma.sync variant (PSB_TC_IMPL=mma).  Scores and
+    features, the BASELINE shape, features scaled far outside the model's range and tie-stress data.  Scores and
     top-N records match the oracle in the same runs."""
     import os
     import tc_cases as tc
     from conftest import GOLDEN
-    out = tc.child(TC_CHECK % os.path.join(GOLDEN, "en_us_ptm_model.npz"), impl)
+    out = tc.child(TC_CHECK % os.path.join(GOLDEN, "en_us_ptm_model.npz"))
     print(out)
     for name, v in out.items():
         assert 0.0 <= v["ratio"] < 0.8, (name, v)

@@ -53,24 +53,15 @@ print(json.dumps(out))
 """
 
 
-@pytest.mark.parametrize("impl", ["wgmma", "mma"])
-def test_crafted_cases_drive_every_counted_path(impl):
-    """wgmma: each case drives its counters.  The legacy mma.sync filter has no lane storage, byte list or work list,
-    and its candidate threshold (per-lane maxima) lists fewer rows, so there each certainty test is only required
-    to fail in some case built for it."""
-    out = tc.child(CHECK_CASES, impl)
+def test_crafted_cases_drive_every_counted_path():
+    """Each case drives every counter it was built for."""
+    out = tc.child(CHECK_CASES)
     print(out)
-    wgmma_only = {"lane_over", "fallback_listed", "fallback_all", "split_lists"}
-    reached = {}
     for name, v in out.items():
         assert 0.0 <= v["ratio"] < 0.8, (name, v)
         assert v["rows"] == v["total"] * v["K"], (name, v)
         for c in v["want"]:
-            if impl == "wgmma":
-                assert v[c] > 0, (impl, name, c, v)
-            elif c not in wgmma_only:
-                reached[c] = reached.get(c, 0) + v[c]
-    assert all(n > 0 for n in reached.values()), reached
+            assert v[c] > 0, (name, c, v)
 
 
 def _tpc_rule(tiles, K, P):
@@ -245,7 +236,7 @@ def test_gaussian_update_switches_the_filter_off_and_on():
     """tc_ok follows the Gaussians: bounds that are not finite leave the scan kernels in charge (no filter rows), the
     update back brings the filter back, and a model created degenerate gets its filter operands on its first good
     update."""
-    out = tc.child(CHECK_UPDATE, "wgmma")
+    out = tc.child(CHECK_UPDATE)
     print(out)
     n = out["per_run"]
     assert out["good"] == n and out["to_degenerate"] == n and out["back"] == 2 * n, out
