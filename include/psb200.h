@@ -436,8 +436,7 @@ int psb_fsg_batch_device(psb_hmmctx_t *c, const psb_fsg_desc_t *g, const int16_t
  *   result  [n_utt][3]                   entries, stack size, frames searched
  * on which ngram_search_find_exit / ngram_search_bp_hyp / the second pass work unchanged.  A full
  * table is an error (PSB_ERR_ARG): later frames read earlier entries.
- * Environment: PSB_SEARCH_WARP=1 selects the warp-per-utterance binding of the kernels;
- * PSB_NGS_BLOCKS / PSB_NGF_CHANNELS size the per-utterance fan-out pool of the first pass (default: one
+ * Environment: PSB_NGS_BLOCKS / PSB_NGF_CHANNELS size the per-utterance fan-out pool of the first pass (default: one
  * block per multi-phone word, at most 8192) and the state area of the second (default: every LM word's
  * chain, at most 65536 channels); running out of either is reported as an error. */
 typedef struct psb_ngram_desc_s {

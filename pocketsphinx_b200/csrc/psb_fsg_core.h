@@ -39,15 +39,9 @@
 #if defined(__CUDACC__) && !defined(PSB_FSG_HOST_EMUL)
 #define FSG_HD __device__ __forceinline__
 #define FSG_HDH __host__ __device__ __forceinline__
-#ifdef PSB_SEARCH_WARP                  /* one WARP per utterance (psb_search_warp.cu): same phases, warp-wide */
-#define FSG_FOR(i, n) for (int i = (int)(threadIdx.x & 31); i < (n); i += 32)
-#define FSG_SYNC() __syncwarp()
-#define FSG_IF_LEADER if ((threadIdx.x & 31) == 0)
-#else                                   /* one CTA per utterance (psb_search.cu) */
-#define FSG_FOR(i, n) for (int i = (int)threadIdx.x; i < (n); i += (int)blockDim.x)
+#define FSG_FOR(i, n) for (int i = (int)threadIdx.x; i < (n); i += (int)blockDim.x)   /* one CTA per utterance */
 #define FSG_SYNC() __syncthreads()
 #define FSG_IF_LEADER if (threadIdx.x == 0)
-#endif
 #define FSG_ATOMIC_MAX(p, v) atomicMax((p), (v))
 #define FSG_ATOMIC_ADD(p, v) atomicAdd((p), (v))
 #define FSG_ATOMIC_MIN(p, v) atomicMin((p), (v))
@@ -152,30 +146,7 @@ struct FsgScalars {
     int scan[34];
 };
 
-#if defined(__CUDACC__) && !defined(PSB_FSG_HOST_EMUL) && defined(PSB_SEARCH_WARP)
-// In-place exclusive scan of a[0..n) by one warp; returns the total to every lane.
-__device__ inline int fsg_exscan(fsg_wp a, int n, int *scan)
-{
-    const int lane = (int)(threadIdx.x & 31);
-    int carry = 0;
-    (void)scan;
-    __syncwarp();
-    for (int base = 0; base < n; base += 32) {
-        const int i = base + lane;
-        const int v = i < n ? a[i] : 0;
-        int incl = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const int t = __shfl_up_sync(0xffffffffu, incl, o);
-            if (lane >= o) incl += t;
-        }
-        if (i < n) a[i] = carry + incl - v;
-        carry += __shfl_sync(0xffffffffu, incl, 31);
-    }
-    __syncwarp();
-    return carry;
-}
-#elif defined(__CUDACC__) && !defined(PSB_FSG_HOST_EMUL)
+#if defined(__CUDACC__) && !defined(PSB_FSG_HOST_EMUL)
 // In-place exclusive scan of a[0..n) by the whole block; returns the total to every thread.
 __device__ inline int fsg_exscan(fsg_wp a, int n, int *scan /* [34], shared */)
 {

@@ -1285,7 +1285,7 @@ extern "C" int psb_hmmset_sweep_device(psb_hmmset_t *s, const int16_t *d_senscr,
         if (ms) PSB_CUDA(cudaStreamSynchronize(s->stream));
         return PSB_OK;
     }
-    // CTA shape: threads x instances per thread (PSB_SWEEP_SHAPE = 0: 256 x 4 (default), 1: 256 x 2, 2: 128 x 4, 3: 512 x 2)
+    // CTA shape: threads x instances per thread (PSB_SWEEP_SHAPE = 0: 256 x 4 (default), 1: 256 x 2, 3: 512 x 2; DESIGN 4.14)
     static const int shape = [] { const char *v = getenv("PSB_SWEEP_SHAPE"); return v ? atoi(v) : 0; }();
     const int buf_bytes = (int)(((size_t)cd.n_sen * 2 + 32 + 127) & ~(size_t)127);
     const int tp_bytes = s->c->n_tmat * cd.n_emit * (cd.n_emit + 1);
@@ -1303,7 +1303,6 @@ extern "C" int psb_hmmset_sweep_device(psb_hmmset_t *s, const int16_t *d_senscr,
     } while (0)
     if (cd.n_emit == 3) {
         if (shape == 1) PSB_SWEEP(3, 2, 256);
-        else if (shape == 2) PSB_SWEEP(3, 4, 128);
         else if (shape == 3) PSB_SWEEP(3, 2, 512);
         else PSB_SWEEP(3, 4, 256);
     }
@@ -1415,8 +1414,8 @@ extern "C" int psb_hmmset_eval_host(psb_hmmset_t *s, const int16_t *senscr, int3
 // its evaluate_hmms, state_align_search.c:65).  One CTA per utterance, the utterance's phone
 // chain in shared memory (SoA), time is the loop inside the kernel: renormalise (:199-203),
 // evaluate_hmms (:64-86), prune_hmms (:88-107), phone_transition (:109-136, a left-to-right
-// scan whose hmm_enter can cascade through not-yet-active successors, so one thread walks it in
-// the reference's order), record_transitions (:153-182) into a token table in HBM, and at the end
+// scan whose hmm_enter can cascade through not-yet-active successors: one warp resolves it as a
+// carry chain that gives the reference's order), record_transitions (:153-182) into a token table in HBM, and at the end
 // the backtrace of state_align_search_finish (:221-279).
 namespace {
 
@@ -1426,7 +1425,7 @@ align_kernel(const int16_t *__restrict__ senscr, const int32_t *__restrict__ utt
              const int32_t *__restrict__ tmatid_g, const int32_t *__restrict__ sf_g, const int32_t *__restrict__ ef_g,
              int32_t *__restrict__ tok_id, int32_t *__restrict__ tok_sc, const int64_t *__restrict__ tok_off,
              int32_t *__restrict__ st_start, int32_t *__restrict__ st_dur, int32_t *__restrict__ st_score,
-             int32_t *__restrict__ status, bool seq_scan)
+             int32_t *__restrict__ status)
 {
     extern __shared__ int sm[];
     const int u = blockIdx.x, tid = threadIdx.x, N = c.n_emit;
@@ -1498,18 +1497,7 @@ align_kernel(const int16_t *__restrict__ senscr, const int32_t *__restrict__ utt
         // (G reads nothing an earlier iteration writes), "active" is A[i] = P[i] | (G[i] & A[i-1]):
         // a carry chain.  One warp resolves 32 phones per step with a 64-bit add
         // (generate = P, propagate = G & ~P), the carry links the steps; E[j] = A[j-1] & G[j].
-        if (seq_scan) {
-            if (tid == 0)
-                for (int i = 0; i < H - 1; ++i) {
-                    if (frame[i] != nf) continue;
-                    if (nf < (sf_g ? sf_g[p0 + i + 1] : 0)) continue;
-                    const int nps = out_score[i];
-                    if (frame[i + 1] < t || nps > score[i + 1]) {        // hmm_enter(nhmm, score, history, nf)
-                        score[i + 1] = nps; hist[i + 1] = out_hist[i]; frame[i + 1] = nf;
-                    }
-                }
-        }
-        else if (tid < 32) {
+        if (tid < 32) {
             unsigned carry = 0u;
             for (int base = 0; base < H; base += 32) {
                 const int j = base + tid;
@@ -1645,7 +1633,7 @@ extern "C" int psb_align_batch_device(psb_hmmctx_t *c, const int16_t *d_senscr, 
         align_kernel<<<(unsigned)n_utt, 128, smem, st>>>(d_senscr, d_i32 + o_utt, dev_ctx(c), d_i32 + o_ph, c->d_al_senid, d_i32 + o_tm,
                                                         sf ? d_i32 + o_sf : nullptr, ef ? d_i32 + o_ef : nullptr, d_tok,
                                                         d_tok + tok_off[(size_t)n_utt], c->d_al_tokoff, d_i32 + o_ss, d_i32 + o_sd,
-                                                        d_i32 + o_sc, d_i32 + o_st, getenv("PSB_ALIGN_SEQ_SCAN") != nullptr);
+                                                        d_i32 + o_sc, d_i32 + o_st);
         g_psb_launches.fetch_add(1, std::memory_order_relaxed);
         e = cudaGetLastError();
     }

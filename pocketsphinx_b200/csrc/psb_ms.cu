@@ -377,19 +377,17 @@ int psb_launch_ms_batch(psb_batch_t *b, const float *d_feats, const int32_t *utt
         dim3 g1((m->n_mgau + 127) / 128, (unsigned)((n + FT - 1) / FT));
         size_t smem = (size_t)FT * m->sumlen * sizeof(float);
         int2 *dist = reinterpret_cast<int2 *>(b->d_msdist);
-        static const bool no_tile = getenv("PSB_MS_NOTILE") != nullptr;     // PSB_MS_NOTILE=1: the untiled kernel (parameters streamed from L2)
         const size_t tile_smem = ((size_t)m->n_density * m->sumlen * 2 + (size_t)m->n_feat * m->n_density) * MS_TCB * sizeof(float)
                                  + (size_t)m->sumlen * MS_TFB * sizeof(float);
-        const bool tile = !no_tile && tile_smem <= 100 * 1024;
+        const bool tile = tile_smem <= 100 * 1024;           // else the untiled kernel (parameters streamed from L2)
         // frames per CTA: enough CTAs for ~4 waves of two resident CTAs per SM, whole 32-frame blocks
         const int tiles_x = (m->n_mgau + MS_TCB - 1) / MS_TCB;
         const long long waves = psb_sm_count(m->device) * 2LL * 4;
         long long fpc = (n * tiles_x + waves - 1) / waves;
         fpc = std::max<long long>(MS_TFB, (fpc + MS_TFB - 1) / MS_TFB * MS_TFB);
         const dim3 gt((unsigned)tiles_x, (unsigned)((n + fpc - 1) / fpc));
-        static const bool no_fuse = [] { const char *v = getenv("PSB_MS_FUSE"); return v && atoi(v) == 0; }();
         // continuous models: mixtures evaluated by the lane that holds the list (the kernel writes raw scores and minima)
-        const bool fuse = tile && !no_fuse && m->sen_is_cb && m->n_mgau > 1;
+        const bool fuse = tile && m->sen_is_cb && m->n_mgau > 1;
         MsSenArgs sa = {m->d_mixw, m->d_logadd_ms, m->logadd_ms_size, m->logadd_ms_zero, d_senscr, b->d_msbest, n_used, m->aw};
         if (fuse) {
             fill_i32<<<(unsigned)((n + 255) / 256), 256, 0, b->stream>>>(b->d_msbest, n, 0x7fffffff);

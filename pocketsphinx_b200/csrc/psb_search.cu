@@ -3,28 +3,6 @@
 // The kernels are thin shells around phase code shared with the host emulation harnesses under
 // tests/emul/ (psb_fsg_core.h, psb_ngs_core.h, psb_ngf_core.h).
 #include "psb_hmmctx.cuh"
-#include "psb_search_launch.h"
-
-// This file is compiled twice: as it stands (one CTA per utterance, plus the C ABI), and through
-// psb_search_warp.cu with PSB_SEARCH_WARP defined (one WARP per utterance, four utterances per CTA:
-// the same phase code with warp-wide loops, __syncwarp() and a shuffle scan; launchers only).  The
-// ABI picks the warp kernels when PSB_SEARCH_WARP=1 is set in the environment.
-#ifdef PSB_SEARCH_WARP
-#define PSB_SRCH(name) name##_warp
-#define PSB_SRCH_UTT(S_type)                                                       \
-    __shared__ S_type S_all[SRCH_THREADS / 32];                                    \
-    S_type &S = S_all[threadIdx.x >> 5];                                           \
-    const int u = (int)blockIdx.x * (SRCH_THREADS / 32) + (int)(threadIdx.x >> 5); \
-    if (u >= n_utt) return
-#define PSB_SRCH_GRID(n_utt) (unsigned)(((n_utt) + SRCH_THREADS / 32 - 1) / (SRCH_THREADS / 32))
-#else
-#define PSB_SRCH(name) name##_cta
-#define PSB_SRCH_UTT(S_type)                                                       \
-    __shared__ S_type S;                                                           \
-    const int u = (int)blockIdx.x;                                                 \
-    (void)n_utt
-#define PSB_SRCH_GRID(n_utt) (unsigned)(n_utt)
-#endif
 
 #include <stdlib.h>
 #include <string.h>
@@ -75,9 +53,10 @@ constexpr int FSG_THREADS = SRCH_THREADS;
 __global__ void __launch_bounds__(FSG_THREADS)
 fsg_search_kernel(const int16_t *__restrict__ senscr, const int32_t *__restrict__ utt_off, HmmCtxDev c, FsgGraph G,
                   const uint16_t *__restrict__ senid_g, const int32_t *__restrict__ tmatid_g,
-                  int32_t *work, size_t work_words, int32_t *hist_out, int cap, int32_t *n_hist, int n_utt)
+                  int32_t *work, size_t work_words, int32_t *hist_out, int cap, int32_t *n_hist)
 {
-    PSB_SRCH_UTT(FsgScalars);
+    __shared__ FsgScalars S;
+    const int u = (int)blockIdx.x;
     const long long f0 = utt_off[u];
     const int T = utt_off[u + 1] - utt_off[u];
     FsgWork W;
@@ -95,21 +74,6 @@ fsg_search_kernel(const int16_t *__restrict__ senscr, const int32_t *__restrict_
 }
 
 }  // namespace
-
-void PSB_SRCH(psb_fsg_launch)(cudaStream_t st, int n_utt, const int16_t *senscr, const int32_t *utt_off, HmmCtxDev c, FsgGraph G,
-                              const uint16_t *senid, const int32_t *tmatid, int32_t *work, size_t work_words, int32_t *hist, int cap,
-                              int32_t *n_hist)
-{
-    fsg_search_kernel<<<PSB_SRCH_GRID(n_utt), FSG_THREADS, 0, st>>>(senscr, utt_off, c, G, senid, tmatid, work, work_words, hist, cap,
-                                                                    n_hist, n_utt);
-}
-
-#ifndef PSB_SEARCH_WARP
-static bool search_warp_mode()
-{
-    const char *e = getenv("PSB_SEARCH_WARP");
-    return e && e[0] == '1';
-}
 
 // Grow-only device workspace kept in the context: repeated calls (one per batch) do not pay
 // cudaMalloc / cudaFree again (DESIGN 4.7).
@@ -189,8 +153,8 @@ extern "C" int psb_fsg_batch_device(psb_hmmctx_t *c, const psb_fsg_desc_t *g, co
         fsg_graph_bind(flat, d_i, G);
         G.n_ci = g->n_ciphone; G.n_emit = N; G.silcipid = g->silcipid; G.start_state = g->start_state;
         G.beam = g->beam; G.pbeam = g->pbeam; G.wbeam = g->wbeam; G.maxhmmpf = g->maxhmmpf;
-        (search_warp_mode() ? psb_fsg_launch_warp : psb_fsg_launch_cta)(st, n_utt, d_senscr, d_i + o_uo, dev_ctx(c), G, d_senid, d_i + o_tm,
-                                                                        d_work, work_words, d_hist, cap_per_utt, d_i + o_nh);
+        fsg_search_kernel<<<n_utt, FSG_THREADS, 0, st>>>(d_senscr, d_i + o_uo, dev_ctx(c), G, d_senid, d_i + o_tm, d_work, work_words,
+                                                         d_hist, cap_per_utt, d_i + o_nh);
         g_psb_launches.fetch_add(1, std::memory_order_relaxed);
         e = cudaGetLastError();
     }
@@ -205,8 +169,6 @@ extern "C" int psb_fsg_batch_device(psb_hmmctx_t *c, const psb_fsg_desc_t *g, co
         PSB_REQUIRE(n_hist[u] >= 0, "psb_fsg_batch_device: scratch overflow in utterance %d (internal)", u);
     return PSB_OK;
 }
-
-#endif  // !PSB_SEARCH_WARP (C ABI of the grammar search)
 
 // ---------------------------------------------------------------------------------------
 // N-gram decoding, first pass (ngram_search_fwdtree.c) for whole batches: SURVEY 8 row f-1 proper.
@@ -255,9 +217,10 @@ constexpr int NGS_THREADS = SRCH_THREADS;
 __global__ void __launch_bounds__(NGS_THREADS)
 ngs_fwdtree_kernel(const int16_t *__restrict__ senscr, const int32_t *__restrict__ utt_off, HmmCtxDev c, NgsGraph G,
                    int32_t *work, size_t work_words, const int32_t *pen, int pl_window, int32_t *bp_out, int bp_cap, int32_t *bss_out,
-                   int bss_cap, int32_t *bp_idx_out, int32_t *result /* [n_utt][3]: bpidx, bss_head, frames done (or -error) */, int n_utt)
+                   int bss_cap, int32_t *bp_idx_out, int32_t *result /* [n_utt][3]: bpidx, bss_head, frames done (or -error) */)
 {
-    PSB_SRCH_UTT(NgsScalars);
+    __shared__ NgsScalars S;
+    const int u = (int)blockIdx.x;
     const long long f0 = utt_off[u];
     const int T = utt_off[u + 1] - utt_off[u];
     NgsWork W;
@@ -284,15 +247,6 @@ ngs_fwdtree_kernel(const int16_t *__restrict__ senscr, const int32_t *__restrict
 
 }  // namespace
 
-void PSB_SRCH(psb_ngs_launch)(cudaStream_t st, int n_utt, const int16_t *senscr, const int32_t *utt_off, HmmCtxDev c, NgsGraph G,
-                              int32_t *work, size_t work_words, const int32_t *pen, int pl_window, int32_t *bp, int bp_cap, int32_t *bss,
-                              int bss_cap, int32_t *bp_idx, int32_t *result)
-{
-    ngs_fwdtree_kernel<<<PSB_SRCH_GRID(n_utt), NGS_THREADS, 0, st>>>(senscr, utt_off, c, G, work, work_words, pen, pl_window, bp, bp_cap, bss, bss_cap,
-                                                                     bp_idx, result, n_utt);
-}
-
-#ifndef PSB_SEARCH_WARP
 extern "C" int psb_ngram_fwdtree_batch_device(psb_hmmctx_t *c, const psb_ngram_desc_t *g, const int16_t *d_senscr,
                                               const int32_t *d_pen, int32_t pl_window, const int32_t *utt_off, int32_t n_utt, int32_t *bp,
                                               int32_t bp_cap_per_utt, int32_t *bss, int32_t bss_cap_per_utt,
@@ -336,9 +290,8 @@ extern "C" int psb_ngram_fwdtree_batch_device(psb_hmmctx_t *c, const psb_ngram_d
     if (e == cudaSuccess) e = cudaMemsetAsync(d_idx, 0, n_idx * 4, st);
     if (e == cudaSuccess) {
         ngs_bind(flat, d_i);
-        (search_warp_mode() ? psb_ngs_launch_warp : psb_ngs_launch_cta)(st, n_utt, d_senscr, d_i + o_uo, dev_ctx(c), flat.G, d_work, work_words,
-                                                                        d_pen, pl_window, d_bp, bp_cap_per_utt, d_bss, bss_cap_per_utt, d_idx,
-                                                                        d_i + o_res);
+        ngs_fwdtree_kernel<<<n_utt, NGS_THREADS, 0, st>>>(d_senscr, d_i + o_uo, dev_ctx(c), flat.G, d_work, work_words, d_pen, pl_window,
+                                                          d_bp, bp_cap_per_utt, d_bss, bss_cap_per_utt, d_idx, d_i + o_res);
         g_psb_launches.fetch_add(1, std::memory_order_relaxed);
         e = cudaGetLastError();
     }
@@ -362,8 +315,6 @@ extern "C" int psb_ngram_fwdtree_batch_device(psb_hmmctx_t *c, const psb_ngram_d
     return PSB_OK;
 }
 
-#endif  // !PSB_SEARCH_WARP
-
 // ---------------------------------------------------------------------------------------
 // N-gram decoding, second pass (ngram_search_fwdflat.c) for whole batches: SURVEY 8 row f-4.  One
 // CTA per utterance, one thread per active word (psb_ngf_core.h, host-emulated against the
@@ -378,9 +329,10 @@ typedef ChanDevEval<NgfGraph, NgfWork> NgfDevEval;
 __global__ void __launch_bounds__(NGS_THREADS)
 ngs_fwdflat_kernel(const int16_t *__restrict__ senscr, const int32_t *__restrict__ utt_off, HmmCtxDev c, NgfGraph G,
                    int32_t *work, size_t work_words, const int32_t *bp_in, int in_cap, const int32_t *n_in, int n_in_stride,
-                   int32_t *bp_out, int bp_cap, int32_t *bss_out, int bss_cap, int32_t *bp_idx_out, int32_t *result, int n_utt)
+                   int32_t *bp_out, int bp_cap, int32_t *bss_out, int bss_cap, int32_t *bp_idx_out, int32_t *result)
 {
-    PSB_SRCH_UTT(NgfScalars);
+    __shared__ NgfScalars S;
+    const int u = (int)blockIdx.x;
     const long long f0 = utt_off[u];
     const int T = utt_off[u + 1] - utt_off[u];
     NgfWork W;
@@ -408,15 +360,6 @@ ngs_fwdflat_kernel(const int16_t *__restrict__ senscr, const int32_t *__restrict
 
 }  // namespace
 
-void PSB_SRCH(psb_ngf_launch)(cudaStream_t st, int n_utt, const int16_t *senscr, const int32_t *utt_off, HmmCtxDev c, NgfGraph G,
-                              int32_t *work, size_t work_words, const int32_t *bp_in, int in_cap, const int32_t *n_in, int n_in_stride,
-                              int32_t *bp, int bp_cap, int32_t *bss, int bss_cap, int32_t *bp_idx, int32_t *result)
-{
-    ngs_fwdflat_kernel<<<PSB_SRCH_GRID(n_utt), NGS_THREADS, 0, st>>>(senscr, utt_off, c, G, work, work_words, bp_in, in_cap, n_in, n_in_stride, bp, bp_cap,
-                                                                     bss, bss_cap, bp_idx, result, n_utt);
-}
-
-#ifndef PSB_SEARCH_WARP
 extern "C" int psb_ngram_fwdflat_batch_device(psb_hmmctx_t *c, const psb_ngram_desc_t *g, const int16_t *d_senscr,
                                               const int32_t *utt_off, int32_t n_utt, const int32_t *bp_first,
                                               int32_t first_cap_per_utt, const int32_t *n_first, int32_t *bp,
@@ -476,9 +419,8 @@ extern "C" int psb_ngram_fwdflat_batch_device(psb_hmmctx_t *c, const psb_ngram_d
     if (e == cudaSuccess) e = cudaMemsetAsync(d_idx, 0, n_idx * 4, st);
     if (e == cudaSuccess) {
         ngf_bind(flat, d_i);
-        (search_warp_mode() ? psb_ngf_launch_warp : psb_ngf_launch_cta)(st, n_utt, d_senscr, d_i + o_uo, dev_ctx(c), flat.G, d_work, work_words, d_in,
-                                                                        first_cap_per_utt, d_i + o_nin, 1, d_bp, bp_cap_per_utt, d_bss, bss_cap_per_utt,
-                                                                        d_idx, d_i + o_res);
+        ngs_fwdflat_kernel<<<n_utt, NGS_THREADS, 0, st>>>(d_senscr, d_i + o_uo, dev_ctx(c), flat.G, d_work, work_words, d_in, first_cap_per_utt,
+                                                          d_i + o_nin, 1, d_bp, bp_cap_per_utt, d_bss, bss_cap_per_utt, d_idx, d_i + o_res);
         g_psb_launches.fetch_add(1, std::memory_order_relaxed);
         e = cudaGetLastError();
     }
@@ -562,12 +504,11 @@ extern "C" int psb_ngram_two_pass_batch_device(psb_hmmctx_t *c, const psb_ngram_
     if (e == cudaSuccess) e = cudaMemsetAsync(d_idx1, 0, n_idx * 4, st);
     if (e == cudaSuccess) e = cudaMemsetAsync(d_idx2, 0, n_idx * 4, st);
     if (e == cudaSuccess) {
-        const bool warp = search_warp_mode();
         ngs_bind(f1, d_i);
         ngf_bind(f2, d_i + o_g2);
-        (warp ? psb_ngs_launch_warp : psb_ngs_launch_cta)(st, n_utt, d_senscr, d_i + o_uo, dev_ctx(c), f1.G, d_work, ww, d_pen, pl_window, d_bp1,
+        ngs_fwdtree_kernel<<<n_utt, NGS_THREADS, 0, st>>>(d_senscr, d_i + o_uo, dev_ctx(c), f1.G, d_work, ww, d_pen, pl_window, d_bp1,
                                                           first_cap_per_utt, d_bss1, first_bss_cap_per_utt, d_idx1, d_i + o_r1);
-        (warp ? psb_ngf_launch_warp : psb_ngf_launch_cta)(st, n_utt, d_senscr, d_i + o_uo, dev_ctx(c), f2.G, d_work, ww, d_bp1, first_cap_per_utt,
+        ngs_fwdflat_kernel<<<n_utt, NGS_THREADS, 0, st>>>(d_senscr, d_i + o_uo, dev_ctx(c), f2.G, d_work, ww, d_bp1, first_cap_per_utt,
                                                           d_i + o_r1, 3, d_bp2, bp_cap_per_utt, d_bss2, bss_cap_per_utt, d_idx2, d_i + o_r2);
         g_psb_launches.fetch_add(2, std::memory_order_relaxed);
         e = cudaGetLastError();
@@ -595,7 +536,6 @@ extern "C" int psb_ngram_two_pass_batch_device(psb_hmmctx_t *c, const psb_ngram_
     }
     return PSB_OK;
 }
-#endif  // !PSB_SEARCH_WARP
 
 // ---------------------------------------------------------------------------------------
 // Self-test hook for the one building block of the search kernels that host emulation cannot run:
@@ -611,16 +551,6 @@ exscan_selftest_kernel(int32_t *a, int n, int32_t *total)
 }
 }  // namespace
 
-void PSB_SRCH(psb_exscan_launch)(int32_t *a, int n, int32_t *total)
-{
-#ifdef PSB_SEARCH_WARP
-    exscan_selftest_kernel<<<1, 32>>>(a, n, total);          // the warp binding scans with one warp
-#else
-    exscan_selftest_kernel<<<1, NGS_THREADS>>>(a, n, total);
-#endif
-}
-
-#ifndef PSB_SEARCH_WARP
 extern "C" int psb_selftest_block_scan(int device, int32_t *a, int32_t n, int32_t *total)
 {
     PSB_REQUIRE(a && total && n >= 0, "psb_selftest_block_scan: bad argument");
@@ -629,7 +559,7 @@ extern "C" int psb_selftest_block_scan(int device, int32_t *a, int32_t n, int32_
     PSB_CUDA(cudaMalloc((void **)&d, ((size_t)n + 2) * 4));
     cudaError_t e = cudaMemcpy(d, a, (size_t)n * 4, cudaMemcpyHostToDevice);
     if (e == cudaSuccess) {
-        (search_warp_mode() ? psb_exscan_launch_warp : psb_exscan_launch_cta)(d, n, d + n);
+        exscan_selftest_kernel<<<1, NGS_THREADS>>>(d, n, d + n);
         g_psb_launches.fetch_add(1, std::memory_order_relaxed);
         e = cudaGetLastError();
     }
@@ -642,4 +572,3 @@ extern "C" int psb_selftest_block_scan(int device, int32_t *a, int32_t n, int32_
     }
     return PSB_OK;
 }
-#endif  // !PSB_SEARCH_WARP

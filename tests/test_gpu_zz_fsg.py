@@ -1,7 +1,6 @@
 """GPU (-m gpu): psb_fsg_batch_device (the grammar search of fsg_search.c on the device) against the
 reference's golden history tables and against the oracle on ragged batches.
 
-The CTA-per-utterance binding of the phase code runs by default; PSB_SEARCH_WARP=1 runs the same cases on the warp one.
 The phase code is also checked on the host against the reference (tests/test_fsg_emul.py)."""
 
 import numpy as np

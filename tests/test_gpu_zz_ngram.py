@@ -1,8 +1,8 @@
 """GPU (-m gpu): psb_ngram_fwdtree_batch_device (the first pass of the n-gram search on the device)
 against the reference's golden backpointer tables and against the oracle on ragged batches.
 
-PSB_SEARCH_WARP=1 runs the same cases on the warp binding of the phase code.  The phase code is also
-checked on the host against the reference (tests/test_ngs_emul.py, tests/test_ngf_emul.py)."""
+The phase code is also checked on the host against the reference (tests/test_ngs_emul.py,
+tests/test_ngf_emul.py)."""
 
 import os
 

@@ -1,6 +1,6 @@
-"""CPU: step-by-step simulation of the two device scans of psb_fsg_core.h (fsg_exscan: CTA-wide with warp
-shuffles + a shared carry, and the one-warp variant of the warp binding) -- the one building block of the
-search kernels the host emulation replaces by a plain loop.  Every statement between two barriers is
+"""CPU: step-by-step simulation of the device scan of psb_fsg_core.h (fsg_exscan: CTA-wide with warp
+shuffles + a shared carry) -- the one building block of the search kernels the host emulation replaces
+by a plain loop.  Every statement between two barriers is
 executed for all "threads" before the next; a shuffle reads the source lane's value from before the
 statement.  This checks the algorithm as written (chunking, carries, partial last chunk, empty input),
 not the CUDA code itself: that is tests/test_gpu_zz_fsg.py::test_block_scan_selftest."""
@@ -33,27 +33,7 @@ def exscan_cta(a, n, nt=128):
     return a, int(scan[33])
 
 
-def exscan_warp(a, n):
-    a = a.copy()
-    lane = np.arange(32)
-    carry, base = 0, 0
-    while base < n:
-        i = base + lane
-        v = np.where(i < n, a[np.minimum(i, n - 1)], 0)
-        incl = v.copy()
-        o = 1
-        while o < 32:
-            t = np.where(lane >= o, incl[np.maximum(lane - o, 0)], 0)
-            incl = np.where(lane >= o, incl + t, incl)
-            o <<= 1
-        m = i < n
-        a[i[m]] = (carry + incl - v)[m]
-        carry += incl[31]                                                  # __shfl_sync(incl, 31)
-        base += 32
-    return a, int(carry)
-
-
-@pytest.mark.parametrize("scan", [exscan_cta, exscan_warp])
+@pytest.mark.parametrize("scan", [exscan_cta])
 def test_scan_as_written(scan):
     rng = np.random.default_rng(1)
     for n in (0, 1, 31, 32, 33, 127, 128, 129, 255, 256, 257, 1000, 4097):
