@@ -517,7 +517,8 @@ int psb_selftest_block_scan(int device, int32_t *a, int32_t n, int32_t *total);
 /* ------------------------------------------------------------------------------------ */
 /* Batched front end (SURVEY 8 row f-2): int16 PCM -> cepstra -> batch CMN -> 1s_c_d_dd features
  * for whole batches, every utterance a fresh stream (ps_start_stream + ps_process_raw(full_utt),
- * pocketsphinx.c:1073, acmod.c:528-560).  The tables are the arrays the reference's own fe_t /
+ * pocketsphinx.c:1073, acmod.c:528-560).  psb_fe_create_ex adds s2_4x / s3_1x39, live CMN and
+ * dither, and sessions of utterances that carry their CMN and dither state.  The tables are the arrays the reference's own fe_t /
  * melfb_t hold after fe_init (fe_internal.h:100-180): a C host passes those pointers. */
 typedef struct psb_fe_desc_s {
     int32_t frame_size, frame_shift, fft_size, fft_order;   /* fe_t */
@@ -548,9 +549,44 @@ int psb_fe_process_host(psb_fe_t *fe, const int16_t *pcm, const int64_t *samp_of
                         float *feats, float *mfcc, int32_t *frame_off);
 int psb_fe_process_device(psb_fe_t *fe, const int16_t *d_pcm, const int64_t *samp_off, int32_t n_utt,
                           float *d_feats, float *d_mfcc, int32_t *frame_off, float *ms);
-/* device copy of the features of the last psb_fe_process_host call, and their dimension */
+/* device copy of the features of the last psb_fe_process_host call, and their dimension: 39 for
+ * 1s_c_d_dd and s3_1x39, 51 for s2_4x (its four streams 12 + 24 + 3 + 12 back to back) */
 const float *psb_fe_device_feats(const psb_fe_t *fe);
 int32_t psb_fe_feat_dim(const psb_fe_t *fe);
+
+/* Feature type, CMN and dither options (feat_init, cmn_set_repr, fe_init_dither).  With them,
+ * psb_fe_desc_t.window and .cmn are not read.  o == NULL is psb_fe_create. */
+#define PSB_FE_MAX_CEP 32
+enum { PSB_FEAT_1S_C_D_DD = 0, PSB_FEAT_S2_4X = 1, PSB_FEAT_S3_1X39 = 2 };   /* -feat (s3_1x39 = 1s_12c_12d_3p_12dd) */
+enum { PSB_CMN_NONE = 0, PSB_CMN_BATCH = 1, PSB_CMN_LIVE = 2 };            /* -cmn (current = batch) */
+typedef struct psb_fe_opts_s {
+    int32_t feat;                          /* PSB_FEAT_*; s2_4x and s3_1x39 need n_cep == 13 */
+    int32_t cmn;                           /* PSB_CMN_* */
+    int32_t varnorm;                       /* -varnorm: must be 0 (not implemented; live CMN refuses it too) */
+    int32_t dither;                        /* -dither: 0 / 1 */
+    int32_t seed;                          /* -seed: the MT19937 seed, init_genrand((unsigned long)seed) */
+    float cmn_init[PSB_FE_MAX_CEP];        /* -cmninit as cmn_set_repr parses it; unused entries 0 */
+} psb_fe_opts_t;
+int psb_fe_create_ex(const psb_fe_desc_t *d, const psb_fe_opts_t *o, int device, psb_fe_t **out);
+
+/* What a ps_decoder_t carries from one utterance to the next: the live-CMN state (cmn_t) and the
+ * dither generator (genrand.c).  ps_start_stream resets neither. */
+typedef struct psb_fe_state_s {
+    float cmn_mean[PSB_FE_MAX_CEP], cmn_sum[PSB_FE_MAX_CEP];
+    int32_t cmn_nframe;
+    int32_t mt_index;                      /* mti: 624 = a twist is due */
+    uint32_t mt[624];
+} psb_fe_state_t;
+/* the state fe_init + cmn_set_repr leave: mean = cmn_init, sum = mean * 500, nframe = 500,
+ * init_genrand(seed) */
+int psb_fe_state_init(const psb_fe_t *fe, psb_fe_state_t *s);
+/* Names the sessions of the next psb_fe_process_* / psb_decode_batch_pcm_host call: session s is
+ * utterances sess_off[s] .. sess_off[s + 1] - 1 (in decode order; sess_off[0] = 0, sess_off[n_sess]
+ * = that call's n_utt), starting from states_in[s] (NULL: psb_fe_state_init for every session).
+ * Without this call every utterance is a session of its own from the initial state. */
+int psb_fe_set_sessions(psb_fe_t *fe, const int32_t *sess_off, int32_t n_sess, const psb_fe_state_t *states_in);
+/* the sessions' states after the last process call (n_sess of them, in session order) */
+int psb_fe_get_states(const psb_fe_t *fe, psb_fe_state_t *states_out, int32_t n_sess);
 /* From audio to phone-loop results in one call: front end, senone scores and Viterbi on the
  * device, features never leave it.  frame_off int32[n_utt + 1] (out) indexes best / pen / senscr
  * like utt_off of psb_decode_batch_host. */

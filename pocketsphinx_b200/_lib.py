@@ -37,6 +37,16 @@ class FeDesc(C.Structure):
                 ("filt_coeffs", C.c_void_p), ("mel_cosine", C.c_void_p), ("lifter", C.c_void_p)]
 
 
+class FeOpts(C.Structure):
+    _fields_ = [("feat", C.c_int32), ("cmn", C.c_int32), ("varnorm", C.c_int32), ("dither", C.c_int32), ("seed", C.c_int32),
+                ("cmn_init", C.c_float * 32)]
+
+
+class FeState(C.Structure):
+    _fields_ = [("cmn_mean", C.c_float * 32), ("cmn_sum", C.c_float * 32), ("cmn_nframe", C.c_int32), ("mt_index", C.c_int32),
+                ("mt", C.c_uint32 * 624)]
+
+
 class FsgDesc(C.Structure):
     _fields_ = [("n_pnode", C.c_int32), ("pnodes", C.c_void_p), ("n_state", C.c_int32), ("roots", C.c_void_p),
                 ("n_link", C.c_int32), ("links", C.c_void_p), ("nulloff", C.c_void_p), ("nullarc", C.c_void_p),
@@ -116,6 +126,10 @@ SYMBOLS = [
     ("psb_fe_feat_dim", C.c_int32, [_VP]),
     ("psb_decode_batch_pcm_host", C.c_int, [_VP, _VP, _VP, _VP, _VP, _I32, _VP, _VP, _VP, _VP]),
     ("psb_fe_process_device", C.c_int, [_VP, _VP, _VP, _I32, _VP, _VP, _VP, C.POINTER(C.c_float)]),
+    ("psb_fe_create_ex", C.c_int, [C.POINTER(FeDesc), C.POINTER(FeOpts), C.c_int, C.POINTER(_VP)]),
+    ("psb_fe_state_init", C.c_int, [_VP, C.POINTER(FeState)]),
+    ("psb_fe_set_sessions", C.c_int, [_VP, _VP, _I32, _VP]),
+    ("psb_fe_get_states", C.c_int, [_VP, _VP, _I32]),
     ("psb_phoneloop_create", C.c_int, [_VP, _I32, _VP, _VP, _I32, _I32, _I32, _I32, C.c_double, C.POINTER(_VP)]),
     ("psb_phoneloop_free", None, [_VP]),
     ("psb_phoneloop_run_device", C.c_int, [_VP, _VP, _VP, _I32, _VP, _VP, _VP, _VP]),

@@ -652,11 +652,13 @@ def ngram_segments(info, model, bp, bss, entry, lm_arrays=None, second_pass=Fals
 
 
 class FrontEnd:
-    """fe/ + feat/ for whole batches on the device (every utterance a fresh stream).  `desc` is the
-    dict of fe_tables.make_fe_desc() -- or the same arrays taken out of the reference's fe_t."""
+    """fe/ + feat/ for whole batches on the device.  `desc` is the dict of fe_tables.make_fe_desc() -- or the
+    same arrays taken out of the reference's fe_t.  `opts` (fe_tables.make_fe_opts(), optional) selects the
+    feature type, CMN (including live), -cmninit and dither; without it every utterance is a fresh stream with
+    desc's 1s_c_d_dd features and CMN."""
 
-    def __init__(self, desc, device=0):
-        from ._lib import FeDesc
+    def __init__(self, desc, device=0, opts=None):
+        from ._lib import FeDesc, FeOpts
         self.desc = desc
         self._keep = {}
         d = FeDesc()
@@ -675,8 +677,51 @@ class FrontEnd:
         d.n_coeffs = int(self._keep["filt_coeffs"].size)
         self.n_cep = int(desc["n_cep"])
         h = C.c_void_p()
-        check(lib().psb_fe_create(C.byref(d), device, C.byref(h)), "psb_fe_create")
+        if opts is None:
+            check(lib().psb_fe_create(C.byref(d), device, C.byref(h)), "psb_fe_create")
+        else:
+            o = FeOpts()
+            for k in ("feat", "cmn", "varnorm", "dither", "seed"):
+                setattr(o, k, int(opts[k]))
+            ci = np.zeros(32, np.float32)
+            v = np.asarray(opts["cmn_init"], np.float32).ravel()[:32]
+            ci[:v.size] = v
+            o.cmn_init[:] = ci.tolist()
+            check(lib().psb_fe_create_ex(C.byref(d), C.byref(o), device, C.byref(h)), "psb_fe_create_ex")
         self.h = h
+        self.feat_dim = lib().psb_fe_feat_dim(h)
+
+    def initial_state(self):
+        """The session state of a fresh decoder: -cmninit's mean and the dither generator seeded with -seed."""
+        from ._lib import FeState
+        s = FeState()
+        check(lib().psb_fe_state_init(self.h, C.byref(s)), "psb_fe_state_init")
+        return s
+
+    def set_sessions(self, sess_off, states=None):
+        """Names the sessions of the next process_* / Batch.decode_pcm_host call: session s is utterances
+        sess_off[s] .. sess_off[s + 1] - 1, starting from states[s] (FeState objects; None: fresh)."""
+        from ._lib import FeState
+        sess_off = np.ascontiguousarray(sess_off, np.int32)
+        n = len(sess_off) - 1
+        arr = None
+        if states is not None:
+            assert len(states) == n
+            arr = (FeState * max(n, 1))(*states)
+        check(lib().psb_fe_set_sessions(self.h, _p(sess_off), n, arr), "psb_fe_set_sessions")
+
+    def get_states(self, n_sess):
+        """The sessions' states after the last call, as a list of FeState."""
+        from ._lib import FeState
+        arr = (FeState * max(n_sess, 1))()
+        check(lib().psb_fe_get_states(self.h, arr, n_sess), "psb_fe_get_states")
+        return [arr[i] for i in range(n_sess)]
+
+    def process_sessions(self, pcm, samp_off, sess_off, states=None, want_mfcc=False):
+        """process_host over named sessions; returns (feats, frame_off, outgoing states[, mfcc])."""
+        self.set_sessions(sess_off, states)
+        r = self.process_host(pcm, samp_off, want_mfcc)
+        return r[:2] + (self.get_states(len(sess_off) - 1),) + r[2:]
 
     def n_frames(self, n_samples):
         return lib().psb_fe_n_frames(self.h, int(n_samples))
@@ -688,13 +733,13 @@ class FrontEnd:
         return off
 
     def process_host(self, pcm, samp_off, want_mfcc=False):
-        """pcm int16 (utterances back to back), samp_off int64 [n_utt+1] -> (feats [T][3*n_cep],
+        """pcm int16 (utterances back to back), samp_off int64 [n_utt+1] -> (feats [T][feat_dim],
         frame_off int32 [n_utt+1][, mfcc after CMN [T][n_cep]])."""
         pcm = np.ascontiguousarray(pcm, np.int16)
         samp_off = np.ascontiguousarray(samp_off, np.int64)
         n_utt = len(samp_off) - 1
         total = sum(self.n_frames(int(samp_off[u + 1] - samp_off[u])) for u in range(n_utt))
-        feats = np.zeros((total, 3 * self.n_cep), np.float32)
+        feats = np.zeros((total, self.feat_dim), np.float32)
         mfcc = np.zeros((total, self.n_cep), np.float32) if want_mfcc else None
         frame_off = np.zeros(n_utt + 1, np.int32)
         check(lib().psb_fe_process_host(self.h, _p(pcm) if pcm.size else None, _p(samp_off), n_utt, _p(feats) if total else None,

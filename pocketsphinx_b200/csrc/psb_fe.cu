@@ -11,6 +11,9 @@
 //   frame counting of fe_process_frames + fe_end_utt                 (fe_interface.c:352-545)
 //   cmn (batch)                                                      (feat/cmn.c:136-200)
 //   feat_1s_c_d_dd_cep2feat with replicated edges                    (feat/feat.c:579-622, 1243-1330)
+//   feat_s2_4x_cep2feat / feat_s3_1x39_cep2feat                      (feat/feat.c:425-538)
+//   cmn_live + cmn_live_shiftwin + cmn_live_update over a session    (feat/cmn_live.c, feat.c:917-938)
+//   dither: MT19937 (util/genrand.c) in the draw order of fe_process_frames + fe_end_utt
 // All tables (window, twiddles, mel filters, DCT cosines, lifter) are INPUTS: the host builds
 // them with the reference's own init code / libm and passes them in psb_fe_desc_t.  The only
 // operation that is not bit-reproducible is log(): device libm vs glibc can differ in the last
@@ -40,6 +43,17 @@ struct psb_fe_s {
     int16_t *d_pcm; size_t pcm_cap;
     float *d_feats; size_t feats_cap;
     int64_t *d_samp_off; int32_t *d_frame_off; int32_t *d_frame_utt; size_t utt_cap, fu_cap;
+    // psb_fe_create_ex options and sessions
+    int feat, feat_dim, dither, seed;
+    float cmn_init[PSB_FE_MAX_CEP];
+    std::vector<int32_t> sess_off;            // set by psb_fe_set_sessions for the next call only
+    std::vector<psb_fe_state_t> states;       // in: the next call's sessions; out: after it
+    bool sess_pending;
+    psb_fe_state_t *d_state; size_t state_cap;
+    int32_t *d_sess_off; size_t sess_cap;
+    int64_t *d_draw; size_t draw_cap;         // per utterance: first tail sample, tail offset, main draws, tail draws
+    int16_t *d_dpcm; size_t dpcm_cap;         // dithered samples of the full frames
+    int16_t *d_tail; size_t tail_cap;         // freshly dithered samples of each utterance's last frame
 };
 
 namespace {
@@ -59,10 +73,14 @@ struct FeDev {
 
 // One CTA per frame: samples -> pre-emphasis -> window -> real FFT -> power spectrum -> mel.
 // frame_utt[f] = utterance of flat frame f; frame_off[u] = first flat frame of utterance u.
+// DITHER: pcm holds the dithered samples of the full frames, and the last frame of utterance u
+// reads its own freshly dithered copy at tail + draw[4u + 1] (fe_end_utt re-reads the overflow
+// samples); its pre-emphasis prior is still the full frames' sample before it.
+template <bool DITHER>
 __global__ void __launch_bounds__(128)
 fe_frame_kernel(FeDev p, const int16_t *__restrict__ pcm, const int64_t *__restrict__ samp_off,
                 const int32_t *__restrict__ frame_off, const int32_t *__restrict__ frame_utt,
-                double *__restrict__ mfspec)
+                double *__restrict__ mfspec, const int16_t *__restrict__ tail, const int64_t *__restrict__ draw)
 {
     extern __shared__ double x[];             // [fft_size] frame, then [fft_size/2 + 1] power spectrum
     double *spec = x + p.fft_size;
@@ -73,6 +91,9 @@ fe_frame_kernel(FeDev p, const int16_t *__restrict__ pcm, const int64_t *__restr
     const int64_t start = (int64_t)k * p.frame_shift;
     int len = (int)min((int64_t)p.frame_size, n - start);
     const int16_t *in = pcm + s0 + start;
+    const int16_t *src = in;
+    if constexpr (DITHER)
+        if (k == frame_off[u + 1] - frame_off[u] - 1) src = tail + draw[4 * u + 1];
     const int tid = threadIdx.x, nt = blockDim.x;
     const int half = p.frame_size / 2;
 
@@ -83,11 +104,11 @@ fe_frame_kernel(FeDev p, const int16_t *__restrict__ pcm, const int64_t *__restr
             double v = 0.0;
             if (i < len) {
                 if (p.alpha != 0.0f) {
-                    const int16_t prev = i > 0 ? in[i - 1] : (start > 0 ? in[-1] : (int16_t)0);
-                    v = (double)in[i] - (double)prev * (double)p.alpha;
+                    const int16_t prev = i > 0 ? src[i - 1] : (start > 0 ? in[-1] : (int16_t)0);
+                    v = (double)src[i] - (double)prev * (double)p.alpha;
                 }
                 else
-                    v = (double)in[i];
+                    v = (double)src[i];
             }
             if (i < half) v = v * p.hamming[i];
             else if (i >= p.frame_size - half && i < p.frame_size) v = v * p.hamming[p.frame_size - 1 - i];
@@ -100,11 +121,11 @@ fe_frame_kernel(FeDev p, const int16_t *__restrict__ pcm, const int64_t *__restr
             double v = 0.0;
             if (i < len) {
                 if (p.alpha != 0.0f) {
-                    const int16_t prev = i > 0 ? in[i - 1] : (start > 0 ? in[-1] : (int16_t)0);
-                    v = (double)in[i] - (double)prev * (double)p.alpha;
+                    const int16_t prev = i > 0 ? src[i - 1] : (start > 0 ? in[-1] : (int16_t)0);
+                    v = (double)src[i] - (double)prev * (double)p.alpha;
                 }
                 else
-                    v = (double)in[i];
+                    v = (double)src[i];
             }
             x[i] = v;
         }
@@ -317,6 +338,152 @@ fe_utt_kernel(FeDev p, const int32_t *__restrict__ frame_off, double *__restrict
     }
 }
 
+// One CTA per session: the session's MT19937 stream (genrand_int32, util/genrand.c), one draw per
+// sample read.  Utterance u draws draw[4u + 2] times for its full frames (sample i <- draw i) and
+// then draw[4u + 3] times for the samples of its last frame, from sample draw[4u] on (fe_end_utt).
+// The twist of 624 words runs in three barrier-separated phases: words < 227 read only old
+// words, words < 454 read the first phase's, the rest read the second's (and word 0).
+constexpr int MT_N = 624, MT_M = 397, FE_DITHER_THREADS = 640;
+
+__global__ void __launch_bounds__(FE_DITHER_THREADS)
+fe_dither_kernel(const int16_t *__restrict__ pcm, const int64_t *__restrict__ samp_off,
+                 const int32_t *__restrict__ sess_off, const int64_t *__restrict__ draw,
+                 psb_fe_state_t *__restrict__ state, int16_t *__restrict__ dpcm, int16_t *__restrict__ tail)
+{
+    __shared__ uint32_t mt[MT_N];
+    const int s = blockIdx.x, tid = threadIdx.x;
+    psb_fe_state_t *st = state + s;
+    for (int i = tid; i < MT_N; i += blockDim.x) mt[i] = st->mt[i];
+    int mti = st->mt_index;
+    __syncthreads();
+    for (int u = sess_off[s]; u < sess_off[s + 1]; ++u) {
+        const int64_t s0 = samp_off[u];
+        for (int part = 0; part < 2; ++part) {
+            const int64_t n = draw[4 * u + 2 + part];
+            const int16_t *in = part ? pcm + s0 + draw[4 * u] : pcm + s0;
+            int16_t *out = part ? tail + draw[4 * u + 1] : dpcm + s0;
+            for (int64_t done = 0; done < n;) {
+                if (mti >= MT_N) {
+                    if (mti == MT_N + 1) {                       // never seeded: init_genrand(5489)
+                        if (tid == 0) {
+                            mt[0] = 5489u;
+                            for (int i = 1; i < MT_N; ++i) mt[i] = 1812433253u * (mt[i - 1] ^ (mt[i - 1] >> 30)) + (uint32_t)i;
+                        }
+                        __syncthreads();
+                    }
+                    for (int ph = 0; ph < 3; ++ph) {
+                        const int lo = ph == 0 ? 0 : ph == 1 ? MT_N - MT_M : 2 * (MT_N - MT_M);
+                        const int hi = ph == 0 ? MT_N - MT_M : ph == 1 ? 2 * (MT_N - MT_M) : MT_N;
+                        const int kk = lo + tid;
+                        uint32_t v = 0;
+                        if (kk < hi) {
+                            const uint32_t y = (mt[kk] & 0x80000000u) | (mt[kk + 1 < MT_N ? kk + 1 : 0] & 0x7fffffffu);
+                            v = mt[kk + MT_M < MT_N ? kk + MT_M : kk + MT_M - MT_N] ^ (y >> 1) ^ ((y & 1u) ? 0x9908b0dfu : 0u);
+                        }
+                        __syncthreads();
+                        if (kk < hi) mt[kk] = v;
+                        __syncthreads();
+                    }
+                    mti = 0;
+                }
+                const int64_t chunk = min((int64_t)(MT_N - mti), n - done);
+                if (tid < chunk) {
+                    uint32_t y = mt[mti + tid];
+                    y ^= y >> 11;
+                    y ^= (y << 7) & 0x9d2c5680u;
+                    y ^= (y << 15) & 0xefc60000u;
+                    y ^= y >> 18;
+                    const int add = ((y >> 1) & 3u) == 0;        // !(genrand_int31() % 4)
+                    const int64_t j = done + tid;
+                    out[j] = (int16_t)(in[j] + add);             // int16 wrap, as fe_read_frame_int16
+                }
+                mti += (int)chunk;
+                done += chunk;
+            }
+        }
+    }
+    __syncthreads();
+    for (int i = tid; i < MT_N; i += blockDim.x) st->mt[i] = mt[i];
+    if (tid == 0) st->mt_index = mti;
+}
+
+// One warp per session, one lane per coefficient: cmn_live over each utterance's frames in order
+// (frames with c0 < 0 are skipped), then cmn_live_shiftwin when more than CMN_WIN_HWM frames are
+// counted and cmn_live_update (feat_cmn with endutt).  ps_end_utt's feat_update_stats repeats the
+// update, which leaves the state as it is.
+__global__ void __launch_bounds__(32)
+fe_cmn_live_kernel(const int32_t *__restrict__ sess_off, const int32_t *__restrict__ frame_off,
+                   float *__restrict__ mfcc, int nc, psb_fe_state_t *__restrict__ state)
+{
+    constexpr int CMN_WIN = 500, CMN_WIN_HWM = 800;
+    psb_fe_state_t *st = state + blockIdx.x;
+    const int c = threadIdx.x;
+    const bool on = c < nc;
+    float mean = on ? st->cmn_mean[c] : 0.f, sum = on ? st->cmn_sum[c] : 0.f;
+    int nframe = st->cmn_nframe;
+    for (int u = sess_off[blockIdx.x]; u < sess_off[blockIdx.x + 1]; ++u) {
+        for (int f = frame_off[u]; f < frame_off[u + 1]; ++f) {
+            float *row = mfcc + (size_t)f * nc;
+            if (row[0] < 0) continue;
+            if (on) {
+                const float v = row[c];
+                sum = __fadd_rn(sum, v);
+                row[c] = __fsub_rn(v, mean);
+            }
+            ++nframe;
+        }
+        if (nframe > CMN_WIN_HWM) {                                      // cmn_live_shiftwin
+            const float sf = (float)(1.0 / nframe);
+            mean = __fdiv_rn(sum, (float)nframe);
+            sum = __fmul_rn(sum, __fmul_rn((float)CMN_WIN, sf));
+            nframe = CMN_WIN;
+        }
+        if (nframe > 0) mean = __fdiv_rn(sum, (float)nframe);           // cmn_live_update
+    }
+    if (on) { st->cmn_mean[c] = mean; st->cmn_sum[c] = sum; }
+    if (c == 0) st->cmn_nframe = nframe;
+}
+
+// The dynamic features of every frame from its utterance's cepstra (after CMN), one thread per
+// (frame, coefficient); frames past either end of the utterance are copies of its first / last
+// (feat_s2mfc2feat_live with beginutt and endutt).
+__global__ void fe_feat_kernel(const int32_t *__restrict__ frame_off, const int32_t *__restrict__ frame_utt,
+                               const float *__restrict__ mfcc, float *__restrict__ feats, int nc, int feat, int dim,
+                               int32_t total)
+{
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (int64_t)total * nc) return;
+    const int f = (int)(i / nc), c = (int)(i % nc);
+    const int u = frame_utt[f], f0 = frame_off[u], T = frame_off[u + 1] - f0, t = f - f0;
+    const float *base = mfcc + (size_t)f0 * nc + c;
+#define CEP(dt) base[(size_t)min(max(t + (dt), 0), T - 1) * nc]
+    float *o = feats + (size_t)f * dim;
+    const float dd = __fsub_rn(__fsub_rn(CEP(3), CEP(-1)), __fsub_rn(CEP(1), CEP(-3)));
+    if (feat == PSB_FEAT_1S_C_D_DD) {                                    // feat.c:579-622
+        o[c] = CEP(0);
+        o[nc + c] = __fsub_rn(CEP(2), CEP(-2));
+        o[2 * nc + c] = dd;
+    }
+    else if (c == 0) {                                                   // POW: C0, DC0, D2C0
+        float *pw = o + (feat == PSB_FEAT_S2_4X ? 36 : 24);
+        pw[0] = CEP(0);
+        pw[1] = __fsub_rn(CEP(2), CEP(-2));
+        pw[2] = dd;
+    }
+    else if (feat == PSB_FEAT_S2_4X) {                                   // feat.c:425-484
+        o[c - 1] = CEP(0);
+        o[12 + c - 1] = __fsub_rn(CEP(2), CEP(-2));
+        o[24 + c - 1] = __fsub_rn(CEP(4), CEP(-4));
+        o[51 - 12 + c - 1] = dd;
+    }
+    else {                                                               // s3_1x39, feat.c:487-538
+        o[c - 1] = CEP(0);
+        o[12 + c - 1] = __fsub_rn(CEP(2), CEP(-2));
+        o[27 + c - 1] = dd;
+    }
+#undef CEP
+}
+
 static FeDev dev_fe(const psb_fe_t *fe)
 {
     FeDev p;
@@ -360,6 +527,7 @@ extern "C" void psb_fe_free(psb_fe_t *fe)
     cudaFree(fe->d_filt_start); cudaFree(fe->d_filt_width); cudaFree(fe->d_filt_coeffs); cudaFree(fe->d_mel_cosine);
     cudaFree(fe->d_lifter); cudaFree(fe->d_rev); cudaFree(fe->d_mfspec); cudaFree(fe->d_mfcc); cudaFree(fe->d_pcm);
     cudaFree(fe->d_feats); cudaFree(fe->d_samp_off); cudaFree(fe->d_frame_off); cudaFree(fe->d_frame_utt);
+    cudaFree(fe->d_state); cudaFree(fe->d_sess_off); cudaFree(fe->d_draw); cudaFree(fe->d_dpcm); cudaFree(fe->d_tail);
     if (fe->ev[0]) cudaEventDestroy(fe->ev[0]);
     if (fe->ev[1]) cudaEventDestroy(fe->ev[1]);
     if (fe->stream) cudaStreamDestroy(fe->stream);
@@ -368,6 +536,11 @@ extern "C" void psb_fe_free(psb_fe_t *fe)
 
 extern "C" int psb_fe_create(const psb_fe_desc_t *d, int device, psb_fe_t **out)
 {
+    return psb_fe_create_ex(d, nullptr, device, out);
+}
+
+extern "C" int psb_fe_create_ex(const psb_fe_desc_t *d, const psb_fe_opts_t *o, int device, psb_fe_t **out)
+{
     PSB_REQUIRE(d && out, "psb_fe_create: bad argument");
     PSB_REQUIRE(d->frame_size > 1 && d->frame_shift > 0 && d->frame_size >= d->frame_shift, "psb_fe_create: bad frame size / shift");
     PSB_REQUIRE(d->fft_size == (1 << d->fft_order) && d->fft_size >= d->frame_size && d->fft_size >= 8 && d->fft_size <= 1024,
@@ -375,8 +548,19 @@ extern "C" int psb_fe_create(const psb_fe_desc_t *d, int device, psb_fe_t **out)
     PSB_REQUIRE(d->n_filt > 0 && d->n_filt <= FE_MAX_FILT && d->n_cep > 0 && d->n_cep <= FE_MAX_CEP && d->n_cep <= d->n_filt,
                 "psb_fe_create: need n_cep <= n_filt <= %d and n_cep <= %d", FE_MAX_FILT, FE_MAX_CEP);
     PSB_REQUIRE(d->transform >= 0 && d->transform <= 2, "psb_fe_create: transform must be 0 (legacy), 1 (dct) or 2 (htk)");
-    PSB_REQUIRE(d->cmn == 0 || d->cmn == 1, "psb_fe_create: cmn must be 0 (none) or 1 (batch); live CMN is a host-side recurrence over utterances");
-    PSB_REQUIRE(d->window == 3, "psb_fe_create: only the 1s_c_d_dd feature type (window 3) is built");
+    if (!o) {
+        PSB_REQUIRE(d->cmn == 0 || d->cmn == 1, "psb_fe_create: cmn must be 0 (none) or 1 (batch); live CMN needs psb_fe_create_ex");
+        PSB_REQUIRE(d->window == 3, "psb_fe_create: only the 1s_c_d_dd feature type (window 3) is built; s2_4x and s3_1x39 need psb_fe_create_ex");
+    }
+    else {
+        PSB_REQUIRE(o->feat >= PSB_FEAT_1S_C_D_DD && o->feat <= PSB_FEAT_S3_1X39,
+                    "psb_fe_create_ex: feat must be 0 (1s_c_d_dd), 1 (s2_4x) or 2 (s3_1x39)");
+        PSB_REQUIRE(o->feat == PSB_FEAT_1S_C_D_DD || d->n_cep == 13, "psb_fe_create_ex: s2_4x and s3_1x39 need n_cep 13 (got %d)", d->n_cep);
+        PSB_REQUIRE(o->cmn >= PSB_CMN_NONE && o->cmn <= PSB_CMN_LIVE, "psb_fe_create_ex: cmn must be 0 (none), 1 (batch) or 2 (live)");
+        PSB_REQUIRE(!o->varnorm, o->cmn == PSB_CMN_LIVE ? "psb_fe_create_ex: variance normalization is not implemented in live mode"
+                                                        : "psb_fe_create_ex: variance normalization is not implemented");
+        PSB_REQUIRE(o->dither == 0 || o->dither == 1, "psb_fe_create_ex: dither must be 0 or 1");
+    }
     PSB_REQUIRE(d->hamming && d->ccc && d->sss && d->spec_start && d->filt_start && d->filt_width && d->filt_coeffs &&
                 d->mel_cosine && (d->lifter_val == 0 || d->lifter), "psb_fe_create: missing table");
     int n_coeffs = 0;
@@ -392,6 +576,13 @@ extern "C" int psb_fe_create(const psb_fe_desc_t *d, int device, psb_fe_t **out)
     fe->frame_size = d->frame_size; fe->frame_shift = d->frame_shift; fe->fft_size = d->fft_size; fe->fft_order = d->fft_order;
     fe->n_filt = d->n_filt; fe->n_cep = d->n_cep; fe->remove_dc = d->remove_dc; fe->remove_noise = d->remove_noise;
     fe->transform = d->transform; fe->lifter_val = d->lifter_val; fe->window = d->window; fe->cmn = d->cmn;
+    fe->feat = PSB_FEAT_1S_C_D_DD; fe->seed = -1;
+    if (o) {
+        fe->feat = o->feat; fe->cmn = o->cmn; fe->dither = o->dither; fe->seed = o->seed;
+        fe->window = o->feat == PSB_FEAT_S2_4X ? 4 : 3;
+        memcpy(fe->cmn_init, o->cmn_init, sizeof(fe->cmn_init));
+    }
+    fe->feat_dim = fe->feat == PSB_FEAT_S2_4X ? 51 : 3 * fe->n_cep;
     fe->n_coeffs = n_coeffs; fe->alpha = d->pre_emphasis_alpha; fe->sqrt_inv_n = d->sqrt_inv_n; fe->sqrt_inv_2n = d->sqrt_inv_2n;
     std::vector<int> rev((size_t)d->fft_size);
     for (int i = 0; i < d->fft_size; ++i) {
@@ -432,9 +623,40 @@ extern "C" int32_t psb_fe_n_frames(const psb_fe_t *fe, int64_t n_samples)
     return (int32_t)(full + 1);
 }
 
+static void state_init(const psb_fe_t *fe, psb_fe_state_t *s)
+{
+    // cmn_set_repr (cmn.c:119-146) and init_genrand((unsigned long)seed) (genrand.c)
+    memset(s, 0, sizeof(*s));
+    for (int i = 0; i < fe->n_cep; ++i) {
+        s->cmn_mean[i] = fe->cmn_init[i];
+        s->cmn_sum[i] = fe->cmn_init[i] * 500;
+    }
+    s->cmn_nframe = 500;
+    s->mt[0] = (uint32_t)fe->seed;
+    for (int i = 1; i < 624; ++i) s->mt[i] = 1812433253u * (s->mt[i - 1] ^ (s->mt[i - 1] >> 30)) + (uint32_t)i;
+    s->mt_index = 624;
+}
+
 static int fe_run(psb_fe_t *fe, const int16_t *d_pcm, const int64_t *samp_off, int32_t n_utt, float *d_feats,
                   float *d_mfcc_out, int32_t *frame_off, float *ms)
 {
+    // sessions: the ones psb_fe_set_sessions named for this call, else one per utterance
+    const bool pending = fe->sess_pending;
+    fe->sess_pending = false;
+    if (pending) {
+        PSB_REQUIRE(fe->sess_off.back() == n_utt, "psb_fe: the sessions cover %d utterances, the call has %d", fe->sess_off.back(), n_utt);
+    }
+    else {
+        fe->sess_off.resize((size_t)n_utt + 1);
+        for (int u = 0; u <= n_utt; ++u) fe->sess_off[(size_t)u] = u;
+        fe->states.clear();
+    }
+    const int32_t n_sess = (int32_t)fe->sess_off.size() - 1;
+    const bool live = fe->cmn == PSB_CMN_LIVE, stateful = live || fe->dither;
+    if (stateful && fe->states.empty()) {
+        fe->states.resize((size_t)n_sess);
+        for (auto &st : fe->states) state_init(fe, &st);
+    }
     std::vector<int32_t> foff((size_t)n_utt + 1);
     foff[0] = 0;
     for (int u = 0; u < n_utt; ++u) {
@@ -446,7 +668,8 @@ static int fe_run(psb_fe_t *fe, const int16_t *d_pcm, const int64_t *samp_off, i
     const int32_t total = foff[(size_t)n_utt];
     if (frame_off) memcpy(frame_off, foff.data(), foff.size() * sizeof(int32_t));
     if (ms) *ms = 0.f;
-    if (total == 0) return PSB_OK;
+    // live CMN updates its state even after an utterance without frames (cmn_live_update)
+    if (total == 0 && !(live && n_sess > 0)) return PSB_OK;
     std::vector<int32_t> futt((size_t)total);
     for (int u = 0; u < n_utt; ++u)
         for (int32_t f = foff[(size_t)u]; f < foff[(size_t)u + 1]; ++f) futt[(size_t)f] = u;
@@ -459,23 +682,79 @@ static int fe_run(psb_fe_t *fe, const int16_t *d_pcm, const int64_t *samp_off, i
         PSB_CUDA(cudaMalloc((void **)&fe->d_samp_off, fe->utt_cap * 8));
         PSB_CUDA(cudaMalloc((void **)&fe->d_frame_off, fe->utt_cap * 4));
     }
-    if (!rc) rc = grow(&fe->d_frame_utt, &fe->fu_cap, (size_t)total);
+    if (!rc) rc = grow(&fe->d_frame_utt, &fe->fu_cap, (size_t)std::max(total, 1));
+    // dither: per utterance the first sample of its last frame, where its copy goes, and the draws
+    // of fe_process_frames (every sample the full frames read) and of fe_end_utt (the last frame's)
+    std::vector<int64_t> draw;
+    int64_t n_tail = 0;
+    if (fe->dither) {
+        draw.resize((size_t)n_utt * 4);
+        for (int u = 0; u < n_utt; ++u) {
+            const int64_t n = samp_off[u + 1] - samp_off[u];
+            const int64_t full = n >= fe->frame_size ? 1 + (n - fe->frame_size) / fe->frame_shift : 0;
+            const int64_t main = full ? fe->frame_size + (full - 1) * fe->frame_shift : 0;
+            const int64_t t0 = full * fe->frame_shift;
+            draw[4 * (size_t)u] = t0;
+            draw[4 * (size_t)u + 1] = n_tail;
+            draw[4 * (size_t)u + 2] = main;
+            draw[4 * (size_t)u + 3] = n > 0 ? n - t0 : 0;
+            n_tail += draw[4 * (size_t)u + 3];
+        }
+        if (!rc) rc = grow(&fe->d_draw, &fe->draw_cap, draw.size() + 1);
+        if (!rc) rc = grow(&fe->d_dpcm, &fe->dpcm_cap, (size_t)std::max<int64_t>(samp_off[n_utt], 1));
+        if (!rc) rc = grow(&fe->d_tail, &fe->tail_cap, (size_t)std::max<int64_t>(n_tail, 1));
+    }
+    if (stateful) {
+        if (!rc) rc = grow(&fe->d_state, &fe->state_cap, (size_t)n_sess);
+        if (!rc) rc = grow(&fe->d_sess_off, &fe->sess_cap, (size_t)n_sess + 1);
+    }
     if (rc) return rc;
     PSB_CUDA(cudaMemcpyAsync(fe->d_samp_off, samp_off, ((size_t)n_utt + 1) * 8, cudaMemcpyHostToDevice, fe->stream));
     PSB_CUDA(cudaMemcpyAsync(fe->d_frame_off, foff.data(), foff.size() * 4, cudaMemcpyHostToDevice, fe->stream));
-    PSB_CUDA(cudaMemcpyAsync(fe->d_frame_utt, futt.data(), futt.size() * 4, cudaMemcpyHostToDevice, fe->stream));
+    if (total) PSB_CUDA(cudaMemcpyAsync(fe->d_frame_utt, futt.data(), futt.size() * 4, cudaMemcpyHostToDevice, fe->stream));
+    if (fe->dither) PSB_CUDA(cudaMemcpyAsync(fe->d_draw, draw.data(), draw.size() * 8, cudaMemcpyHostToDevice, fe->stream));
+    if (stateful) {
+        PSB_CUDA(cudaMemcpyAsync(fe->d_state, fe->states.data(), (size_t)n_sess * sizeof(psb_fe_state_t), cudaMemcpyHostToDevice, fe->stream));
+        PSB_CUDA(cudaMemcpyAsync(fe->d_sess_off, fe->sess_off.data(), ((size_t)n_sess + 1) * 4, cudaMemcpyHostToDevice, fe->stream));
+    }
     const FeDev p = dev_fe(fe);
     const size_t smem = ((size_t)fe->fft_size + fe->fft_size / 2 + 1) * sizeof(double);
+    // the features of 1s_c_d_dd without live CMN come out of fe_utt_kernel; every other
+    // configuration normalises and builds them in the kernels behind it
+    const bool utt_feats = fe->feat == PSB_FEAT_1S_C_D_DD && !live;
     PSB_CUDA(cudaEventRecord(fe->ev[0], fe->stream));
-    fe_frame_kernel<<<(unsigned)total, 128, smem, fe->stream>>>(p, d_pcm, fe->d_samp_off, fe->d_frame_off, fe->d_frame_utt,
-                                                              fe->d_mfspec);
-    PSB_LAUNCH_CHECK();
-    fe_utt_kernel<<<(unsigned)n_utt, 64, 0, fe->stream>>>(p, fe->d_frame_off, fe->d_mfspec, fe->d_mfcc, d_feats, fe->cmn,
-                                                         fe->window);
-    PSB_LAUNCH_CHECK();
+    if (fe->dither && n_sess) {
+        fe_dither_kernel<<<(unsigned)n_sess, FE_DITHER_THREADS, 0, fe->stream>>>(d_pcm, fe->d_samp_off, fe->d_sess_off, fe->d_draw,
+                                                                            fe->d_state, fe->d_dpcm, fe->d_tail);
+        PSB_LAUNCH_CHECK();
+    }
+    if (total) {
+        if (fe->dither)
+            fe_frame_kernel<true><<<(unsigned)total, 128, smem, fe->stream>>>(p, fe->d_dpcm, fe->d_samp_off, fe->d_frame_off,
+                                                                            fe->d_frame_utt, fe->d_mfspec, fe->d_tail, fe->d_draw);
+        else
+            fe_frame_kernel<false><<<(unsigned)total, 128, smem, fe->stream>>>(p, d_pcm, fe->d_samp_off, fe->d_frame_off,
+                                                                             fe->d_frame_utt, fe->d_mfspec, nullptr, nullptr);
+        PSB_LAUNCH_CHECK();
+        fe_utt_kernel<<<(unsigned)n_utt, 64, 0, fe->stream>>>(p, fe->d_frame_off, fe->d_mfspec, fe->d_mfcc,
+                                                             utt_feats ? d_feats : nullptr, live ? 0 : fe->cmn, fe->window);
+        PSB_LAUNCH_CHECK();
+    }
+    if (live) {
+        fe_cmn_live_kernel<<<(unsigned)n_sess, 32, 0, fe->stream>>>(fe->d_sess_off, fe->d_frame_off, fe->d_mfcc, fe->n_cep, fe->d_state);
+        PSB_LAUNCH_CHECK();
+    }
+    if (!utt_feats && d_feats && total) {
+        const int64_t work = (int64_t)total * fe->n_cep;
+        fe_feat_kernel<<<(unsigned)((work + 255) / 256), 256, 0, fe->stream>>>(fe->d_frame_off, fe->d_frame_utt, fe->d_mfcc, d_feats,
+                                                                           fe->n_cep, fe->feat, fe->feat_dim, total);
+        PSB_LAUNCH_CHECK();
+    }
     PSB_CUDA(cudaEventRecord(fe->ev[1], fe->stream));
-    if (d_mfcc_out)
+    if (d_mfcc_out && total)
         PSB_CUDA(cudaMemcpyAsync(d_mfcc_out, fe->d_mfcc, (size_t)total * fe->n_cep * 4, cudaMemcpyDeviceToDevice, fe->stream));
+    if (stateful)
+        PSB_CUDA(cudaMemcpyAsync(fe->states.data(), fe->d_state, (size_t)n_sess * sizeof(psb_fe_state_t), cudaMemcpyDeviceToHost, fe->stream));
     PSB_CUDA(cudaStreamSynchronize(fe->stream));
     if (ms) PSB_CUDA(cudaEventElapsedTime(ms, fe->ev[0], fe->ev[1]));
     return PSB_OK;
@@ -501,12 +780,12 @@ extern "C" int psb_fe_process_host(psb_fe_t *fe, const int16_t *pcm, const int64
     int64_t total = 0;
     for (int u = 0; u < n_utt; ++u) total += psb_fe_n_frames(fe, samp_off[u + 1] - samp_off[u]);
     int rc = grow(&fe->d_pcm, &fe->pcm_cap, (size_t)std::max<int64_t>(ns, 1));
-    if (!rc) rc = grow(&fe->d_feats, &fe->feats_cap, (size_t)std::max<int64_t>(total, 1) * 3 * fe->n_cep);
+    if (!rc) rc = grow(&fe->d_feats, &fe->feats_cap, (size_t)std::max<int64_t>(total, 1) * fe->feat_dim);
     if (rc) return rc;
     if (ns) PSB_CUDA(cudaMemcpyAsync(fe->d_pcm, pcm, (size_t)ns * 2, cudaMemcpyHostToDevice, fe->stream));
     rc = fe_run(fe, fe->d_pcm, samp_off, n_utt, fe->d_feats, nullptr, frame_off, nullptr);
     if (rc) return rc;
-    if (total && feats) PSB_CUDA(cudaMemcpy(feats, fe->d_feats, (size_t)total * 3 * fe->n_cep * 4, cudaMemcpyDeviceToHost));
+    if (total && feats) PSB_CUDA(cudaMemcpy(feats, fe->d_feats, (size_t)total * fe->feat_dim * 4, cudaMemcpyDeviceToHost));
     if (total && mfcc) PSB_CUDA(cudaMemcpy(mfcc, fe->d_mfcc, (size_t)total * fe->n_cep * 4, cudaMemcpyDeviceToHost));
     return PSB_OK;
 }
@@ -518,5 +797,41 @@ extern "C" const float *psb_fe_device_feats(const psb_fe_t *fe)
 
 extern "C" int32_t psb_fe_feat_dim(const psb_fe_t *fe)
 {
-    return fe ? 3 * fe->n_cep : 0;
+    return fe ? fe->feat_dim : 0;
+}
+
+extern "C" int psb_fe_state_init(const psb_fe_t *fe, psb_fe_state_t *s)
+{
+    PSB_REQUIRE(fe && s, "psb_fe_state_init: bad argument");
+    state_init(fe, s);
+    return PSB_OK;
+}
+
+extern "C" int psb_fe_set_sessions(psb_fe_t *fe, const int32_t *sess_off, int32_t n_sess, const psb_fe_state_t *states_in)
+{
+    PSB_REQUIRE(fe && sess_off && n_sess >= 0, "psb_fe_set_sessions: bad argument");
+    PSB_REQUIRE(sess_off[0] == 0, "psb_fe_set_sessions: sess_off[0] must be 0");
+    for (int s = 0; s < n_sess; ++s)
+        PSB_REQUIRE(sess_off[s + 1] >= sess_off[s], "psb_fe_set_sessions: sess_off not monotone at %d", s);
+    if (states_in)
+        for (int s = 0; s < n_sess; ++s)
+            PSB_REQUIRE(states_in[s].mt_index >= 0 && states_in[s].mt_index <= 625 && states_in[s].cmn_nframe >= 0,
+                        "psb_fe_set_sessions: state %d is not a front-end state", s);
+    fe->sess_off.assign(sess_off, sess_off + n_sess + 1);
+    fe->states.clear();
+    if (states_in) fe->states.assign(states_in, states_in + n_sess);
+    fe->sess_pending = true;
+    return PSB_OK;
+}
+
+extern "C" int psb_fe_get_states(const psb_fe_t *fe, psb_fe_state_t *states_out, int32_t n_sess)
+{
+    PSB_REQUIRE(fe && states_out && n_sess >= 0, "psb_fe_get_states: bad argument");
+    PSB_REQUIRE(!fe->sess_off.empty() && n_sess == (int32_t)fe->sess_off.size() - 1,
+                "psb_fe_get_states: the last call had %d sessions", fe->sess_off.empty() ? 0 : (int)fe->sess_off.size() - 1);
+    for (int s = 0; s < n_sess; ++s) {
+        if (fe->states.empty()) state_init(fe, &states_out[s]);     // nothing carried: the state is the initial one
+        else states_out[s] = fe->states[(size_t)s];
+    }
+    return PSB_OK;
 }

@@ -13,12 +13,12 @@ import os
 import numpy as np
 
 from . import api, lextree
-from .fe_tables import make_fe_desc
+from .fe_tables import CMN_TYPES, FEAT_TYPES, make_fe_desc, make_fe_opts
 from .model import PackedModel
 
 # config_macro.h (the reference's defaults for every front-end / feature key this class looks at)
 FE_REFERENCE_DEFAULTS = dict(feat="1s_c_d_dd", cmn="live", agc="none", varnorm="no", lda="", svspec="", dither="no",
-                             round_filters="yes", ncep="13", frate="100", nfft="0", cmninit="40,3,-1", samprate="16000",
+                             round_filters="yes", ncep="13", frate="100", nfft="0", cmninit="40,3,-1", seed="-1", samprate="16000",
                              wlen="0.025625", nfilt="40", lowerf="133.33334", upperf="6855.4976", alpha="0.97",
                              transform="legacy", lifter="0", remove_noise="no", remove_dc="no", unit_area="yes", doublebw="no")
 PL_DEFAULTS = dict(pl_window="5", pl_beam="1e-10", pl_pbeam="1e-10", pl_pip="1.0", pl_weight="3.0")
@@ -39,28 +39,28 @@ class Decoder:
         fp.update(read_feat_params(os.path.join(hmm, "feat.params")))
         fp.update({k: v for k, v in cfg.items() if k in FE_REFERENCE_DEFAULTS})
         yes = ("yes", "1", "true", "True")
-        if fp["cmn"] == "current":                       # the reference's alias for batch (cmn.c: cmn_type_str)
-            fp["cmn"] = "batch"
         unsupported = []
-        if fp["feat"] != "1s_c_d_dd": unsupported.append("-feat " + fp["feat"])
-        if fp["cmn"] != "batch": unsupported.append("-cmn " + fp["cmn"])
+        if fp["feat"] not in FEAT_TYPES: unsupported.append("-feat " + fp["feat"])
+        if fp["cmn"] not in CMN_TYPES: unsupported.append("-cmn " + fp["cmn"])
         if fp["agc"] != "none": unsupported.append("-agc " + fp["agc"])
         if fp["varnorm"] in yes: unsupported.append("-varnorm yes")
         if fp["lda"]: unsupported.append("-lda")
         if fp["svspec"] not in ("", "0-12/13-25/26-38"): unsupported.append("-svspec " + fp["svspec"])
-        if fp["dither"] in yes: unsupported.append("-dither yes")
-        if fp["round_filters"] not in yes: unsupported.append("-round_filters no")
         if int(fp["ncep"]) != 13: unsupported.append("-ncep " + fp["ncep"])
         if int(fp["frate"]) != 100: unsupported.append("-frate " + fp["frate"])
         if int(fp["nfft"]) != 0: unsupported.append("-nfft " + fp["nfft"])
-        if fp["cmninit"] not in ("", FE_REFERENCE_DEFAULTS["cmninit"]) and fp["cmn"] != "batch": unsupported.append("-cmninit")
         if unsupported:
             raise NotImplementedError("front end settings the device front end does not implement: " + ", ".join(unsupported))
-        self.fe = api.FrontEnd(make_fe_desc(samprate=float(fp["samprate"]), wlen=float(fp["wlen"]), nfilt=int(fp["nfilt"]),
-                                            lowerf=float(fp["lowerf"]), upperf=float(fp["upperf"]), alpha=float(fp["alpha"]),
-                                            transform=fp["transform"], lifter=int(fp["lifter"]), remove_noise=fp["remove_noise"] in yes,
-                                            remove_dc=fp["remove_dc"] in yes, unit_area=fp["unit_area"] in yes,
-                                            doublebw=fp["doublebw"] in yes), device)
+        opts = make_fe_opts(feat=fp["feat"], cmn=fp["cmn"], cmninit=fp["cmninit"], dither=fp["dither"] in yes,
+                            seed=int(fp["seed"]), ncep=int(fp["ncep"]))
+        desc = make_fe_desc(samprate=float(fp["samprate"]), wlen=float(fp["wlen"]), nfilt=int(fp["nfilt"]),
+                            lowerf=float(fp["lowerf"]), upperf=float(fp["upperf"]), alpha=float(fp["alpha"]),
+                            transform=fp["transform"], lifter=int(fp["lifter"]), remove_noise=fp["remove_noise"] in yes,
+                            remove_dc=fp["remove_dc"] in yes, unit_area=fp["unit_area"] in yes,
+                            round_filters=fp["round_filters"] in yes, doublebw=fp["doublebw"] in yes)
+        # 1s_c_d_dd with batch CMN and no dither is the front end desc alone describes
+        plain = (opts["feat"], opts["cmn"], opts["dither"]) == (0, 1, 0)
+        self.fe = api.FrontEnd(desc, device) if plain else api.FrontEnd(desc, device, opts)
         search_cfg = {k: v for k, v in cfg.items() if k in lextree.DEFAULTS}
         self.search = lextree.ngram_search_from_files(hmm, dict_file, lm_file, **search_cfg)
         self.model = api.Model(self.pm, device)
@@ -77,14 +77,34 @@ class Decoder:
         self.second_pass = search_cfg.get("fwdflat", "yes") in ("yes", "1", "true", "True")
         self.bp_cap = int(cfg.get("latsize", 5000))
 
-    def decode_raw_batch(self, utterances):
-        """utterances: int16 arrays, each a whole utterance.  Returns one dict per utterance: hyp (the words, fillers
-        and <s> / </s> left out), score, seg [n][7] = entry, wid, sf, ef, path score, ascr, lscr, and words()."""
+    def decode_raw_batch(self, utterances, sessions=None):
+        """utterances: int16 arrays, each a whole utterance.  sessions: None (every utterance a fresh decoder) or one
+        session id per utterance; the utterances of one id are one decoder's, in list order, from a fresh decoder
+        (the front end's live CMN and dither state carry over).  Returns one dict per utterance: hyp (the words,
+        fillers and <s> / </s> left out), score, seg [n][7] = entry, wid, sf, ef, path score, ascr, lscr, and words()."""
+        if sessions is None:
+            return self._decode(utterances, None)
+        assert len(sessions) == len(utterances)
+        first = {}
+        for i, sid in enumerate(sessions):
+            first.setdefault(sid, i)
+        # the front end wants each session's utterances consecutive, in decode order
+        order = sorted(range(len(utterances)), key=lambda i: (first[sessions[i]], i))
+        sizes = [sessions.count(sid) for sid in sorted(first, key=first.get)]
+        res = self._decode([utterances[i] for i in order], np.cumsum([0] + sizes))
+        out = [None] * len(utterances)
+        for j, i in enumerate(order):
+            out[i] = res[j]
+        return out
+
+    def _decode(self, utterances, sess_off):
         import torch
         g = self.search
         info = g["info"]
         off = api.FrontEnd.sample_offsets([len(u) for u in utterances])
         pcm = np.concatenate([np.ascontiguousarray(u, np.int16) for u in utterances]) if utterances else np.zeros(0, np.int16)
+        if sess_off is not None:
+            self.fe.set_sessions(sess_off)
         frame_off, best, pen = self.batch.decode_pcm_host(self.fe, self.phoneloop, pcm, off)
         d_scr = self.batch.senscr_device_ptr()
         d_pen = (torch.from_numpy(np.ascontiguousarray(pen, np.int32)).to(torch.device("cuda", self.device))
