@@ -526,6 +526,7 @@ extern "C" int psb_phoneloop_run_host(psb_phoneloop_t *p, const int16_t *senscr,
 // never reach the best score.
 constexpr int HS_V = 4;                     // instances per thread
 constexpr int HS_TS = 512;                  // storage tile: [tile][field][HS_TS], so a CTA's fields are one contiguous block
+constexpr int SWEEP_FR = 2;                 // hmmset_sweep_kernel: frames per block barrier (2 * SWEEP_FR score rows in flight)
 // threads per CTA: 128 (default) or 256 (PSB_HMMSET_THREADS)
 
 struct psb_hmmset_s {
@@ -784,14 +785,16 @@ hmmset_eval_kernel(HmmSetDev s, HmmCtxDev c, const int16_t *__restrict__ senscr,
 // frames -- evaluate_channels over a fixed active set, ngram_search_fwdtree.c:702-715 -- a CTA can
 // keep its slice of a segment (THREADS x V instances) in REGISTERS for the whole utterance and
 // only the segment's int16 score row of each frame has to arrive: 2 * n_sen bytes per frame,
-// staged by the TMA unit (cp.async.bulk global -> shared, completion on an mbarrier) two frames
-// ahead into a double buffer, so that the copy of frame t+2 overlaps the arithmetic of frames t
-// and t+1.  One elected thread arms the barrier and issues the copy; everybody waits on the
+// staged by the TMA unit (cp.async.bulk global -> shared, completion on an mbarrier) 2 * SWEEP_FR
+// frames ahead, so that the copies of the next SWEEP_FR frames overlap the arithmetic of the
+// current ones.  One elected thread arms the barrier and issues the copy; everybody waits on the
 // barrier's phase.  Bulk copies need 16-byte aligned source, destination and size: the copy
 // starts at the row's address rounded down to 16 and ends at its end rounded up, the row is read
 // at its offset inside the buffer; the matrix's LAST row is copied by the threads themselves so
-// that nothing past the allocation is touched.  Per frame one block-wide max (REDUX + one
-// shared-memory hop) and one atomicMax per CTA into best[t][segment].  Results are bit-identical
+// that nothing past the allocation is touched.  Per frame one warp max (REDUX) into a shared slot;
+// one block barrier per SWEEP_FR frames, after which warp 0 reduces the slots and issues one
+// atomicMax per frame and CTA into best[t][segment].  The 3-state step runs on per-instance
+// constants decoded before the frame loop (hmm_step_3st_dec).  Results are bit-identical
 // to n_frames calls of hmmset_eval_kernel (tests/test_gpu_parity.py).
 //
 // BEAM: the same sweep with the beam pruning of prune_channels between frames (ngram_search_fwdtree.c:1130-1181 and the
@@ -828,20 +831,23 @@ __device__ __forceinline__ void cluster_sync_all()
 }
 
 template <int NS, int V, int THREADS, bool BEAM>
-__global__ void __launch_bounds__(THREADS)
+__global__ void __launch_bounds__(THREADS, BEAM ? 1 : 2)
 hmmset_sweep_kernel(HmmSetDev s, HmmCtxDev c, const int16_t *__restrict__ senscr, long long rows_total,
                     const int64_t *__restrict__ row0, const int32_t *__restrict__ n_rows, int n_frames,
                     int32_t *__restrict__ best_out, int n_tmat, int buf_bytes, int frame0, int beam, int maxhmmpf,
                     int32_t *__restrict__ n_active_out)
 {
     static_assert(!BEAM || THREADS == 256, "the histogram walk maps one bin to one thread");
-    // score rows in flight: two for the plain sweep (its frame is longer than half a bulk copy's latency), six under the
-    // beam, where a CTA whose instances have mostly left runs ahead of the copies (the floor of the
-    // pruned sweep is the per-frame exchange, DESIGN 4.19)
-    constexpr int NBUF = BEAM ? 6 : 2;
+    // frames per block barrier: FR for the plain sweep (its warps run FR frames apart at most and leave their per-frame
+    // maxima in double-buffered slots), one under the beam, whose pruning needs every frame's segment maximum
+    constexpr int FR = BEAM ? 1 : SWEEP_FR;
+    // score rows in flight: 2 * FR for the plain sweep (the copies of the next FR frames run while the current FR are
+    // evaluated), six under the beam, where a CTA whose instances have mostly left runs ahead of the copies (the floor
+    // of the pruned sweep is the per-frame exchange, DESIGN 4.19)
+    constexpr int NBUF = BEAM ? 6 : 2 * FR;
     extern __shared__ __align__(128) unsigned char sw_smem[];       // [NBUF][buf_bytes] score rows, then the transition matrices
     __shared__ __align__(8) uint64_t full[NBUF];
-    __shared__ int red[2][THREADS / 32];
+    __shared__ int red[2 * FR][THREADS / 32];
     __shared__ int redc[BEAM ? 2 : 1][THREADS / 32];
     __shared__ __align__(8) int2 cl_slot[BEAM ? 2 : 1][16];                 // [parity][rank in the cluster] {maximum, count}, written by the peers
     __shared__ __align__(8) uint64_t xbar[2];                               // ... whose arrival these count
@@ -869,47 +875,54 @@ hmmset_sweep_kernel(HmmSetDev s, HmmCtxDev c, const int16_t *__restrict__ senscr
     uint8_t *tps = sw_smem + NBUF * (size_t)buf_bytes;
     for (int q = tid; q < n_tmat * NS * (NS + 1); q += THREADS) tps[q] = c.tp[q];
 
-    // this thread's V instances (THREADS apart: neighbouring threads read neighbouring words)
+    // this thread's V instances (THREADS apart: neighbouring threads read neighbouring words); senone ids are kept as
+    // byte offsets into the score row
     int sc[V][NS], hi[V][NS], sid[V][NS], osc[V], ohi[V], tmo[V];
-    unsigned tpk[V][3];                                   // 3-state: the instance's 12 transition bytes in registers
-    int32_t *p32[V];
+    HmmTp3 tk[V];                                         // 3-state: the instance's transitions, decoded once
     bool live[V], act[V], touched[V];
+    const int64_t rem64 = n - j_base - tid;
+    const int rem = rem64 < 0 ? -1 : rem64 > V * THREADS ? V * THREADS : (int)rem64;   // live[v] == v * THREADS < rem
+    // instance v's int32 fields (recomputed after the frame loop rather than kept live through it)
+    auto state_i32 = [&](int v) {
+        const int64_t j = j_base + (int64_t)v * THREADS + tid;
+        const int64_t i = s.seg_base[seg] + (j < n ? j : 0);
+        return s.i32 + (i / HS_TS) * (int64_t)(2 * NS + 4) * HS_TS + (i % HS_TS);
+    };
 #pragma unroll
     for (int v = 0; v < V; ++v) {
         const int64_t j = j_base + (int64_t)v * THREADS + tid;
         live[v] = j < n;
         const int64_t i = s.seg_base[seg] + (live[v] ? j : 0);
-        const int64_t b32 = (i / HS_TS) * (int64_t)(2 * NS + 4) * HS_TS + (i % HS_TS);
         const int64_t b16 = (i / HS_TS) * (int64_t)(NS + 2) * HS_TS + (i % HS_TS);
-        p32[v] = s.i32 + b32;
+        const int32_t *p32 = state_i32(v);
         const uint16_t *p16 = s.u16 + b16;
 #pragma unroll
         for (int k = 0; k < NS; ++k) {
-            sc[v][k] = live[v] ? p32[v][k * HS_TS] : PSB_WORST_SCORE;
-            hi[v][k] = live[v] ? p32[v][(NS + k) * HS_TS] : -1;
-            sid[v][k] = live[v] ? p16[k * HS_TS] : 0;
+            sc[v][k] = live[v] ? p32[k * HS_TS] : PSB_WORST_SCORE;
+            hi[v][k] = live[v] ? p32[(NS + k) * HS_TS] : -1;
+            sid[v][k] = live[v] ? 2 * (int)p16[k * HS_TS] : 0;
         }
-        osc[v] = live[v] ? p32[v][2 * NS * HS_TS] : PSB_WORST_SCORE;
-        ohi[v] = live[v] ? p32[v][(2 * NS + 1) * HS_TS] : -1;
+        osc[v] = live[v] ? p32[2 * NS * HS_TS] : PSB_WORST_SCORE;
+        ohi[v] = live[v] ? p32[(2 * NS + 1) * HS_TS] : -1;
         tmo[v] = live[v] ? (int)(int16_t)p16[(NS + 1) * HS_TS] * NS * (NS + 1) : 0;
-        act[v] = BEAM ? (live[v] && p32[v][(2 * NS + 3) * HS_TS] == frame0) : live[v];
+        act[v] = BEAM ? (live[v] && p32[(2 * NS + 3) * HS_TS] == frame0) : live[v];
         touched[v] = act[v];
     }
     __syncthreads();                                      // the transition matrices are staged
     if (NS == 3) {
 #pragma unroll
-        for (int v = 0; v < V; ++v)
-#pragma unroll
-            for (int q = 0; q < 3; ++q) {
-                const uint8_t *t4 = tps + tmo[v] + 4 * q;
-                tpk[v][q] = (unsigned)t4[0] | ((unsigned)t4[1] << 8) | ((unsigned)t4[2] << 16) | ((unsigned)t4[3] << 24);
-            }
+        for (int v = 0; v < V; ++v) tk[v] = hmm_tp3_decode(tps + tmo[v]);
     }
     const int64_t r0 = row0 ? row0[seg] : seg;
     const int64_t rstep = row0 ? 1 : gridDim.y;
     const size_t row_bytes = (size_t)c.n_sen * 2;
     auto row_addr = [&](int t) { return reinterpret_cast<uintptr_t>(senscr + (size_t)(r0 + (int64_t)t * rstep) * c.n_sen); };
-    auto tma_ok = [&](int t) { return r0 + (int64_t)t * rstep + 1 < rows_total; };
+    // frames t < t_tma have their row staged by TMA; only the matrix's last row (if it is reached) is not
+    const int64_t lim = rows_total - 1 - r0;
+    const int t_tma = lim <= 0 ? 0 : (int)min((int64_t)T, (lim + rstep - 1) / rstep);
+    auto tma_ok = [&](int t) { return t < t_tma; };
+    // the row's offset inside its 16-byte granule, from 32-bit arithmetic (the granule only needs the low bits)
+    const unsigned a_lo0 = (unsigned)row_addr(0), a_step = (unsigned)((size_t)rstep * row_bytes);
     if (BEAM) cluster_sync_all();                         // every peer runs (its shared memory may be written) and has zeroed its histograms
     auto issue = [&](int t) {                                         // one thread: arm the barrier, start the copy
         const uintptr_t a = row_addr(t), a16 = a & ~(uintptr_t)15;
@@ -932,66 +945,80 @@ hmmset_sweep_kernel(HmmSetDev s, HmmCtxDev c, const int16_t *__restrict__ senscr
     for (int t = 0; t < T; ++t) {
         const int b = t & 1, rb = t % NBUF;
         unsigned char *buf = sw_smem + (size_t)rb * buf_bytes;
-        const uintptr_t a = row_addr(t);
         const int16_t *srow;
         if (BEAM && cta_empty)
             srow = reinterpret_cast<const int16_t *>(buf);            // nothing to evaluate
         else if (tma_ok(t)) {
             mbar_wait(&full[rb], (unsigned)(t / NBUF) & 1u);
-            srow = reinterpret_cast<const int16_t *>(buf + (a & 15));
+            srow = reinterpret_cast<const int16_t *>(buf + ((a_lo0 + (unsigned)t * a_step) & 15u));
         }
         else {                                                        // last row of the matrix: plain copy
-            const int16_t *g = reinterpret_cast<const int16_t *>(a);
+            const int16_t *g = reinterpret_cast<const int16_t *>(row_addr(t));
             int16_t *d = reinterpret_cast<int16_t *>(buf);
             for (int q = tid; q < c.n_sen; q += THREADS) d[q] = g[q];
             __syncthreads();
             srow = d;
         }
+        const unsigned char *srowb = reinterpret_cast<const unsigned char *>(srow);
+        auto score_at = [&](int off) { return (int)*reinterpret_cast<const int16_t *>(srowb + off); };
         int best = PSB_WORST_SCORE, cnt = 0;
 #pragma unroll
         for (int v = 0; v < V; ++v) {
             if (BEAM && !act[v]) continue;
             ++cnt;
-            HmmReg h;
-            int obs[PSB_HMM_MAX_NSTATE];
-#pragma unroll
-            for (int k = 0; k < PSB_HMM_MAX_NSTATE; ++k) {
-                h.score[k] = k < NS ? sc[v][k < NS ? k : 0] : PSB_WORST_SCORE;
-                h.hist[k] = k < NS ? hi[v][k < NS ? k : 0] : -1;
-                h.senid[k] = 0;
-                obs[k] = k < NS ? -(int)srow[sid[v][k < NS ? k : 0]] : 0;
-            }
-            h.out_score = osc[v]; h.out_hist = ohi[v]; h.best = PSB_WORST_SCORE;
             int bb;
             if (NS == 3) {
-                uint8_t tl[12];                                       // byte extracts from registers, no shared-memory reads
-#pragma unroll
-                for (int q = 0; q < 12; ++q) tl[q] = (uint8_t)(tpk[v][q >> 2] >> (8 * (q & 3)));
-                bb = hmm_step_3st(h, tl, obs);
+                int (&s3)[3] = *reinterpret_cast<int (*)[3]>(sc[v]);
+                int (&h3)[3] = *reinterpret_cast<int (*)[3]>(hi[v]);
+                bb = hmm_step_3st_dec(s3, h3, osc[v], ohi[v], tk[v], score_at(sid[v][0]), score_at(sid[v][1]),
+                                      score_at(sid[v][NS > 2 ? 2 : 0]));
             }
-            else
-                bb = hmm_step_5st(h, tps + tmo[v], obs);
-            if (live[v]) best = max(best, bb);
+            else {
+                HmmReg h;
+                int obs[PSB_HMM_MAX_NSTATE];
 #pragma unroll
-            for (int k = 0; k < NS; ++k) { sc[v][k] = h.score[k]; hi[v][k] = h.hist[k]; }
-            osc[v] = h.out_score; ohi[v] = h.out_hist;
+                for (int k = 0; k < PSB_HMM_MAX_NSTATE; ++k) {
+                    h.score[k] = k < NS ? sc[v][k < NS ? k : 0] : PSB_WORST_SCORE;
+                    h.hist[k] = k < NS ? hi[v][k < NS ? k : 0] : -1;
+                    h.senid[k] = 0;
+                    obs[k] = k < NS ? -score_at(sid[v][k < NS ? k : 0]) : 0;
+                }
+                h.out_score = osc[v]; h.out_hist = ohi[v]; h.best = PSB_WORST_SCORE;
+                bb = hmm_step_5st(h, tps + tmo[v], obs);
+#pragma unroll
+                for (int k = 0; k < NS; ++k) { sc[v][k] = h.score[k]; hi[v][k] = h.hist[k]; }
+                osc[v] = h.out_score; ohi[v] = h.out_hist;
+            }
+            if (v * THREADS < rem) best = max(best, bb);                // live[v], one compare
             best_final[v] = bb;
         }
         best = __reduce_max_sync(0xffffffffu, best);
         if (BEAM) cnt = __reduce_add_sync(0xffffffffu, cnt);
+        const int slot = t % (2 * FR);
         if ((tid & 31) == 0) {
-            red[b][tid >> 5] = best;
+            red[slot][tid >> 5] = best;
             if (BEAM) redc[b][tid >> 5] = cnt;
         }
-        __syncthreads();                                              // buf[b] and red[b] are complete / free
-        if (tid == 0 && t + NBUF < T && tma_ok(t + NBUF) && !cta_empty) issue(t + NBUF);
+        if (FR > 1 && t % FR != FR - 1 && t + 1 < T) continue;       // the barrier closes FR frames (or the last ones)
+        const int tf = t - t % FR;                                    // first frame this barrier closes
+        __syncthreads();                                              // frames tf..t: their rows and maxima are complete / free
+        if (tid == 0 && !cta_empty)
+#pragma unroll 1
+            for (int u = tf + NBUF; u <= t + NBUF; ++u)
+                if (u < T && tma_ok(u)) issue(u);
         if (tid < 32) {
-            int v = tid < THREADS / 32 ? red[b][tid] : PSB_WORST_SCORE;
-            v = __reduce_max_sync(0xffffffffu, v);
             if (!BEAM) {
-                if (tid == 0) atomicMax(best_out + (size_t)t * gridDim.y + seg, v);
+                // warp 0 publishes the closed frames; the warps fill the other FR slots before the next barrier
+#pragma unroll 1
+                for (int u = tf; u <= t; ++u) {
+                    int v = tid < THREADS / 32 ? red[u % (2 * FR)][tid] : PSB_WORST_SCORE;
+                    v = __reduce_max_sync(0xffffffffu, v);
+                    if (tid == 0) atomicMax(best_out + (size_t)u * gridDim.y + seg, v);
+                }
             }
             else {
+                int v = tid < THREADS / 32 ? red[slot][tid] : PSB_WORST_SCORE;
+                v = __reduce_max_sync(0xffffffffu, v);
                 int cc = tid < THREADS / 32 ? redc[b][tid] : 0;
                 cc = __reduce_add_sync(0xffffffffu, cc);
                 if (tid == 0) mbar_expect_tx(&xbar[b], n_rank * 8u);  // this frame's n_rank messages (own included)
@@ -1057,15 +1084,16 @@ hmmset_sweep_kernel(HmmSetDev s, HmmCtxDev c, const int16_t *__restrict__ senscr
 #pragma unroll
     for (int v = 0; v < V; ++v) {
         if (!live[v] || !touched[v]) continue;            // BEAM: instances that were never active stay as they are
+        int32_t *p32 = state_i32(v);
 #pragma unroll
         for (int k = 0; k < NS; ++k) {
-            p32[v][k * HS_TS] = sc[v][k];
-            p32[v][(NS + k) * HS_TS] = hi[v][k];
+            p32[k * HS_TS] = sc[v][k];
+            p32[(NS + k) * HS_TS] = hi[v][k];
         }
-        p32[v][2 * NS * HS_TS] = osc[v];
-        p32[v][(2 * NS + 1) * HS_TS] = ohi[v];
-        p32[v][(2 * NS + 2) * HS_TS] = best_final[v];
-        if (BEAM) p32[v][(2 * NS + 3) * HS_TS] = act[v] ? frame0 + T : -1;
+        p32[2 * NS * HS_TS] = osc[v];
+        p32[(2 * NS + 1) * HS_TS] = ohi[v];
+        p32[(2 * NS + 2) * HS_TS] = best_final[v];
+        if (BEAM) p32[(2 * NS + 3) * HS_TS] = act[v] ? frame0 + T : -1;
     }
 }
 
@@ -1285,11 +1313,9 @@ extern "C" int psb_hmmset_sweep_device(psb_hmmset_t *s, const int16_t *d_senscr,
         if (ms) PSB_CUDA(cudaStreamSynchronize(s->stream));
         return PSB_OK;
     }
-    // CTA shape: threads x instances per thread (PSB_SWEEP_SHAPE = 0: 256 x 4 (default), 1: 256 x 2, 3: 512 x 2; DESIGN 4.14)
-    static const int shape = [] { const char *v = getenv("PSB_SWEEP_SHAPE"); return v ? atoi(v) : 0; }();
     const int buf_bytes = (int)(((size_t)cd.n_sen * 2 + 32 + 127) & ~(size_t)127);
     const int tp_bytes = s->c->n_tmat * cd.n_emit * (cd.n_emit + 1);
-    const size_t smem = 2 * (size_t)buf_bytes + tp_bytes;
+    const size_t smem = 2 * SWEEP_FR * (size_t)buf_bytes + tp_bytes;            // NBUF of the plain instantiation
     PSB_REQUIRE(smem <= 200 * 1024, "psb_hmmset_sweep: %d senones / %d transition matrices do not fit shared memory", cd.n_sen, s->c->n_tmat);
     const HmmSetDev sd = dev_set(s);
     PSB_CUDA(cudaEventRecord(s->ev[0], s->stream));
@@ -1301,13 +1327,9 @@ extern "C" int psb_hmmset_sweep_device(psb_hmmset_t *s, const int16_t *d_senscr,
         kern<<<grid, THREADS, smem, s->stream>>>(sd, cd, d_senscr, (long long)rows_total, d_row0, d_n_rows, n_frames, d_best,  \
                                                 s->c->n_tmat, buf_bytes, 0, 0, -1, nullptr);                                   \
     } while (0)
-    if (cd.n_emit == 3) {
-        if (shape == 1) PSB_SWEEP(3, 2, 256);
-        else if (shape == 3) PSB_SWEEP(3, 2, 512);
-        else PSB_SWEEP(3, 4, 256);
-    }
-    else
-        PSB_SWEEP(5, 4, 256);
+    // one CTA shape, 256 threads x 4 instances (the beam sweep's; the shapes timed against it are in DESIGN 4.14)
+    if (cd.n_emit == 3) PSB_SWEEP(3, 4, 256);
+    else PSB_SWEEP(5, 4, 256);
 #undef PSB_SWEEP
     PSB_LAUNCH_CHECK();
     PSB_CUDA(cudaEventRecord(s->ev[1], s->stream));

@@ -81,6 +81,63 @@ __device__ __forceinline__ int hmm_step_3st(HmmReg &h, const uint8_t *tp, const 
 #undef TP
 }
 
+// hmm_step_3st for a kernel that runs the same instance over many frames (the fused sweep,
+// psb_hmm.cu): the transition bytes are decoded once per instance into ready-to-add ints, the
+// two "is this arc allowed" tests (TP(1,3), TP(0,2) against TMAT_WORST) into all-ones / zero
+// masks, and every tie-ordered pick is a compare + select with no branch.  The other kernels
+// see each instance once per launch and keep hmm_step_3st, which reads the bytes in place.
+// Same bits as hmm_step_3st, the floor and the stale-t2 quirk included: an absent arc yields
+// INT_MIN by masking, never by arithmetic on a sentinel.
+struct HmmTp3 {
+    int p00, p01, p11, p12, p22, p23, p02, p13;   // -tp[i][j]
+    int m02, m13;                                 // -1: the arc exists (tp byte != 255), 0: it does not
+};
+
+__device__ __forceinline__ HmmTp3 hmm_tp3_decode(const uint8_t *tp)
+{
+    HmmTp3 k;
+    k.p00 = -(int)tp[0]; k.p01 = -(int)tp[1]; k.p02 = -(int)tp[2];
+    k.p11 = -(int)tp[5]; k.p12 = -(int)tp[6]; k.p13 = -(int)tp[7];
+    k.p22 = -(int)tp[10]; k.p23 = -(int)tp[11];
+    // opaque to the compiler, so that the masks stay in registers instead of being re-derived from the bytes every frame
+    asm("mov.b32 %0, %1;" : "=r"(k.m02) : "r"(k.p02 > PSB_TMAT_WORST ? -1 : 0));
+    asm("mov.b32 %0, %1;" : "=r"(k.m13) : "r"(k.p13 > PSB_TMAT_WORST ? -1 : 0));
+    return k;
+}
+
+// (m ? a : b) for an all-ones / zero mask m: one LOP3
+__device__ __forceinline__ int hmm_msel(int m, int a, int b) { return (a & m) | (b & ~m); }
+
+// x_i = senscore of state i's senone (not negated); returns the instance's best score
+__device__ __forceinline__ int hmm_step_3st_dec(int (&sc)[3], int (&hi)[3], int &osc, int &ohi, const HmmTp3 &k,
+                                                int x0, int x1, int x2)
+{
+    const int s2 = sc[2] - x2, s1 = sc[1] - x1, s0 = sc[0] - x0;
+    // exit state, only when s1 > WORST (hmm.c:545-556)
+    const bool a = s1 > PSB_WORST_SCORE;
+    const int e1 = s2 + k.p23;
+    const int e2 = hmm_msel(k.m13, s1 + k.p13, INT_MIN);
+    const int s3 = max(max(e1, e2), PSB_WORST_SCORE);
+    const int oh = e1 > e2 ? hi[2] : hi[1];
+    osc = a ? s3 : osc;
+    ohi = a ? oh : ohi;
+    // state 2: t2 keeps its exit-state value (or INT_MIN) when TP(0,2) is absent
+    const int u2 = hmm_msel(k.m02, s0 + k.p02, a ? e2 : INT_MIN);
+    const int u0 = s2 + k.p22, u1 = s1 + k.p12;
+    const int m01 = max(u0, u1);
+    const int n2 = max(max(m01, u2), PSB_WORST_SCORE);
+    const int h2 = u2 > m01 ? hi[0] : (u0 > u1 ? hi[2] : hi[1]);      // hmm_pick3's tie order
+    // state 1
+    const int v0 = s1 + k.p11, v1 = s0 + k.p01;
+    const int n1 = max(max(v0, v1), PSB_WORST_SCORE);
+    const int h1 = v0 > v1 ? hi[1] : hi[0];
+    // state 0
+    const int n0 = max(s0 + k.p00, PSB_WORST_SCORE);
+    sc[0] = n0; sc[1] = n1; sc[2] = n2;
+    hi[1] = h1; hi[2] = h2;
+    return max(max(a ? s3 : PSB_WORST_SCORE, n2), max(n1, n0));
+}
+
 // hmm_vit_eval_5st_lr (hmm.c:223-353)
 __device__ __forceinline__ int hmm_step_5st(HmmReg &h, const uint8_t *tp, const int (&obs)[PSB_HMM_MAX_NSTATE])
 {
