@@ -594,6 +594,57 @@ int psb_decode_batch_pcm_host(psb_batch_t *b, psb_fe_t *fe, psb_phoneloop_t *p, 
                               const int64_t *samp_off, int32_t n_utt, int32_t *frame_off,
                               int32_t *best, int32_t *pen, int16_t *senscr);
 
+/* ------------------------------------------------------------------------------------ */
+/* Voice activity detection and endpointing for whole batches of int16 streams (ps_vad.c,
+ * ps_endpointer.c, common_audio/vad/).  For each stream: the decision of ps_vad_classify on every
+ * full frame of a fresh ps_vad_init(mode, sample_rate, frame_length), and the segments a fresh
+ * ps_endpointer_init(window, ratio, mode, sample_rate, frame_length) produces when
+ * ps_endpointer_process is called on every full frame and ps_endpointer_end_stream once with the
+ * remaining samples (0 <= r < frame size) -- also when r is 0, which the reference's Python
+ * Segmenter skips.  Timestamp callbacks and state carried across calls are not implemented: every
+ * call takes whole streams.
+ * Refused like ps_vad_set_input_params (ps_vad.c:91-127) and ps_endpointer_init
+ * (ps_endpointer.c:63-116): a rate with no supported rate within 50 % (8/16/32/48 kHz), frames other
+ * than 10/20/30 ms at that rate, mode outside 0..3, ratios whose start_frames or end_frames fall
+ * outside (0, maxlen).  Also refused, though the reference accepts them: rates whose closest supported
+ * rate is 48 kHz (44.1 and 48 kHz input), whose 48->8 kHz resampler is not implemented; and windows of
+ * more than 57 727 frames (maxlen; the endpointer's queue of decisions is kept in shared memory, four
+ * streams per CTA: about 577 s at 10 ms frames).  Zero for sample_rate / frame_length /
+ * window / ratio is the reference's default (16000, 0.03, 0.3, 0.9). */
+typedef struct psb_vad_opts_s {
+    int32_t mode;                 /* 0..3, ps_vad_mode_t */
+    int32_t sample_rate;          /* Hz */
+    double frame_length;          /* seconds */
+    double window, ratio;         /* endpointer */
+    int32_t warmup;               /* frames each parallel chunk of the filter bank runs ahead of its
+                                     first frame: 0 = the frames of 0.5 s, -1 = none (every chunk
+                                     boundary is then repaired); the result never depends on it */
+} psb_vad_opts_t;
+typedef struct psb_vad_s psb_vad_t;
+int psb_vad_create(const psb_vad_opts_t *o, int device, psb_vad_t **out);
+void psb_vad_free(psb_vad_t *v);
+int32_t psb_vad_frame_size(const psb_vad_t *v);       /* samples per frame (ps_vad_frame_size) */
+double psb_vad_frame_length(const psb_vad_t *v);      /* frame_size / sample_rate (vad.h:178) */
+int32_t psb_vad_sample_rate(const psb_vad_t *v);
+int32_t psb_vad_start_frames(const psb_vad_t *v);     /* ps_endpointer_t.start_frames / end_frames / maxlen */
+int32_t psb_vad_end_frames(const psb_vad_t *v);
+int32_t psb_vad_maxlen(const psb_vad_t *v);
+int32_t psb_vad_warmup(const psb_vad_t *v);           /* the warm-up in frames after the default is applied */
+int64_t psb_vad_last_repairs(const psb_vad_t *v);     /* chunk recomputations of the last call's repair passes */
+int32_t psb_vad_last_passes(const psb_vad_t *v);      /* repair passes of the last call (the last one recomputes nothing) */
+/* pcm: the streams' samples back to back, samp_off int64[n_streams + 1] (host, samp_off[0] = 0).
+ * Outputs: frame_off int32[n_streams + 1] (host): stream s has frames frame_off[s] .. frame_off[s + 1] - 1;
+ * flags int8[frames] (0 / 1); seg_n int32[n_streams]: stream s's segment count; its segments are
+ * rows frame_off[s] .. frame_off[s] + seg_n[s] - 1 of segs int64[frames][2] (first sample, one past
+ * the last, relative to the stream) and times double[frames][2] (ps_endpointer_speech_start /
+ * speech_end); a stream has at most one segment per frame.  _device: pcm, flags, seg_n, segs and
+ * times on the device, *ms (may be NULL) = device time of the kernels. */
+int psb_vad_process_host(psb_vad_t *v, const int16_t *pcm, const int64_t *samp_off, int32_t n_streams,
+                         int8_t *flags, int32_t *frame_off, int32_t *seg_n, int64_t *segs, double *times);
+int psb_vad_process_device(psb_vad_t *v, const int16_t *d_pcm, const int64_t *samp_off, int32_t n_streams,
+                           int8_t *d_flags, int32_t *frame_off, int32_t *d_seg_n, int64_t *d_segs, double *d_times,
+                           float *ms);
+
 /* number of kernels launched by this library in the calling process so far */
 int64_t psb_kernel_launch_count(void);
 

@@ -54,6 +54,11 @@ class FsgDesc(C.Structure):
                 ("pbeam", C.c_int32), ("wbeam", C.c_int32), ("maxhmmpf", C.c_int32)]
 
 
+class VadOpts(C.Structure):
+    _fields_ = [("mode", C.c_int32), ("sample_rate", C.c_int32), ("frame_length", C.c_double), ("window", C.c_double),
+                ("ratio", C.c_double), ("warmup", C.c_int32)]
+
+
 class NgramDesc(C.Structure):
     _fields_ = [("info", C.c_void_p), ("model", C.c_void_p), ("model_len", C.c_int64), ("ci_tmat", C.c_void_p),
                 ("ci_ssid", C.c_void_p), ("lm_arrays", C.c_void_p), ("lm_arrays_len", C.c_int64)]
@@ -139,6 +144,19 @@ SYMBOLS = [
     ("psb_sendump_write", C.c_int, [C.c_char_p, C.c_char_p, _I32, C.c_double, _VP, _I64]),
     ("psb_sendump_read", _I64, [C.c_char_p, _VP, _VP, _I64]),
     ("psb_batch_set_pipeline", C.c_int, [_VP, C.c_int]),
+    ("psb_vad_create", C.c_int, [C.POINTER(VadOpts), C.c_int, C.POINTER(_VP)]),
+    ("psb_vad_free", None, [_VP]),
+    ("psb_vad_frame_size", _I32, [_VP]),
+    ("psb_vad_frame_length", C.c_double, [_VP]),
+    ("psb_vad_sample_rate", _I32, [_VP]),
+    ("psb_vad_start_frames", _I32, [_VP]),
+    ("psb_vad_end_frames", _I32, [_VP]),
+    ("psb_vad_maxlen", _I32, [_VP]),
+    ("psb_vad_warmup", _I32, [_VP]),
+    ("psb_vad_last_repairs", _I64, [_VP]),
+    ("psb_vad_last_passes", _I32, [_VP]),
+    ("psb_vad_process_host", C.c_int, [_VP, _VP, _VP, _I32, _VP, _VP, _VP, _VP, _VP]),
+    ("psb_vad_process_device", C.c_int, [_VP, _VP, _VP, _I32, _VP, _VP, _VP, _VP, _VP, C.POINTER(C.c_float)]),
     ("psb_kernel_launch_count", _I64, []),
 ]
 

@@ -760,3 +760,80 @@ class FrontEnd:
         if self.h:
             lib().psb_fe_free(self.h)
             self.h = None
+
+
+class Endpointer:
+    """ps_endpointer_t for whole batches of int16 streams on the device (arguments as the reference's Python
+    Endpointer: window, ratio, vad_mode, sample_rate, frame_length; 0 / None = the reference's default).  Every
+    stream is one whole recording: ps_endpointer_process on each full frame, then ps_endpointer_end_stream with the
+    rest -- also when the rest is empty, which the reference's Python Segmenter skips.  warmup: None (default), 0 (no
+    warm-up: every chunk boundary of the parallel filter bank is repaired) or a frame count; results never depend on
+    it.  Rates that map to 48 kHz (44.1 / 48 kHz input) are refused."""
+
+    def __init__(self, window=0.3, ratio=0.9, vad_mode=0, sample_rate=16000, frame_length=0.03, device=0, warmup=None):
+        from ._lib import VadOpts
+        o = VadOpts()
+        o.mode, o.sample_rate, o.frame_length = int(vad_mode), int(sample_rate or 0), float(frame_length or 0.0)
+        o.window, o.ratio = float(window or 0.0), float(ratio or 0.0)
+        o.warmup = 0 if warmup is None else (-1 if int(warmup) == 0 else int(warmup))
+        h = C.c_void_p()
+        check(lib().psb_vad_create(C.byref(o), device, C.byref(h)), "psb_vad_create")
+        self.h = h
+        L = lib()
+        self.frame_size, self.frame_length, self.sample_rate = L.psb_vad_frame_size(h), L.psb_vad_frame_length(h), L.psb_vad_sample_rate(h)
+        self.start_frames, self.end_frames, self.maxlen = L.psb_vad_start_frames(h), L.psb_vad_end_frames(h), L.psb_vad_maxlen(h)
+        self.warmup = L.psb_vad_warmup(h)
+
+    def process(self, streams):
+        """(flags int8 [frames], frame_off int32 [n + 1], seg_n int32 [n], segs int64 [frames][2], times float64 [frames][2])."""
+        streams = [np.ascontiguousarray(s, np.int16) for s in streams]
+        n = len(streams)
+        samp_off = np.zeros(n + 1, np.int64)
+        samp_off[1:] = np.cumsum([len(s) for s in streams])
+        pcm = np.concatenate(streams) if n else np.zeros(0, np.int16)
+        total = int(sum(len(s) // self.frame_size for s in streams))
+        flags = np.zeros(max(total, 1), np.int8)
+        frame_off = np.zeros(n + 1, np.int32)
+        seg_n = np.zeros(max(n, 1), np.int32)
+        segs = np.zeros((max(total, 1), 2), np.int64)
+        times = np.zeros((max(total, 1), 2), np.float64)
+        check(lib().psb_vad_process_host(self.h, _p(pcm) if pcm.size else None, _p(samp_off), n, _p(flags), _p(frame_off),
+                                         _p(seg_n), _p(segs), _p(times)), "psb_vad_process_host")
+        return flags[:total], frame_off, seg_n[:n], segs, times
+
+    def classify_batch(self, streams):
+        """Per stream, int8 [full frames]: ps_vad_classify of each frame on a fresh VAD."""
+        flags, frame_off = self.process(streams)[:2]
+        return [flags[frame_off[i]:frame_off[i + 1]] for i in range(len(frame_off) - 1)]
+
+    def segment_batch(self, streams):
+        """Per stream, [(start_time, end_time, start_sample, end_sample)] with the reference's float64 times."""
+        _, frame_off, seg_n, segs, times = self.process(streams)
+        out = []
+        for i in range(len(frame_off) - 1):
+            r = range(int(frame_off[i]), int(frame_off[i]) + int(seg_n[i]))
+            out.append([(float(times[j, 0]), float(times[j, 1]), int(segs[j, 0]), int(segs[j, 1])) for j in r])
+        return out
+
+    @property
+    def last_repairs(self):
+        """Chunk recomputations of the last call: chunks whose start state differed from their predecessor's end."""
+        return int(lib().psb_vad_last_repairs(self.h))
+
+    @property
+    def last_passes(self):
+        """Repair passes of the last call; the last pass recomputes nothing."""
+        return int(lib().psb_vad_last_passes(self.h))
+
+    def close(self):
+        if self.h:
+            lib().psb_vad_free(self.h)
+            self.h = None
+
+
+class Vad(Endpointer):
+    """ps_vad_t for whole batches (arguments as the reference's Python Vad: mode, sample_rate, frame_length):
+    classify_batch(streams) gives ps_vad_classify's decision for every full frame of each stream."""
+
+    def __init__(self, mode=0, sample_rate=16000, frame_length=0.03, device=0, warmup=None):
+        super().__init__(0.3, 0.9, mode, sample_rate, frame_length, device, warmup)

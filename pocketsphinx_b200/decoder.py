@@ -76,6 +76,8 @@ class Decoder:
                                        float(pl["pl_weight"]))
         self.second_pass = search_cfg.get("fwdflat", "yes") in ("yes", "1", "true", "True")
         self.bp_cap = int(cfg.get("latsize", 5000))
+        self.sample_rate = int(float(fp["samprate"]))
+        self.max_utts = max_utts
 
     def decode_raw_batch(self, utterances, sessions=None):
         """utterances: int16 arrays, each a whole utterance.  sessions: None (every utterance a fresh decoder) or one
@@ -95,6 +97,38 @@ class Decoder:
         out = [None] * len(utterances)
         for j, i in enumerate(order):
             out[i] = res[j]
+        return out
+
+    def decode_stream_batch(self, streams, vad_mode=0, vad_window=0.3, vad_ratio=0.9, vad_frame_length=0.03):
+        """Whole recordings in, words out: every stream is cut into speech segments by the device endpointer (at the
+        model's sample rate; api.Endpointer), and all segments of all streams are decoded in one decode_raw_batch call
+        with one session per stream, so a stream's segments are one decoder's utterances in order (live CMN and dither
+        carry over, as for a reference decoder fed the segments one after another).  Returns, per stream, a list of
+        dicts: start_time, end_time (the endpointer's float64 seconds), start_sample, end_sample, and decode_raw_batch's
+        hyp, score, seg, words, n_frames.  The segments count against max_utts / max_frames of this Decoder."""
+        ep = api.Endpointer(vad_window, vad_ratio, vad_mode, self.sample_rate, vad_frame_length, self.device)
+        try:
+            segs = ep.segment_batch(streams)
+        finally:
+            ep.close()
+        utts, sessions = [], []
+        for i, (pcm, ss) in enumerate(zip(streams, segs)):
+            for _, _, a, b in ss:
+                utts.append(np.asarray(pcm)[a:b])
+                sessions.append(i)
+        if len(utts) > self.max_utts:
+            raise ValueError("%d speech segments, more than this Decoder's max_utts (%d): create it with a larger max_utts"
+                             % (len(utts), self.max_utts))
+        res = self.decode_raw_batch(utts, sessions) if utts else []
+        out, k = [], 0
+        for ss in segs:
+            row = []
+            for t0, t1, a, b in ss:
+                d = dict(res[k])
+                d.update(start_time=t0, end_time=t1, start_sample=a, end_sample=b)
+                row.append(d)
+                k += 1
+            out.append(row)
         return out
 
     def _decode(self, utterances, sess_off):
