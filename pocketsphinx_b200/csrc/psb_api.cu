@@ -419,9 +419,8 @@ static int score_dispatch(psb_batch_t *b, const float *d_feats, const int32_t *u
 static int check_offsets(const psb_batch_t *b, const int32_t *utt_off, int32_t n_utt)
 {
     PSB_REQUIRE(utt_off && n_utt >= 0, "bad utt_off / n_utt");
-    PSB_REQUIRE(utt_off[0] == 0, "utt_off[0] must be 0");
-    for (int u = 0; u < n_utt; ++u)
-        PSB_REQUIRE(utt_off[u + 1] >= utt_off[u], "utt_off must be non-decreasing");
+    const int rc = psb_check_utt_off("psb_batch", utt_off, n_utt);
+    if (rc) return rc;
     PSB_REQUIRE(n_utt <= b->max_utts && utt_off[n_utt] <= b->max_frames, "batch exceeds psb_batch_create limits");
     return PSB_OK;
 }

@@ -124,6 +124,7 @@ phoneloop_kernel(const int16_t *__restrict__ senscr, const int32_t *__restrict__
     int *pen_buf = frame + H;              // [window][H]
     int *sval = pen_buf + P.window * H;    // [32]
     int *sidx = sval + 32;                 // [32]
+    const HmmSoA<> V{score, hist, out_score, out_hist, bestsc, H};
 
     const int u = blockIdx.x;
     const long long f0 = utt_off[u];
@@ -131,8 +132,7 @@ phoneloop_kernel(const int16_t *__restrict__ senscr, const int32_t *__restrict__
 
     // phone_loop_search_start (:155-175): hmm_clear + hmm_enter(0, -1, 0)
     for (int i = tid; i < H; i += blockDim.x) {
-        for (int s = 0; s < N; ++s) { score[s * H + i] = PSB_WORST_SCORE; hist[s * H + i] = -1; }
-        out_score[i] = PSB_WORST_SCORE; out_hist[i] = -1; bestsc[i] = PSB_WORST_SCORE;
+        V.clear(i, N);
         score[i] = 0; hist[i] = -1; frame[i] = 0;
         for (int w = 0; w < P.window; ++w) pen_buf[w * H + i] = 0;
     }
@@ -147,13 +147,7 @@ phoneloop_kernel(const int16_t *__restrict__ senscr, const int32_t *__restrict__
         // evaluate_hmms (:193-214)
         for (int i = tid; i < H; i += blockDim.x) {
             HmmReg h;
-#pragma unroll
-            for (int s = 0; s < PSB_HMM_MAX_NSTATE; ++s) {
-                h.score[s] = s < N ? score[s * H + i] : PSB_WORST_SCORE;
-                h.hist[s] = s < N ? hist[s * H + i] : -1;
-                h.senid[s] = s < N ? senid_g[s * H + i] : PSB_BAD_SSID;
-            }
-            h.out_score = out_score[i]; h.out_hist = out_hist[i]; h.best = bestsc[i];
+            V.load(h, i, N, senid_g + i, H);
             if (renorm) {                                    // hmm_normalize (hmm.c:206-216)
 #pragma unroll
                 for (int s = 0; s < PSB_HMM_MAX_NSTATE; ++s)
@@ -164,10 +158,7 @@ phoneloop_kernel(const int16_t *__restrict__ senscr, const int32_t *__restrict__
                 int b = hmm_step(h, c, tmatid_g[i], false, row);
                 if (b > bs) bs = b;
             }
-#pragma unroll
-            for (int s = 0; s < PSB_HMM_MAX_NSTATE; ++s)
-                if (s < N) { score[s * H + i] = h.score[s]; hist[s * H + i] = h.hist[s]; }
-            out_score[i] = h.out_score; out_hist[i] = h.out_hist; bestsc[i] = h.best;
+            V.store(h, i, N);
         }
         int dummy;
         bs = block_reduce_max_pair<int>(bs, 0, sidx, sval, dummy);
@@ -260,11 +251,13 @@ extern "C" int psb_hmmctx_create(int32_t n_emit_state, const uint8_t *tp, int32_
     memset(c, 0, sizeof(*c));
     c->device = device; c->n_emit = n_emit_state; c->n_tmat = n_tmat; c->n_sseq = n_sseq; c->n_sen = n_sen;
     size_t tpb = (size_t)n_tmat * n_emit_state * (n_emit_state + 1);
+    const size_t sseq_bytes = std::max<size_t>(2, (size_t)n_sseq * n_emit_state * 2);
     cudaError_t e = cudaMalloc(&c->d_tp, tpb);
     if (e == cudaSuccess) e = cudaMemcpy(c->d_tp, tp, tpb, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMalloc(&c->d_sseq, std::max<size_t>(2, (size_t)n_sseq * n_emit_state * 2));
-    if (e == cudaSuccess && n_sseq > 0 && sseq)
-        e = cudaMemcpy(c->d_sseq, sseq, (size_t)n_sseq * n_emit_state * 2, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMalloc(&c->d_sseq, sseq_bytes);
+    if (e == cudaSuccess && !(c->h_sseq = (uint16_t *)calloc(sseq_bytes, 1))) e = cudaErrorMemoryAllocation;
+    if (e == cudaSuccess && n_sseq > 0 && sseq) memcpy(c->h_sseq, sseq, (size_t)n_sseq * n_emit_state * 2);
+    if (e == cudaSuccess) e = cudaMemcpy(c->d_sseq, c->h_sseq, sseq_bytes, cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking);
     if (e == cudaSuccess) e = cudaMalloc(&c->d_senscr, (size_t)n_sen * 2);
     if (e == cudaSuccess) e = cudaMallocHost(&c->h_senscr, (size_t)n_sen * 2);
@@ -285,7 +278,7 @@ extern "C" void psb_hmmctx_free(psb_hmmctx_t *c)
     cudaSetDevice(c->device);
     if (c->stream) cudaStreamSynchronize(c->stream);
     cudaFree(c->d_tp); cudaFree(c->d_sseq); cudaFree(c->d_hmms); cudaFree(c->d_senscr); cudaFree(c->d_best);
-    cudaFree(c->d_al_i32); cudaFree(c->d_al_tok); cudaFree(c->d_al_senid); cudaFree(c->d_al_tokoff);
+    free(c->h_sseq);
     for (void *p : c->d_srch) cudaFree(p);
     if (c->al_ev[0]) cudaEventDestroy(c->al_ev[0]);
     if (c->al_ev[1]) cudaEventDestroy(c->al_ev[1]);
@@ -395,18 +388,9 @@ extern "C" int psb_phoneloop_create(psb_hmmctx_t *c, int32_t n_phones, const int
 {
     PSB_REQUIRE(c && out && n_phones > 0 && ssid && tmatid && window >= 0, "psb_phoneloop_create: bad argument");
     PSB_CUDA(cudaSetDevice(c->device));
-    std::vector<uint16_t> sseq((size_t)c->n_sseq * c->n_emit);
-    PSB_CUDA(cudaMemcpy(sseq.data(), c->d_sseq, sseq.size() * 2, cudaMemcpyDeviceToHost));
-    std::vector<uint16_t> senid((size_t)c->n_emit * n_phones);
-    for (int i = 0; i < n_phones; ++i) {
-        PSB_REQUIRE(ssid[i] >= 0 && ssid[i] < c->n_sseq, "ssid[%d] out of range", i);
-        PSB_REQUIRE(tmatid[i] >= 0 && tmatid[i] < c->n_tmat, "tmatid[%d] out of range", i);
-        for (int s = 0; s < c->n_emit; ++s) {
-            uint16_t v = sseq[(size_t)ssid[i] * c->n_emit + s];         // hmm_init, non-mpx (hmm.c:99-102)
-            PSB_REQUIRE(v < c->n_sen, "senone id %d out of range", v);
-            senid[(size_t)s * n_phones + i] = v;
-        }
-    }
+    std::vector<uint16_t> senid((size_t)c->n_emit * n_phones);          // [state][phone]: coalesced reads in the kernel
+    const int rc = ctx_senids(c, "psb_phoneloop_create", n_phones, ssid, tmatid, senid.data(), 1, n_phones);
+    if (rc) return rc;
     psb_phoneloop_t *p = new psb_phoneloop_t();
     memset(p, 0, sizeof(*p));
     p->c = c; p->n_phones = n_phones; p->window = window; p->beam = beam; p->pbeam = pbeam; p->pip = pip;
@@ -464,6 +448,8 @@ extern "C" int psb_phoneloop_run_device(psb_phoneloop_t *p, const int16_t *d_sen
 {
     PSB_REQUIRE(p && d_senscr && utt_off && n_utt >= 0, "psb_phoneloop_run_device: bad argument");
     if (n_utt == 0) return PSB_OK;
+    int rc = ctx_check_utts("psb_phoneloop_run_device", utt_off, n_utt, d_senscr);
+    if (rc) return rc;
     PSB_CUDA(cudaSetDevice(p->c->device));
     cudaStream_t st = batch ? psb_batch_stream((psb_batch_t *)batch) : p->stream;
     int32_t *d_off = nullptr;
@@ -471,7 +457,7 @@ extern "C" int psb_phoneloop_run_device(psb_phoneloop_t *p, const int16_t *d_sen
     PSB_CUDA(cudaMalloc(&d_off, (size_t)(n_utt + 1) * 4));
     PSB_CUDA(cudaMemcpyAsync(d_off, utt_off, (size_t)(n_utt + 1) * 4, cudaMemcpyHostToDevice, st));
     if (final_hmms) PSB_CUDA(cudaMalloc(&d_final, (size_t)n_utt * p->n_phones * sizeof(psb_hmm_t)));
-    int rc = psb_phoneloop_launch(p, d_senscr, d_off, n_utt, d_best, d_pen, d_final, nullptr, st);
+    rc = psb_phoneloop_launch(p, d_senscr, d_off, n_utt, d_best, d_pen, d_final, nullptr, st);
     if (!rc && final_hmms) {
         cudaError_t e = cudaMemcpyAsync(final_hmms, d_final, (size_t)n_utt * p->n_phones * sizeof(psb_hmm_t),
                                         cudaMemcpyDeviceToHost, st);
@@ -488,10 +474,11 @@ extern "C" int psb_phoneloop_run_host(psb_phoneloop_t *p, const int16_t *senscr,
 {
     PSB_REQUIRE(p && senscr && utt_off && n_utt >= 0, "psb_phoneloop_run_host: bad argument");
     if (n_utt == 0) return PSB_OK;
+    int rc = ctx_check_utts("psb_phoneloop_run_host", utt_off, n_utt, senscr);
+    if (rc) return rc;
     PSB_CUDA(cudaSetDevice(p->c->device));
     const size_t total = utt_off[n_utt], H = p->n_phones;
     int16_t *d_scr = nullptr; int32_t *d_off = nullptr, *d_best = nullptr, *d_pen = nullptr; psb_hmm_t *d_tr = nullptr;
-    int rc = PSB_OK;
     cudaError_t e = cudaMalloc(&d_scr, std::max<size_t>(2, total * p->c->n_sen * 2));
     if (e == cudaSuccess) e = cudaMemcpy(d_scr, senscr, total * p->c->n_sen * 2, cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaMalloc(&d_off, (size_t)(n_utt + 1) * 4);
@@ -1462,6 +1449,7 @@ align_kernel(const int16_t *__restrict__ senscr, const int32_t *__restrict__ utt
     int *frame = out_hist + H;             // [H]
     int *sval = frame + H;                 // [32]
     int *sidx = sval + 32;                 // [32]
+    const HmmSoA<false> V{score, hist, out_score, out_hist, nullptr, H};
     int32_t *tid_u = tok_id + tok_off[u], *tsc_u = tok_sc + tok_off[u];
     int32_t *ss = st_start + (size_t)p0 * N, *sd = st_dur + (size_t)p0 * N, *sc = st_score + (size_t)p0 * N;
 
@@ -1469,8 +1457,8 @@ align_kernel(const int16_t *__restrict__ senscr, const int32_t *__restrict__ utt
     if (H == 0) { if (tid == 0) status[u] = -1; return; }
     // hmm_init -> hmm_clear (hmm.c:85-105, 180-196), then state_align_search_start: hmm_enter(hmms, 0, 0, 0)
     for (int i = tid; i < H; i += blockDim.x) {
-        for (int s = 0; s < N; ++s) { score[s * H + i] = PSB_WORST_SCORE; hist[s * H + i] = -1; }
-        out_score[i] = PSB_WORST_SCORE; out_hist[i] = -1; frame[i] = -1;
+        V.clear(i, N);
+        frame[i] = -1;
     }
     __syncthreads();
     if (tid == 0) { score[0] = 0; hist[0] = 0; frame[0] = 0; }
@@ -1484,13 +1472,7 @@ align_kernel(const int16_t *__restrict__ senscr, const int32_t *__restrict__ utt
         int bs = PSB_WORST_SCORE;
         for (int i = tid; i < H; i += blockDim.x) {
             HmmReg h;
-#pragma unroll
-            for (int s = 0; s < PSB_HMM_MAX_NSTATE; ++s) {
-                h.score[s] = s < N ? score[s * H + i] : PSB_WORST_SCORE;
-                h.hist[s] = s < N ? hist[s * H + i] : -1;
-                h.senid[s] = s < N ? senid_g[(size_t)(p0 + i) * N + s] : PSB_BAD_SSID;
-            }
-            h.out_score = out_score[i]; h.out_hist = out_hist[i]; h.best = PSB_WORST_SCORE;
+            V.load(h, i, N, senid_g + (size_t)(p0 + i) * N, 1);
             if (renorm) {                                    // hmm_normalize, every phone
 #pragma unroll
                 for (int s = 0; s < PSB_HMM_MAX_NSTATE; ++s)
@@ -1501,10 +1483,7 @@ align_kernel(const int16_t *__restrict__ senscr, const int32_t *__restrict__ utt
                 const int b = hmm_step(h, c, tmatid_g[p0 + i], false, row);
                 if (b > bs) bs = b;
             }
-#pragma unroll
-            for (int s = 0; s < PSB_HMM_MAX_NSTATE; ++s)
-                if (s < N) { score[s * H + i] = h.score[s]; hist[s * H + i] = h.hist[s]; }
-            out_score[i] = h.out_score; out_hist[i] = h.out_hist;
+            V.store(h, i, N);
             // prune_hmms: stays active unless the alignment constraint ends it
             if (frame[i] >= t && !(nf > (ef_g ? ef_g[p0 + i] : INT_MAX))) frame[i] = nf;
         }
@@ -1588,36 +1567,28 @@ extern "C" int psb_align_batch_device(psb_hmmctx_t *c, const int16_t *d_senscr, 
     PSB_REQUIRE(c && utt_off && ph_off && n_utt >= 0 && st_start && st_dur && st_score && status,
                 "psb_align_batch_device: bad argument");
     if (n_utt == 0) return PSB_OK;
-    PSB_REQUIRE(utt_off[0] == 0 && ph_off[0] == 0, "psb_align_batch_device: offsets must start at 0");
+    int rc = ctx_check_utts("psb_align_batch_device", utt_off, n_utt, d_senscr);
+    if (rc) return rc;
+    PSB_REQUIRE(ph_off[0] == 0, "psb_align_batch_device: offsets must start at 0");
     const int N = c->n_emit;
     const int total_ph = ph_off[n_utt];
     PSB_REQUIRE(total_ph == 0 || (ssid && tmatid), "psb_align_batch_device: phones missing");
-    PSB_REQUIRE(d_senscr || utt_off[n_utt] == 0, "psb_align_batch_device: scores missing");
     PSB_CUDA(cudaSetDevice(c->device));
-    std::vector<uint16_t> sseq((size_t)c->n_sseq * N);
-    PSB_CUDA(cudaMemcpy(sseq.data(), c->d_sseq, sseq.size() * 2, cudaMemcpyDeviceToHost));
     std::vector<uint16_t> senid((size_t)std::max(total_ph, 1) * N);
     std::vector<int64_t> tok_off((size_t)n_utt + 1);
     int max_h = 0;
     tok_off[0] = 0;
     for (int u = 0; u < n_utt; ++u) {
         const int H = ph_off[u + 1] - ph_off[u], T = utt_off[u + 1] - utt_off[u];
-        PSB_REQUIRE(H >= 0 && T >= 0, "psb_align_batch_device: offsets not monotone at %d", u);
+        PSB_REQUIRE(H >= 0, "psb_align_batch_device: ph_off not monotone at %d", u);
         max_h = std::max(max_h, H);
         tok_off[(size_t)u + 1] = tok_off[(size_t)u] + (int64_t)T * H * N;
     }
-    for (int i = 0; i < total_ph; ++i) {
-        PSB_REQUIRE(ssid[i] >= 0 && ssid[i] < c->n_sseq, "ssid[%d] out of range", i);
-        PSB_REQUIRE(tmatid[i] >= 0 && tmatid[i] < c->n_tmat, "tmatid[%d] out of range", i);
-        for (int s = 0; s < N; ++s) {
-            const uint16_t v = sseq[(size_t)ssid[i] * N + s];           // hmm_init, non-mpx (hmm.c:99-102)
-            PSB_REQUIRE(v < c->n_sen, "senone id %d out of range", v);
-            senid[(size_t)i * N + s] = v;
-        }
-    }
+    rc = ctx_senids(c, "psb_align_batch_device", total_ph, ssid, tmatid, senid.data(), N, 1);
+    if (rc) return rc;
     const size_t smem = ((size_t)(2 * N + 3) * max_h + 64) * sizeof(int);
     PSB_REQUIRE(smem <= 200 * 1024, "psb_align_batch_device: %d phones in one utterance do not fit shared memory", max_h);
-    // grow-only workspace in the context: one int32 block
+    // workspace: one int32 block
     //   utt_off | ph_off | tmatid | sf | ef | start | dur | score | status
     // plus the token table (2 x frames x states), the senone ids and the token offsets
     const size_t n_state = (size_t)total_ph * N;
@@ -1625,47 +1596,37 @@ extern "C" int psb_align_batch_device(psb_hmmctx_t *c, const int16_t *d_senscr, 
                  o_ss = o_ef + total_ph, o_sd = o_ss + n_state, o_sc = o_sd + n_state, o_st = o_sc + n_state,
                  n_i32 = o_st + n_utt;
     const size_t n_tok = (size_t)tok_off[(size_t)n_utt] * 2;
-    auto grow = [](void **p, size_t *cap, size_t need, size_t elem) -> cudaError_t {
-        if (need <= *cap) return cudaSuccess;
-        if (*p) cudaFree(*p);
-        *p = nullptr; *cap = 0;
-        const size_t want = need + need / 8 + 256;
-        cudaError_t e = cudaMalloc(p, want * elem);
-        if (e == cudaSuccess) *cap = want;
-        return e;
-    };
-    cudaError_t e = grow((void **)&c->d_al_i32, &c->al_i32_cap, n_i32, 4);
-    if (e == cudaSuccess) e = grow((void **)&c->d_al_tok, &c->al_tok_cap, std::max<size_t>(n_tok, 1), 4);
-    if (e == cudaSuccess) e = grow((void **)&c->d_al_senid, &c->al_senid_cap, senid.size(), 2);
-    if (e == cudaSuccess) e = grow((void **)&c->d_al_tokoff, &c->al_tokoff_cap, tok_off.size(), 8);
+    int32_t *d_i32 = nullptr, *d_tok = nullptr;
+    uint16_t *d_senid = nullptr;
+    int64_t *d_tokoff = nullptr;
+    cudaError_t e = srch_reserve(c, 0, n_i32, &d_i32);
+    if (e == cudaSuccess) e = srch_reserve(c, 1, n_tok, &d_tok);
+    if (e == cudaSuccess) e = srch_reserve(c, 2, senid.size(), &d_senid);
+    if (e == cudaSuccess) e = srch_reserve(c, 3, tok_off.size(), &d_tokoff);
     if (e == cudaSuccess && !c->al_ev[0]) e = cudaEventCreate(&c->al_ev[0]);
     if (e == cudaSuccess && !c->al_ev[1]) e = cudaEventCreate(&c->al_ev[1]);
-    int32_t *d_i32 = c->d_al_i32, *d_tok = c->d_al_tok;
     cudaStream_t st = c->stream;
     if (e == cudaSuccess) e = cudaMemcpyAsync(d_i32 + o_utt, utt_off, ((size_t)n_utt + 1) * 4, cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess) e = cudaMemcpyAsync(d_i32 + o_ph, ph_off, ((size_t)n_utt + 1) * 4, cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess && total_ph) e = cudaMemcpyAsync(d_i32 + o_tm, tmatid, (size_t)total_ph * 4, cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess && total_ph && sf) e = cudaMemcpyAsync(d_i32 + o_sf, sf, (size_t)total_ph * 4, cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess && total_ph && ef) e = cudaMemcpyAsync(d_i32 + o_ef, ef, (size_t)total_ph * 4, cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(c->d_al_senid, senid.data(), senid.size() * 2, cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(c->d_al_tokoff, tok_off.data(), tok_off.size() * 8, cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_senid, senid.data(), senid.size() * 2, cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_tokoff, tok_off.data(), tok_off.size() * 8, cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(align_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e == cudaSuccess) e = cudaEventRecord(c->al_ev[0], st);
     if (e == cudaSuccess) {
-        align_kernel<<<(unsigned)n_utt, 128, smem, st>>>(d_senscr, d_i32 + o_utt, dev_ctx(c), d_i32 + o_ph, c->d_al_senid, d_i32 + o_tm,
+        align_kernel<<<(unsigned)n_utt, 128, smem, st>>>(d_senscr, d_i32 + o_utt, dev_ctx(c), d_i32 + o_ph, d_senid, d_i32 + o_tm,
                                                         sf ? d_i32 + o_sf : nullptr, ef ? d_i32 + o_ef : nullptr, d_tok,
-                                                        d_tok + tok_off[(size_t)n_utt], c->d_al_tokoff, d_i32 + o_ss, d_i32 + o_sd,
+                                                        d_tok + tok_off[(size_t)n_utt], d_tokoff, d_i32 + o_ss, d_i32 + o_sd,
                                                         d_i32 + o_sc, d_i32 + o_st);
-        g_psb_launches.fetch_add(1, std::memory_order_relaxed);
-        e = cudaGetLastError();
+        e = cudaEventRecord(c->al_ev[1], st);
     }
-    if (e == cudaSuccess) e = cudaEventRecord(c->al_ev[1], st);
-    if (e == cudaSuccess && n_state) e = cudaMemcpyAsync(st_start, d_i32 + o_ss, n_state * 4, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess && n_state) e = cudaMemcpyAsync(st_dur, d_i32 + o_sd, n_state * 4, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess && n_state) e = cudaMemcpyAsync(st_score, d_i32 + o_sc, n_state * 4, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(status, d_i32 + o_st, (size_t)n_utt * 4, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e == cudaSuccess) e = cudaEventElapsedTime(&c->last_align_ms, c->al_ev[0], c->al_ev[1]);
+    rc = ctx_finish(c, "psb_align_batch_device", e, 1,
+                    {{st_start, d_i32 + o_ss, n_state * 4}, {st_dur, d_i32 + o_sd, n_state * 4},
+                     {st_score, d_i32 + o_sc, n_state * 4}, {status, d_i32 + o_st, (size_t)n_utt * 4}});
+    if (rc) return rc;
+    e = cudaEventElapsedTime(&c->last_align_ms, c->al_ev[0], c->al_ev[1]);
     if (e != cudaSuccess) {
         psb_set_error("psb_align_batch_device: %s", cudaGetErrorString(e));
         return PSB_ERR_CUDA;
@@ -1685,13 +1646,13 @@ extern "C" int psb_align_batch_host(psb_hmmctx_t *c, const int16_t *senscr, cons
 {
     PSB_REQUIRE(c && utt_off && n_utt >= 0, "psb_align_batch_host: bad argument");
     if (n_utt == 0) return PSB_OK;
+    int rc = ctx_check_utts("psb_align_batch_host", utt_off, n_utt, senscr);
+    if (rc) return rc;
     PSB_CUDA(cudaSetDevice(c->device));
     const size_t nb = (size_t)utt_off[n_utt] * c->n_sen * 2;
-    PSB_REQUIRE(nb == 0 || senscr, "psb_align_batch_host: scores missing");
     int16_t *d = nullptr;
     PSB_CUDA(cudaMalloc((void **)&d, std::max<size_t>(nb, 2)));
     cudaError_t e = nb ? cudaMemcpy(d, senscr, nb, cudaMemcpyHostToDevice) : cudaSuccess;
-    int rc = PSB_OK;
     if (e == cudaSuccess)
         rc = psb_align_batch_device(c, d, utt_off, n_utt, ph_off, ssid, tmatid, sf, ef, st_start, st_dur, st_score, status);
     cudaFree(d);
@@ -1735,13 +1696,14 @@ kws_kernel(const int16_t *__restrict__ senscr, const int32_t *__restrict__ utt_o
     int *frame = bestsc + H;               // [H]
     int *sval = frame + H;                 // [32]
     int *sidx = sval + 32;                 // [32]
+    const HmmSoA<> V{score, hist, out_score, out_hist, bestsc, H};
     int32_t *my_hits = hits + (size_t)u * cap * 5;
     int nh = 0;
 
     // kws_search_reinit: hmm_init (= hmm_clear); kws_search_start: phone loop hmm_clear + hmm_enter(0, -1, 0)
     for (int i = tid; i < H; i += blockDim.x) {
-        for (int s = 0; s < N; ++s) { score[s * H + i] = PSB_WORST_SCORE; hist[s * H + i] = -1; }
-        out_score[i] = PSB_WORST_SCORE; out_hist[i] = -1; bestsc[i] = PSB_WORST_SCORE; frame[i] = -1;
+        V.clear(i, N);
+        frame[i] = -1;
         if (i < n_pl) { score[i] = 0; hist[i] = -1; frame[i] = 0; }
     }
     __syncthreads();
@@ -1753,19 +1715,10 @@ kws_kernel(const int16_t *__restrict__ senscr, const int32_t *__restrict__ utt_o
         for (int i = tid; i < H; i += blockDim.x) {
             if (i >= n_pl && !(frame[i] > 0)) continue;
             HmmReg h;
-#pragma unroll
-            for (int s = 0; s < PSB_HMM_MAX_NSTATE; ++s) {
-                h.score[s] = s < N ? score[s * H + i] : PSB_WORST_SCORE;
-                h.hist[s] = s < N ? hist[s * H + i] : -1;
-                h.senid[s] = s < N ? senid_g[(size_t)i * N + s] : PSB_BAD_SSID;
-            }
-            h.out_score = out_score[i]; h.out_hist = out_hist[i]; h.best = bestsc[i];
+            V.load(h, i, N, senid_g + (size_t)i * N, 1);
             const int b = hmm_step(h, c, tmatid_g[i], false, row);
             if (b > bs) bs = b;
-#pragma unroll
-            for (int s = 0; s < PSB_HMM_MAX_NSTATE; ++s)
-                if (s < N) { score[s * H + i] = h.score[s]; hist[s * H + i] = h.hist[s]; }
-            out_score[i] = h.out_score; out_hist[i] = h.out_hist; bestsc[i] = h.best;
+            V.store(h, i, N);
         }
         int dummy;
         bs = block_reduce_max_pair<int>(bs, 0, sidx, sval, dummy);
@@ -1775,8 +1728,8 @@ kws_kernel(const int16_t *__restrict__ senscr, const int32_t *__restrict__ utt_o
         for (int i = tid; i < H; i += blockDim.x) {
             if (i >= n_pl) {
                 if (frame[i] > 0 && bestsc[i] < thresh) {
-                    for (int s = 0; s < N; ++s) { score[s * H + i] = PSB_WORST_SCORE; hist[s * H + i] = -1; }
-                    out_score[i] = PSB_WORST_SCORE; out_hist[i] = -1; bestsc[i] = PSB_WORST_SCORE; frame[i] = -1;
+                    V.clear(i, N);
+                    frame[i] = -1;
                 }
             }
             else if (out_score[i] > cand) { cand = out_score[i]; cidx = i; }   // first best exit of the phone loop
@@ -1841,15 +1794,20 @@ extern "C" int psb_kws_batch_device(psb_hmmctx_t *c, const int16_t *d_senscr, co
     PSB_REQUIRE(c && utt_off && n_utt >= 0 && n_pl > 0 && pl_ssid && pl_tmat && n_kp >= 0 && kp_off && hits && n_hits &&
                 cap_per_utt > 0, "psb_kws_batch_device: bad argument");
     if (n_utt == 0) return PSB_OK;
-    PSB_REQUIRE(utt_off[0] == 0 && kp_off[0] == 0, "psb_kws_batch_device: offsets must start at 0");
-    PSB_REQUIRE(d_senscr || utt_off[n_utt] == 0, "psb_kws_batch_device: scores missing");
+    int rc = ctx_check_utts("psb_kws_batch_device", utt_off, n_utt, d_senscr);
+    if (rc) return rc;
+    PSB_REQUIRE(kp_off[0] == 0, "psb_kws_batch_device: offsets must start at 0");
+    for (int k = 0; k < n_kp; ++k)
+        PSB_REQUIRE(kp_off[k + 1] >= kp_off[k], "psb_kws_batch_device: kp_off not monotone at %d", k);
     const int N = c->n_emit, n_k = kp_off[n_kp], H = n_pl + n_k;
-    PSB_REQUIRE(n_k == 0 || (kp_ssid && kp_tmat && kp_thresh), "psb_kws_batch_device: keyphrase tables missing");
+    PSB_REQUIRE((n_kp == 0 || kp_thresh) && (n_k == 0 || (kp_ssid && kp_tmat)), "psb_kws_batch_device: keyphrase tables missing");
     PSB_REQUIRE(H <= 4 * 128, "psb_kws_batch_device: %d HMMs exceed the 512 this kernel keeps per utterance", H);
     PSB_CUDA(cudaSetDevice(c->device));
-    std::vector<uint16_t> sseq((size_t)c->n_sseq * N);
-    PSB_CUDA(cudaMemcpy(sseq.data(), c->d_sseq, sseq.size() * 2, cudaMemcpyDeviceToHost));
-    std::vector<uint16_t> senid((size_t)H * N);
+    std::vector<uint16_t> senid((size_t)H * N);      // the phone loop, then the keyphrases' chains
+    rc = ctx_senids(c, "psb_kws_batch_device (phone loop)", n_pl, pl_ssid, pl_tmat, senid.data(), N, 1);
+    if (rc) return rc;
+    rc = ctx_senids(c, "psb_kws_batch_device (keyphrases)", n_k, kp_ssid, kp_tmat, senid.data() + (size_t)n_pl * N, N, 1);
+    if (rc) return rc;
     std::vector<int32_t> ibuf;                       // utt_off | kp_off | kp_thresh | tmatid[H] | kp_of[n_k]
     ibuf.insert(ibuf.end(), utt_off, utt_off + n_utt + 1);
     const size_t o_kpoff = ibuf.size();
@@ -1857,50 +1815,28 @@ extern "C" int psb_kws_batch_device(psb_hmmctx_t *c, const int16_t *d_senscr, co
     const size_t o_thr = ibuf.size();
     for (int k = 0; k < n_kp; ++k) ibuf.push_back(kp_thresh[k]);
     const size_t o_tm = ibuf.size();
-    for (int i = 0; i < H; ++i) {
-        const int ss = i < n_pl ? pl_ssid[i] : kp_ssid[i - n_pl], tm = i < n_pl ? pl_tmat[i] : kp_tmat[i - n_pl];
-        PSB_REQUIRE(ss >= 0 && ss < c->n_sseq, "kws: ssid %d out of range", ss);
-        PSB_REQUIRE(tm >= 0 && tm < c->n_tmat, "kws: tmatid %d out of range", tm);
-        for (int s = 0; s < N; ++s) {
-            const uint16_t v = sseq[(size_t)ss * N + s];
-            PSB_REQUIRE(v < c->n_sen, "senone id %d out of range", v);
-            senid[(size_t)i * N + s] = v;
-        }
-        ibuf.push_back(tm);
-    }
+    ibuf.insert(ibuf.end(), pl_tmat, pl_tmat + n_pl);
+    if (n_k) ibuf.insert(ibuf.end(), kp_tmat, kp_tmat + n_k);
     const size_t o_of = ibuf.size();
-    for (int k = 0; k < n_kp; ++k) {
-        PSB_REQUIRE(kp_off[k + 1] >= kp_off[k], "psb_kws_batch_device: kp_off not monotone at %d", k);
+    for (int k = 0; k < n_kp; ++k)
         for (int j = kp_off[k]; j < kp_off[k + 1]; ++j) ibuf.push_back(k);
-    }
     const size_t o_nh = ibuf.size();
     ibuf.resize(o_nh + (size_t)n_utt, 0);
     const size_t smem = ((size_t)(2 * N + 4) * H + 64) * sizeof(int);
     int32_t *d_i = nullptr, *d_hits = nullptr;
     uint16_t *d_senid = nullptr;
     const size_t hits_n = (size_t)n_utt * cap_per_utt * 5;
-    cudaError_t e = cudaMalloc((void **)&d_i, ibuf.size() * 4);
-    if (e == cudaSuccess) e = cudaMalloc((void **)&d_hits, hits_n * 4);
-    if (e == cudaSuccess) e = cudaMalloc((void **)&d_senid, senid.size() * 2);
+    cudaError_t e = srch_reserve(c, 0, ibuf.size(), &d_i);
+    if (e == cudaSuccess) e = srch_reserve(c, 1, hits_n, &d_hits);
+    if (e == cudaSuccess) e = srch_reserve(c, 2, senid.size(), &d_senid);
     cudaStream_t st = c->stream;
     if (e == cudaSuccess) e = cudaMemcpyAsync(d_i, ibuf.data(), ibuf.size() * 4, cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess) e = cudaMemcpyAsync(d_senid, senid.data(), senid.size() * 2, cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(kws_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e == cudaSuccess) {
+    if (e == cudaSuccess)
         kws_kernel<<<(unsigned)n_utt, 128, smem, st>>>(d_senscr, d_i, dev_ctx(c), n_pl, n_kp, d_i + o_kpoff, d_i + o_thr, d_senid,
                                                       d_i + o_tm, d_i + o_of, beam, plp, d_hits, cap_per_utt, d_i + o_nh);
-        g_psb_launches.fetch_add(1, std::memory_order_relaxed);
-        e = cudaGetLastError();
-    }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(hits, d_hits, hits_n * 4, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(n_hits, d_i + o_nh, (size_t)n_utt * 4, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    cudaFree(d_i); cudaFree(d_hits); cudaFree(d_senid);
-    if (e != cudaSuccess) {
-        psb_set_error("psb_kws_batch_device: %s", cudaGetErrorString(e));
-        return PSB_ERR_CUDA;
-    }
-    return PSB_OK;
+    return ctx_finish(c, "psb_kws_batch_device", e, 1, {{hits, d_hits, hits_n * 4}, {n_hits, d_i + o_nh, (size_t)n_utt * 4}});
 }
 
 // ---------------------------------------------------------------------------------------
@@ -1943,14 +1879,15 @@ allphone_kernel(const int16_t *__restrict__ senscr, const int32_t *__restrict__ 
     int *sidx = sval + 32;                 // [32]
     int *wsum = sidx + 32;                 // [32]
     int *pci = wsum + 32;                  // [H] (LM) CI phone of the predecessor entry of this node's new entry, or -1
+    const HmmSoA<> V{score, hist, out_score, out_hist, bestsc, H};
     int32_t *my_hist = hist_out + (size_t)u * cap * ROW;
     int nh = 0;                                                   // uniform across the block
     const int chunk = (H + nt - 1) / nt, c0 = min(H, tid * chunk), c1 = min(H, c0 + chunk);
 
     // allphone_search_start: hmm_clear everything, hmm_enter(silence, 0, 0, 0)
     for (int i = tid; i < H; i += nt) {
-        for (int s = 0; s < N; ++s) { score[s * H + i] = PSB_WORST_SCORE; hist[s * H + i] = -1; }
-        out_score[i] = PSB_WORST_SCORE; out_hist[i] = -1; bestsc[i] = PSB_WORST_SCORE; frame[i] = -1; ex_idx[i] = -1;
+        V.clear(i, N);
+        frame[i] = -1; ex_idx[i] = -1;
     }
     __syncthreads();
     if (tid == 0) { score[start] = 0; hist[start] = 0; frame[start] = 0; }
@@ -1963,19 +1900,10 @@ allphone_kernel(const int16_t *__restrict__ senscr, const int32_t *__restrict__ 
         for (int i = tid; i < H; i += nt) {                       // phmm_eval_all
             if (frame[i] != t) continue;
             HmmReg h;
-#pragma unroll
-            for (int s = 0; s < PSB_HMM_MAX_NSTATE; ++s) {
-                h.score[s] = s < N ? score[s * H + i] : PSB_WORST_SCORE;
-                h.hist[s] = s < N ? hist[s * H + i] : -1;
-                h.senid[s] = s < N ? senid_g[(size_t)i * N + s] : PSB_BAD_SSID;
-            }
-            h.out_score = out_score[i]; h.out_hist = out_hist[i]; h.best = bestsc[i];
+            V.load(h, i, N, senid_g + (size_t)i * N, 1);
             const int b = hmm_step(h, c, tmatid_g[i], false, row);
             if (b > bs) bs = b;
-#pragma unroll
-            for (int s = 0; s < PSB_HMM_MAX_NSTATE; ++s)
-                if (s < N) { score[s * H + i] = h.score[s]; hist[s * H + i] = h.hist[s]; }
-            out_score[i] = h.out_score; out_hist[i] = h.out_hist; bestsc[i] = h.best;
+            V.store(h, i, N);
         }
         int dummy;
         const int best = block_reduce_max_pair<int>(bs, 0, sidx, sval, dummy);
@@ -2020,10 +1948,9 @@ allphone_kernel(const int16_t *__restrict__ senscr, const int32_t *__restrict__ 
                 ex_idx[i] = k++;
                 frame[i] = nf;
             }
-            else {                                                // hmm_clear
-                for (int s = 0; s < N; ++s) { score[s * H + i] = PSB_WORST_SCORE; hist[s * H + i] = -1; }
-                out_score[i] = PSB_WORST_SCORE; out_hist[i] = -1; bestsc[i] = PSB_WORST_SCORE; frame[i] = -1;
-                ex_idx[i] = -1;
+            else {
+                V.clear(i, N);
+                frame[i] = -1; ex_idx[i] = -1;
             }
         }
         nh += total;
@@ -2064,31 +1991,23 @@ static int allphone_common(psb_hmmctx_t *c, const int16_t *d_senscr, const int32
     PSB_REQUIRE(c && utt_off && n_utt >= 0 && n_nodes > 0 && ssid && tmatid && succ_off && hist && n_hist && cap_per_utt > 0 &&
                 start >= 0 && start < n_nodes, "psb_allphone_batch_device: bad argument");
     if (n_utt == 0) return PSB_OK;
-    PSB_REQUIRE(utt_off[0] == 0 && succ_off[0] == 0, "psb_allphone_batch_device: offsets must start at 0");
-    PSB_REQUIRE(d_senscr || utt_off[n_utt] == 0, "psb_allphone_batch_device: scores missing");
+    int rc = ctx_check_utts("psb_allphone_batch_device", utt_off, n_utt, d_senscr);
+    if (rc) return rc;
+    PSB_REQUIRE(succ_off[0] == 0, "psb_allphone_batch_device: offsets must start at 0");
     const int N = c->n_emit, H = n_nodes, n_links = succ_off[n_nodes];
     PSB_REQUIRE(n_links == 0 || succ, "psb_allphone_batch_device: successor lists missing");
     const size_t smem = ((size_t)(2 * N + 6) * H + 96) * sizeof(int);
     PSB_REQUIRE(smem <= 200 * 1024, "psb_allphone_batch_device: a graph of %d PHMMs does not fit shared memory "
                 "(context-independent graphs, -allphone_ci yes, have one node per phone)", H);
     PSB_CUDA(cudaSetDevice(c->device));
-    std::vector<uint16_t> sseq((size_t)c->n_sseq * N);
-    PSB_CUDA(cudaMemcpy(sseq.data(), c->d_sseq, sseq.size() * 2, cudaMemcpyDeviceToHost));
     std::vector<uint16_t> senid((size_t)H * N);
+    rc = ctx_senids(c, "psb_allphone_batch_device", H, ssid, tmatid, senid.data(), N, 1);
+    if (rc) return rc;
     // predecessor lists in node order (= the order the reference appends and walks history entries)
     std::vector<int32_t> ibuf;                       // utt_off | tmatid[H] | pred_off[H+1] | pred[n_links] | n_hist[n_utt]
     ibuf.insert(ibuf.end(), utt_off, utt_off + n_utt + 1);
     const size_t o_tm = ibuf.size();
-    for (int i = 0; i < H; ++i) {
-        PSB_REQUIRE(ssid[i] >= 0 && ssid[i] < c->n_sseq, "allphone: ssid[%d] out of range", i);
-        PSB_REQUIRE(tmatid[i] >= 0 && tmatid[i] < c->n_tmat, "allphone: tmatid[%d] out of range", i);
-        for (int s = 0; s < N; ++s) {
-            const uint16_t v = sseq[(size_t)ssid[i] * N + s];
-            PSB_REQUIRE(v < c->n_sen, "senone id %d out of range", v);
-            senid[(size_t)i * N + s] = v;
-        }
-        ibuf.push_back(tmatid[i]);
-    }
+    ibuf.insert(ibuf.end(), tmatid, tmatid + H);
     std::vector<int32_t> pcount((size_t)H + 1, 0);
     for (int i = 0; i < H; ++i) {
         PSB_REQUIRE(succ_off[i + 1] >= succ_off[i], "psb_allphone_batch_device: succ_off not monotone at %d", i);
@@ -2125,9 +2044,9 @@ static int allphone_common(psb_hmmctx_t *c, const int16_t *d_senscr, const int32
     int32_t *d_i = nullptr, *d_hist = nullptr;
     uint16_t *d_senid = nullptr;
     const size_t hist_n = (size_t)n_utt * cap_per_utt * ROW;
-    cudaError_t e = cudaMalloc((void **)&d_i, ibuf.size() * 4);
-    if (e == cudaSuccess) e = cudaMalloc((void **)&d_hist, hist_n * 4);
-    if (e == cudaSuccess) e = cudaMalloc((void **)&d_senid, senid.size() * 2);
+    cudaError_t e = srch_reserve(c, 0, ibuf.size(), &d_i);
+    if (e == cudaSuccess) e = srch_reserve(c, 1, hist_n, &d_hist);
+    if (e == cudaSuccess) e = srch_reserve(c, 2, senid.size(), &d_senid);
     cudaStream_t st = c->stream;
     if (e == cudaSuccess) e = cudaMemcpyAsync(d_i, ibuf.data(), ibuf.size() * 4, cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess) e = cudaMemcpyAsync(d_senid, senid.data(), senid.size() * 2, cudaMemcpyHostToDevice, st);
@@ -2142,18 +2061,9 @@ static int allphone_common(psb_hmmctx_t *c, const int16_t *d_senscr, const int32
             allphone_kernel<false><<<(unsigned)n_utt, 128, smem, st>>>(d_senscr, d_i, dev_ctx(c), H, d_senid, d_i + o_tm, d_i + o_poff,
                                                                       d_i + o_pred, start, beam, pbeam, inspen, d_hist, cap_per_utt,
                                                                       d_i + o_nh, 0, nullptr, nullptr, nullptr);
-        g_psb_launches.fetch_add(1, std::memory_order_relaxed);
-        e = cudaGetLastError();
     }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(hist, d_hist, hist_n * 4, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(n_hist, d_i + o_nh, (size_t)n_utt * 4, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    cudaFree(d_i); cudaFree(d_hist); cudaFree(d_senid);
-    if (e != cudaSuccess) {
-        psb_set_error("psb_allphone_batch_device: %s", cudaGetErrorString(e));
-        return PSB_ERR_CUDA;
-    }
-    return PSB_OK;
+    return ctx_finish(c, "psb_allphone_batch_device", e, 1,
+                      {{hist, d_hist, hist_n * 4}, {n_hist, d_i + o_nh, (size_t)n_utt * 4}});
 }
 
 extern "C" int psb_allphone_batch_device(psb_hmmctx_t *c, const int16_t *d_senscr, const int32_t *utt_off, int32_t n_utt,

@@ -379,3 +379,48 @@ __device__ __forceinline__ int hmm_step(HmmReg &h, const HmmCtxDev &c, int tmati
     if (mpx && n == 5) return hmm_step_5st_mpx(h, c, tp, senscr);
     return hmm_step_any(h, c, tp, senscr, mpx);
 }
+
+// An HMM set the whole-utterance kernels keep as a struct of arrays (shared or global memory): state s of
+// HMM i at [s * stride + i], the exit state and the best score at [i].  BEST = false: the caller keeps no
+// best score (best is not used), and a loaded HMM starts from WORST_SCORE.
+template <bool BEST = true>
+struct HmmSoA {
+    int *score, *hist;            // [n_emit][stride]
+    int *out_score, *out_hist;    // [stride]
+    int *best;                    // [stride]
+    int stride;
+
+    // HMM i into registers.  Its senone ids are sen[s * sen_stride]; for a multiplexed channel (mss given)
+    // its per-state senone-sequence ids are mss[s * stride + i] instead.
+    template <class SenT>
+    __device__ __forceinline__ void load(HmmReg &h, int i, int n, const SenT *sen, int sen_stride, const int *mss = nullptr) const
+    {
+#pragma unroll
+        for (int s = 0; s < PSB_HMM_MAX_NSTATE; ++s) {
+            h.score[s] = s < n ? score[s * stride + i] : PSB_WORST_SCORE;
+            h.hist[s] = s < n ? hist[s * stride + i] : -1;
+            h.senid[s] = s < n ? (mss ? mss[s * stride + i] : sen[s * sen_stride]) : PSB_BAD_SSID;
+        }
+        h.out_score = out_score[i]; h.out_hist = out_hist[i]; h.best = BEST ? best[i] : PSB_WORST_SCORE;
+    }
+    // HMM i back from registers; a multiplexed channel's senone-sequence ids, which follow the winning
+    // predecessors, go back to mss
+    __device__ __forceinline__ void store(const HmmReg &h, int i, int n, int *mss = nullptr) const
+    {
+#pragma unroll
+        for (int s = 0; s < PSB_HMM_MAX_NSTATE; ++s)
+            if (s < n) {
+                score[s * stride + i] = h.score[s]; hist[s * stride + i] = h.hist[s];
+                if (mss) mss[s * stride + i] = h.senid[s];
+            }
+        out_score[i] = h.out_score; out_hist[i] = h.out_hist;
+        if (BEST) best[i] = h.best;
+    }
+    // hmm_clear (hmm.c:180-196) of HMM i; each caller resets its own frame field
+    __device__ __forceinline__ void clear(int i, int n) const
+    {
+        for (int s = 0; s < n; ++s) { score[s * stride + i] = PSB_WORST_SCORE; hist[s * stride + i] = -1; }
+        out_score[i] = PSB_WORST_SCORE; out_hist[i] = -1;
+        if (BEST) best[i] = PSB_WORST_SCORE;
+    }
+};

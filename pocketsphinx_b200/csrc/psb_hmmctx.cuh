@@ -1,27 +1,27 @@
 // psb_hmmctx.cuh -- the HMM context object behind psb_hmmctx_t, shared by psb_hmm.cu (hmm_vit_eval,
-// phone loop, alignment, keyword spotting, phone decoding) and psb_search.cu (grammar / n-gram search).
+// phone loop, alignment, keyword spotting, phone decoding) and psb_search.cu (grammar / n-gram search),
+// and the plumbing its whole-utterance entry points share.
 #pragma once
 #include "psb_hmm.cuh"
 
+#include <initializer_list>
+
+// A context serves one host thread at a time.  Every entry point that runs on its stream returns with the
+// stream idle, so the next call, whichever entry point it is, may reuse the workspace slots.
 struct psb_hmmctx_s {
     int device;
     int n_emit, n_tmat, n_sseq, n_sen;
     uint8_t *d_tp;
-    uint16_t *d_sseq;
+    uint16_t *d_sseq, *h_sseq;    // [n_sseq][n_emit], on the device and on the host
     cudaStream_t stream;
     // staging for psb_hmm_vit_eval_batch
     psb_hmm_t *d_hmms, *h_hmms;
     size_t hmm_cap;
     int16_t *d_senscr, *h_senscr;
     int32_t *d_best, *h_best;
-    // grow-only workspace of psb_align_batch_* (token table, phone tables, results)
-    int32_t *d_al_i32, *d_al_tok;
-    uint16_t *d_al_senid;
-    int64_t *d_al_tokoff;
-    size_t al_i32_cap, al_tok_cap, al_senid_cap, al_tokoff_cap;
-    cudaEvent_t al_ev[2];
+    cudaEvent_t al_ev[2];         // around the last psb_align_batch_* kernel
     float last_align_ms;
-    // grow-only device workspace of the search entry points (psb_search.cu)
+    // grow-only device workspace of the whole-utterance entry points (srch_reserve)
     void *d_srch[10];
     size_t srch_cap[10];
 };
@@ -31,4 +31,75 @@ static inline HmmCtxDev dev_ctx(const psb_hmmctx_t *c)
     HmmCtxDev d;
     d.n_emit = c->n_emit; d.n_sen = c->n_sen; d.tp = c->d_tp; d.sseq = c->d_sseq;
     return d;
+}
+
+// Grow-only device workspace kept in the context: repeated calls (one per batch) do not pay
+// cudaMalloc / cudaFree again.
+template <class T>
+static cudaError_t srch_reserve(psb_hmmctx_t *c, int slot, size_t count, T **out)
+{
+    const size_t bytes = (count > 0 ? count : 1) * sizeof(T);
+    if (bytes > c->srch_cap[slot]) {
+        cudaFree(c->d_srch[slot]);
+        c->d_srch[slot] = nullptr; c->srch_cap[slot] = 0;
+        const cudaError_t e = cudaMalloc(&c->d_srch[slot], bytes + bytes / 4);
+        if (e != cudaSuccess) return e;
+        c->srch_cap[slot] = bytes + bytes / 4;
+    }
+    *out = (T *)c->d_srch[slot];
+    return cudaSuccess;
+}
+
+// The utterances of a whole-utterance entry point: offsets from 0 that never decrease, and scores wherever
+// there are frames.
+static inline int ctx_check_utts(const char *fn, const int32_t *utt_off, int32_t n_utt, const void *senscr)
+{
+    const int rc = psb_check_utt_off(fn, utt_off, n_utt);
+    if (rc) return rc;
+    PSB_REQUIRE(senscr || utt_off[n_utt] == 0, "%s: scores missing", fn);
+    return PSB_OK;
+}
+
+// hmm_init of n non-multiplexed HMMs (hmm.c:99-102): HMM i = (ssid[i], tmatid[i]) gets the senone ids of
+// its senone sequence, state s at senid[i * hmm_stride + s * state_stride].
+static inline int ctx_senids(const psb_hmmctx_t *c, const char *what, int n, const int32_t *ssid, const int32_t *tmatid,
+                             uint16_t *senid, size_t hmm_stride, size_t state_stride)
+{
+    const int N = c->n_emit;
+    for (int i = 0; i < n; ++i) {
+        PSB_REQUIRE(ssid[i] >= 0 && ssid[i] < c->n_sseq, "%s: ssid[%d] = %d out of range", what, i, ssid[i]);
+        PSB_REQUIRE(tmatid[i] >= 0 && tmatid[i] < c->n_tmat, "%s: tmatid[%d] = %d out of range", what, i, tmatid[i]);
+        for (int s = 0; s < N; ++s) {
+            const uint16_t v = c->h_sseq[(size_t)ssid[i] * N + s];
+            PSB_REQUIRE(v < c->n_sen, "%s: senone id %d out of range", what, v);
+            senid[i * hmm_stride + s * state_stride] = v;
+        }
+    }
+    return PSB_OK;
+}
+
+struct CtxCopy {
+    void *dst;
+    const void *src;
+    size_t bytes;
+};
+
+// The end of a whole-utterance entry point, after its launches (made only when e was cudaSuccess): count
+// them, copy the results back to the host, wait for the stream -- also after an error, so that the next
+// call finds it idle -- and turn a CUDA error into a message naming fn.
+static inline int ctx_finish(psb_hmmctx_t *c, const char *fn, cudaError_t e, int launches, std::initializer_list<CtxCopy> out)
+{
+    if (e == cudaSuccess) {
+        g_psb_launches.fetch_add(launches, std::memory_order_relaxed);
+        e = cudaGetLastError();
+    }
+    for (const CtxCopy &o : out)
+        if (e == cudaSuccess && o.bytes) e = cudaMemcpyAsync(o.dst, o.src, o.bytes, cudaMemcpyDeviceToHost, c->stream);
+    const cudaError_t s = cudaStreamSynchronize(c->stream);
+    if (e == cudaSuccess) e = s;
+    if (e != cudaSuccess) {
+        psb_set_error("%s: %s", fn, cudaGetErrorString(e));
+        return PSB_ERR_CUDA;
+    }
+    return PSB_OK;
 }

@@ -62,6 +62,15 @@ inline int psb_sm_count(int device)
         }                                                                                \
     } while (0)
 
+// Utterance offsets given from outside (utt_off[n_utt + 1], host): they start at 0 and never decrease.
+static inline int psb_check_utt_off(const char *fn, const int32_t *utt_off, int32_t n_utt)
+{
+    PSB_REQUIRE(utt_off[0] == 0, "%s: utt_off[0] must be 0", fn);
+    for (int u = 0; u < n_utt; ++u)
+        PSB_REQUIRE(utt_off[u + 1] >= utt_off[u], "%s: utt_off not monotone at %d", fn, u);
+    return PSB_OK;
+}
+
 static inline int roundup(int x, int m) { return (x + m - 1) / m * m; }
 
 // Gaussian record of one codeword in HBM/SMEM: {det, mean0, var0, mean1, var1, ...} padded

@@ -29,20 +29,12 @@ struct FsgDevEval {
     int P;
     __device__ __forceinline__ int operator()(const FsgWork &W, int p) const
     {
-        HmmReg h;
+        const HmmSoA<> V{W.score, W.hist, W.out_score, W.out_hist, W.best, P};
         const int N = c.n_emit;
-#pragma unroll
-        for (int s = 0; s < PSB_HMM_MAX_NSTATE; ++s) {
-            h.score[s] = s < N ? W.score[s * P + p] : PSB_WORST_SCORE;
-            h.hist[s] = s < N ? W.hist[s * P + p] : -1;
-            h.senid[s] = s < N ? senid_g[(size_t)p * N + s] : PSB_BAD_SSID;
-        }
-        h.out_score = W.out_score[p]; h.out_hist = W.out_hist[p]; h.best = W.best[p];
+        HmmReg h;
+        V.load(h, p, N, senid_g + (size_t)p * N, 1);
         const int b = hmm_step(h, c, tmatid_g[p], false, row);
-#pragma unroll
-        for (int s = 0; s < PSB_HMM_MAX_NSTATE; ++s)
-            if (s < N) { W.score[s * P + p] = h.score[s]; W.hist[s * P + p] = h.hist[s]; }
-        W.out_score[p] = h.out_score; W.out_hist[p] = h.out_hist; W.best[p] = h.best;
+        V.store(h, p, N);
         return b;
     }
 };
@@ -75,23 +67,6 @@ fsg_search_kernel(const int16_t *__restrict__ senscr, const int32_t *__restrict_
 
 }  // namespace
 
-// Grow-only device workspace kept in the context: repeated calls (one per batch) do not pay
-// cudaMalloc / cudaFree again (DESIGN 4.7).
-template <class T>
-static cudaError_t srch_reserve(psb_hmmctx_t *c, int slot, size_t count, T **out)
-{
-    const size_t bytes = (count > 0 ? count : 1) * sizeof(T);
-    if (bytes > c->srch_cap[slot]) {
-        cudaFree(c->d_srch[slot]);
-        c->d_srch[slot] = nullptr; c->srch_cap[slot] = 0;
-        const cudaError_t e = cudaMalloc(&c->d_srch[slot], bytes + bytes / 4);
-        if (e != cudaSuccess) return e;
-        c->srch_cap[slot] = bytes + bytes / 4;
-    }
-    *out = (T *)c->d_srch[slot];
-    return cudaSuccess;
-}
-
 static_assert(FSG_WORST_SCORE == PSB_WORST_SCORE, "score floor");
 static_assert(FSG_MAX_NSTATE == PSB_HMM_MAX_NSTATE, "state count");
 
@@ -101,10 +76,8 @@ extern "C" int psb_fsg_batch_device(psb_hmmctx_t *c, const psb_fsg_desc_t *g, co
 {
     PSB_REQUIRE(c && g && utt_off && n_utt >= 0 && hist && n_hist && cap_per_utt > 0, "psb_fsg_batch_device: bad argument");
     if (n_utt == 0) return PSB_OK;
-    PSB_REQUIRE(utt_off[0] == 0, "psb_fsg_batch_device: offsets must start at 0");
-    PSB_REQUIRE(d_senscr || utt_off[n_utt] == 0, "psb_fsg_batch_device: scores missing");
-    for (int u = 0; u < n_utt; ++u)
-        PSB_REQUIRE(utt_off[u + 1] >= utt_off[u], "psb_fsg_batch_device: utt_off not monotone at %d", u);
+    int rc = ctx_check_utts("psb_fsg_batch_device", utt_off, n_utt, d_senscr);
+    if (rc) return rc;
     PSB_REQUIRE(g->start_state >= 0 && g->start_state < g->n_state, "psb_fsg_batch_device: start state out of range");
     PSB_REQUIRE(g->silcipid >= 0 && g->silcipid < g->n_ciphone, "psb_fsg_batch_device: silence phone out of range");
     FsgFlat flat;
@@ -116,18 +89,9 @@ extern "C" int psb_fsg_batch_device(psb_hmmctx_t *c, const psb_fsg_desc_t *g, co
     }
     const int N = c->n_emit, P = flat.P;
     PSB_CUDA(cudaSetDevice(c->device));
-    std::vector<uint16_t> sseq((size_t)c->n_sseq * N);
-    PSB_CUDA(cudaMemcpy(sseq.data(), c->d_sseq, sseq.size() * 2, cudaMemcpyDeviceToHost));
     std::vector<uint16_t> senid((size_t)P * N);
-    for (int i = 0; i < P; ++i) {
-        PSB_REQUIRE(flat.ssid[i] >= 0 && flat.ssid[i] < c->n_sseq, "fsg: pnode %d: ssid out of range", i);
-        PSB_REQUIRE(flat.tmatid[i] >= 0 && flat.tmatid[i] < c->n_tmat, "fsg: pnode %d: tmatid out of range", i);
-        for (int s = 0; s < N; ++s) {
-            const uint16_t v = sseq[(size_t)flat.ssid[i] * N + s];
-            PSB_REQUIRE(v < c->n_sen, "senone id %d out of range", v);
-            senid[(size_t)i * N + s] = v;
-        }
-    }
+    rc = ctx_senids(c, "psb_fsg_batch_device (pnodes)", P, flat.ssid.data(), flat.tmatid.data(), senid.data(), N, 1);
+    if (rc) return rc;
     // one int32 block: graph | tmatid[P] | utt_off[n_utt+1] | n_hist[n_utt]
     std::vector<int32_t> ibuf(flat.buf);
     const size_t o_tm = ibuf.size();
@@ -155,16 +119,9 @@ extern "C" int psb_fsg_batch_device(psb_hmmctx_t *c, const psb_fsg_desc_t *g, co
         G.beam = g->beam; G.pbeam = g->pbeam; G.wbeam = g->wbeam; G.maxhmmpf = g->maxhmmpf;
         fsg_search_kernel<<<n_utt, FSG_THREADS, 0, st>>>(d_senscr, d_i + o_uo, dev_ctx(c), G, d_senid, d_i + o_tm, d_work, work_words,
                                                          d_hist, cap_per_utt, d_i + o_nh);
-        g_psb_launches.fetch_add(1, std::memory_order_relaxed);
-        e = cudaGetLastError();
     }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(hist, d_hist, hist_n * 4, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(n_hist, d_i + o_nh, (size_t)n_utt * 4, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) {
-        psb_set_error("psb_fsg_batch_device: %s", cudaGetErrorString(e));
-        return PSB_ERR_CUDA;
-    }
+    rc = ctx_finish(c, "psb_fsg_batch_device", e, 1, {{hist, d_hist, hist_n * 4}, {n_hist, d_i + o_nh, (size_t)n_utt * 4}});
+    if (rc) return rc;
     for (int u = 0; u < n_utt; ++u)
         PSB_REQUIRE(n_hist[u] >= 0, "psb_fsg_batch_device: scratch overflow in utterance %d (internal)", u);
     return PSB_OK;
@@ -189,24 +146,13 @@ struct ChanDevEval {
     const int16_t *row;
     __device__ __forceinline__ int operator()(const WorkT &W, int ch, bool mpx, int sid = -1) const      // sid: static-table index
     {
-        HmmReg h;
-        const int N = c.n_emit, M = G->M;
+        const HmmSoA<> V{W.score, W.hist, W.out_score, W.out_hist, W.best, G->M};
+        const int N = c.n_emit;
         if (sid < 0) sid = ch;
-#pragma unroll
-        for (int s = 0; s < PSB_HMM_MAX_NSTATE; ++s) {
-            h.score[s] = s < N ? W.score[s * M + ch] : PSB_WORST_SCORE;
-            h.hist[s] = s < N ? W.hist[s * M + ch] : -1;
-            h.senid[s] = s < N ? (mpx ? W.mss[s * M + ch] : G->senid[(size_t)sid * N + s]) : PSB_BAD_SSID;
-        }
-        h.out_score = W.out_score[ch]; h.out_hist = W.out_hist[ch]; h.best = W.best[ch];
+        HmmReg h;
+        V.load(h, ch, N, G->senid + (size_t)sid * N, 1, mpx ? W.mss : nullptr);
         const int b = hmm_step(h, c, G->tmatid[sid], mpx, row);
-#pragma unroll
-        for (int s = 0; s < PSB_HMM_MAX_NSTATE; ++s)
-            if (s < N) {
-                W.score[s * M + ch] = h.score[s]; W.hist[s * M + ch] = h.hist[s];
-                if (mpx) W.mss[s * M + ch] = h.senid[s];
-            }
-        W.out_score[ch] = h.out_score; W.out_hist[ch] = h.out_hist; W.best[ch] = h.best;
+        V.store(h, ch, N, mpx ? W.mss : nullptr);
         return b;
     }
 };
@@ -255,18 +201,14 @@ extern "C" int psb_ngram_fwdtree_batch_device(psb_hmmctx_t *c, const psb_ngram_d
     PSB_REQUIRE(c && g && g->info && g->model && g->ci_tmat && utt_off && n_utt >= 0 && bp && bss && bp_idx && result &&
                 bp_cap_per_utt > 0 && bss_cap_per_utt > 0, "psb_ngram_fwdtree_batch_device: bad argument");
     if (n_utt == 0) return PSB_OK;
-    PSB_REQUIRE(utt_off[0] == 0, "psb_ngram_fwdtree_batch_device: offsets must start at 0");
+    int rc = ctx_check_utts("psb_ngram_fwdtree_batch_device", utt_off, n_utt, d_senscr);
+    if (rc) return rc;
     PSB_REQUIRE(pl_window >= 0, "psb_ngram_fwdtree_batch_device: negative look-ahead window");
-    PSB_REQUIRE(d_senscr || utt_off[n_utt] == 0, "psb_ngram_fwdtree_batch_device: scores missing");
-    for (int u = 0; u < n_utt; ++u)
-        PSB_REQUIRE(utt_off[u + 1] >= utt_off[u], "psb_ngram_fwdtree_batch_device: utt_off not monotone at %d", u);
     PSB_CUDA(cudaSetDevice(c->device));
     const int N = c->n_emit;
-    std::vector<uint16_t> sseq((size_t)c->n_sseq * N);
-    PSB_CUDA(cudaMemcpy(sseq.data(), c->d_sseq, sseq.size() * 2, cudaMemcpyDeviceToHost));
     NgsFlat flat;
     std::string err;
-    if (ngs_flatten(g->info, g->model, (long long)g->model_len, g->lm_arrays, (long long)g->lm_arrays_len, g->ci_tmat, sseq.data(), c->n_sseq, N, c->n_tmat, c->n_sen, flat, err) != 0) {
+    if (ngs_flatten(g->info, g->model, (long long)g->model_len, g->lm_arrays, (long long)g->lm_arrays_len, g->ci_tmat, c->h_sseq, c->n_sseq, N, c->n_tmat, c->n_sen, flat, err) != 0) {
         psb_set_error("psb_ngram_fwdtree_batch_device: %s", err.c_str());
         return PSB_ERR_ARG;
     }
@@ -292,18 +234,10 @@ extern "C" int psb_ngram_fwdtree_batch_device(psb_hmmctx_t *c, const psb_ngram_d
         ngs_bind(flat, d_i);
         ngs_fwdtree_kernel<<<n_utt, NGS_THREADS, 0, st>>>(d_senscr, d_i + o_uo, dev_ctx(c), flat.G, d_work, work_words, d_pen, pl_window,
                                                           d_bp, bp_cap_per_utt, d_bss, bss_cap_per_utt, d_idx, d_i + o_res);
-        g_psb_launches.fetch_add(1, std::memory_order_relaxed);
-        e = cudaGetLastError();
     }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(bp, d_bp, n_bp * 4, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(bss, d_bss, n_bss * 4, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(bp_idx, d_idx, n_idx * 4, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(result, d_i + o_res, (size_t)n_utt * 12, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) {
-        psb_set_error("psb_ngram_fwdtree_batch_device: %s", cudaGetErrorString(e));
-        return PSB_ERR_CUDA;
-    }
+    rc = ctx_finish(c, "psb_ngram_fwdtree_batch_device", e, 1,
+                    {{bp, d_bp, n_bp * 4}, {bss, d_bss, n_bss * 4}, {bp_idx, d_idx, n_idx * 4}, {result, d_i + o_res, (size_t)n_utt * 12}});
+    if (rc) return rc;
     for (int u = 0; u < n_utt; ++u) {
         PSB_REQUIRE(result[u * 3 + 2] != -1, "psb_ngram_fwdtree_batch_device: utterance %d overflowed the backpointer table "
                     "or the score stack (%d entries / %d scores allowed)", u, bp_cap_per_utt, bss_cap_per_utt);
@@ -370,11 +304,10 @@ extern "C" int psb_ngram_fwdflat_batch_device(psb_hmmctx_t *c, const psb_ngram_d
                 bss && bp_idx && result && first_cap_per_utt > 0 && bp_cap_per_utt > 0 && bss_cap_per_utt > 0,
                 "psb_ngram_fwdflat_batch_device: bad argument (the descriptor needs ci_ssid for this pass)");
     if (n_utt == 0) return PSB_OK;
-    PSB_REQUIRE(utt_off[0] == 0, "psb_ngram_fwdflat_batch_device: offsets must start at 0");
-    PSB_REQUIRE(d_senscr || utt_off[n_utt] == 0, "psb_ngram_fwdflat_batch_device: scores missing");
+    int rc = ctx_check_utts("psb_ngram_fwdflat_batch_device", utt_off, n_utt, d_senscr);
+    if (rc) return rc;
     int t_max = 0;
     for (int u = 0; u < n_utt; ++u) {
-        PSB_REQUIRE(utt_off[u + 1] >= utt_off[u], "psb_ngram_fwdflat_batch_device: utt_off not monotone at %d", u);
         PSB_REQUIRE(n_first[u] >= -1 && n_first[u] <= first_cap_per_utt, "psb_ngram_fwdflat_batch_device: n_first[%d] out of range", u);
         const int32_t *b = bp_first + (size_t)u * first_cap_per_utt * NGS_BP_ROW;
         const int T = utt_off[u + 1] - utt_off[u];
@@ -387,11 +320,9 @@ extern "C" int psb_ngram_fwdflat_batch_device(psb_hmmctx_t *c, const psb_ngram_d
     }
     PSB_CUDA(cudaSetDevice(c->device));
     const int N = c->n_emit;
-    std::vector<uint16_t> sseq((size_t)c->n_sseq * N);
-    PSB_CUDA(cudaMemcpy(sseq.data(), c->d_sseq, sseq.size() * 2, cudaMemcpyDeviceToHost));
     NgfFlat flat;
     std::string err;
-    if (ngf_flatten(g->info, g->model, (long long)g->model_len, g->lm_arrays, (long long)g->lm_arrays_len, g->ci_tmat, g->ci_ssid, sseq.data(), c->n_sseq, N, c->n_tmat, c->n_sen, flat, err) != 0) {
+    if (ngf_flatten(g->info, g->model, (long long)g->model_len, g->lm_arrays, (long long)g->lm_arrays_len, g->ci_tmat, g->ci_ssid, c->h_sseq, c->n_sseq, N, c->n_tmat, c->n_sen, flat, err) != 0) {
         psb_set_error("psb_ngram_fwdflat_batch_device: %s", err.c_str());
         return PSB_ERR_ARG;
     }
@@ -421,18 +352,10 @@ extern "C" int psb_ngram_fwdflat_batch_device(psb_hmmctx_t *c, const psb_ngram_d
         ngf_bind(flat, d_i);
         ngs_fwdflat_kernel<<<n_utt, NGS_THREADS, 0, st>>>(d_senscr, d_i + o_uo, dev_ctx(c), flat.G, d_work, work_words, d_in, first_cap_per_utt,
                                                           d_i + o_nin, 1, d_bp, bp_cap_per_utt, d_bss, bss_cap_per_utt, d_idx, d_i + o_res);
-        g_psb_launches.fetch_add(1, std::memory_order_relaxed);
-        e = cudaGetLastError();
     }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(bp, d_bp, n_bp * 4, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(bss, d_bss, n_bss * 4, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(bp_idx, d_idx, n_idx * 4, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(result, d_i + o_res, (size_t)n_utt * 12, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) {
-        psb_set_error("psb_ngram_fwdflat_batch_device: %s", cudaGetErrorString(e));
-        return PSB_ERR_CUDA;
-    }
+    rc = ctx_finish(c, "psb_ngram_fwdflat_batch_device", e, 1,
+                    {{bp, d_bp, n_bp * 4}, {bss, d_bss, n_bss * 4}, {bp_idx, d_idx, n_idx * 4}, {result, d_i + o_res, (size_t)n_utt * 12}});
+    if (rc) return rc;
     for (int u = 0; u < n_utt; ++u) {
         PSB_REQUIRE(result[u * 3 + 2] != -1, "psb_ngram_fwdflat_batch_device: utterance %d overflowed the backpointer table "
                     "or the score stack (%d entries / %d scores allowed)", u, bp_cap_per_utt, bss_cap_per_utt);
@@ -457,22 +380,18 @@ extern "C" int psb_ngram_two_pass_batch_device(psb_hmmctx_t *c, const psb_ngram_
                 first_cap_per_utt > 0 && first_bss_cap_per_utt > 0 && bp_cap_per_utt > 0 && bss_cap_per_utt > 0 && pl_window >= 0,
                 "psb_ngram_two_pass_batch_device: bad argument");
     if (n_utt == 0) return PSB_OK;
-    PSB_REQUIRE(utt_off[0] == 0, "psb_ngram_two_pass_batch_device: offsets must start at 0");
-    PSB_REQUIRE(d_senscr || utt_off[n_utt] == 0, "psb_ngram_two_pass_batch_device: scores missing");
+    int rc = ctx_check_utts("psb_ngram_two_pass_batch_device", utt_off, n_utt, d_senscr);
+    if (rc) return rc;
     int t_max = 0;
-    for (int u = 0; u < n_utt; ++u) {
-        PSB_REQUIRE(utt_off[u + 1] >= utt_off[u], "psb_ngram_two_pass_batch_device: utt_off not monotone at %d", u);
+    for (int u = 0; u < n_utt; ++u)
         if (utt_off[u + 1] - utt_off[u] > t_max) t_max = utt_off[u + 1] - utt_off[u];
-    }
     PSB_CUDA(cudaSetDevice(c->device));
     const int N = c->n_emit;
-    std::vector<uint16_t> sseq((size_t)c->n_sseq * N);
-    PSB_CUDA(cudaMemcpy(sseq.data(), c->d_sseq, sseq.size() * 2, cudaMemcpyDeviceToHost));
     NgsFlat f1;
     NgfFlat f2;
     std::string err;
-    if (ngs_flatten(g->info, g->model, (long long)g->model_len, g->lm_arrays, (long long)g->lm_arrays_len, g->ci_tmat, sseq.data(), c->n_sseq, N, c->n_tmat, c->n_sen, f1, err) != 0 ||
-        ngf_flatten(g->info, g->model, (long long)g->model_len, g->lm_arrays, (long long)g->lm_arrays_len, g->ci_tmat, g->ci_ssid, sseq.data(), c->n_sseq, N, c->n_tmat, c->n_sen, f2, err) != 0) {
+    if (ngs_flatten(g->info, g->model, (long long)g->model_len, g->lm_arrays, (long long)g->lm_arrays_len, g->ci_tmat, c->h_sseq, c->n_sseq, N, c->n_tmat, c->n_sen, f1, err) != 0 ||
+        ngf_flatten(g->info, g->model, (long long)g->model_len, g->lm_arrays, (long long)g->lm_arrays_len, g->ci_tmat, g->ci_ssid, c->h_sseq, c->n_sseq, N, c->n_tmat, c->n_sen, f2, err) != 0) {
         psb_set_error("psb_ngram_two_pass_batch_device: %s", err.c_str());
         return PSB_ERR_ARG;
     }
@@ -510,20 +429,12 @@ extern "C" int psb_ngram_two_pass_batch_device(psb_hmmctx_t *c, const psb_ngram_
                                                           first_cap_per_utt, d_bss1, first_bss_cap_per_utt, d_idx1, d_i + o_r1);
         ngs_fwdflat_kernel<<<n_utt, NGS_THREADS, 0, st>>>(d_senscr, d_i + o_uo, dev_ctx(c), f2.G, d_work, ww, d_bp1, first_cap_per_utt,
                                                           d_i + o_r1, 3, d_bp2, bp_cap_per_utt, d_bss2, bss_cap_per_utt, d_idx2, d_i + o_r2);
-        g_psb_launches.fetch_add(2, std::memory_order_relaxed);
-        e = cudaGetLastError();
     }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(bp, d_bp2, n_bp2 * 4, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(bss, d_bss2, n_bss2 * 4, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(bp_idx, d_idx2, n_idx * 4, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(result, d_i + o_r2, (size_t)n_utt * 12, cudaMemcpyDeviceToHost, st);
     std::vector<int32_t> r1((size_t)n_utt * 3);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(r1.data(), d_i + o_r1, (size_t)n_utt * 12, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) {
-        psb_set_error("psb_ngram_two_pass_batch_device: %s", cudaGetErrorString(e));
-        return PSB_ERR_CUDA;
-    }
+    rc = ctx_finish(c, "psb_ngram_two_pass_batch_device", e, 2,
+                    {{bp, d_bp2, n_bp2 * 4}, {bss, d_bss2, n_bss2 * 4}, {bp_idx, d_idx2, n_idx * 4},
+                     {result, d_i + o_r2, (size_t)n_utt * 12}, {r1.data(), d_i + o_r1, (size_t)n_utt * 12}});
+    if (rc) return rc;
     if (first_result) memcpy(first_result, r1.data(), r1.size() * 4);
     for (int u = 0; u < n_utt; ++u) {
         PSB_REQUIRE(r1[(size_t)u * 3 + 2] != -1, "psb_ngram_two_pass_batch_device: utterance %d: first pass overflowed its tables (%d entries / %d scores)",
