@@ -543,42 +543,58 @@ void psb_fe_free(psb_fe_t *fe);
 /* frames fe_process_frames + fe_end_utt produce for n_samples (fe_interface.c:352-545) */
 int32_t psb_fe_n_frames(const psb_fe_t *fe, int64_t n_samples);
 /* pcm: the utterances' samples back to back, samp_off int64[n_utt + 1] (host).  Outputs:
- * frame_off int32[n_utt + 1] (host), feats float [frames][3 * n_cep], mfcc (may be NULL) float
- * [frames][n_cep] = the cepstra after CMN.  *ms (may be NULL) = device time of the two kernels. */
+ * frame_off int32[n_utt + 1] (host), feats float [frames][psb_fe_feat_dim], mfcc (may be NULL) float
+ * [frames][n_cep] = the cepstra after CMN and AGC (what the reference's buffers hold after
+ * feat_cmn + feat_agc, which work in place).  *ms (may be NULL) = device time of the kernels. */
 int psb_fe_process_host(psb_fe_t *fe, const int16_t *pcm, const int64_t *samp_off, int32_t n_utt,
                         float *feats, float *mfcc, int32_t *frame_off);
 int psb_fe_process_device(psb_fe_t *fe, const int16_t *d_pcm, const int64_t *samp_off, int32_t n_utt,
                           float *d_feats, float *d_mfcc, int32_t *frame_off, float *ms);
 /* device copy of the features of the last psb_fe_process_host call, and their dimension: 39 for
- * 1s_c_d_dd and s3_1x39, 51 for s2_4x (its four streams 12 + 24 + 3 + 12 back to back) */
+ * 1s_c_d_dd and s3_1x39, 51 for s2_4x (its four streams 12 + 24 + 3 + 12 back to back), the LDA
+ * output dimension with a transform */
 const float *psb_fe_device_feats(const psb_fe_t *fe);
 int32_t psb_fe_feat_dim(const psb_fe_t *fe);
 
-/* Feature type, CMN and dither options (feat_init, cmn_set_repr, fe_init_dither).  With them,
- * psb_fe_desc_t.window and .cmn are not read.  o == NULL is psb_fe_create. */
+/* Feature type, CMN, AGC, LDA and dither options (feat_init, feat_read_lda, cmn_set_repr,
+ * fe_init_dither).  With them, psb_fe_desc_t.window and .cmn are not read.  o == NULL is
+ * psb_fe_create.  Per utterance the cepstra go through CMN (with -varnorm), then AGC on c0, then
+ * the dynamic features, then the LDA transform (feat_s2mfc2feat_block_utt, feat.c:1277-1307).
+ * All-zero AGC / LDA fields select neither. */
 #define PSB_FE_MAX_CEP 32
 enum { PSB_FEAT_1S_C_D_DD = 0, PSB_FEAT_S2_4X = 1, PSB_FEAT_S3_1X39 = 2 };   /* -feat (s3_1x39 = 1s_12c_12d_3p_12dd) */
 enum { PSB_CMN_NONE = 0, PSB_CMN_BATCH = 1, PSB_CMN_LIVE = 2 };            /* -cmn (current = batch) */
+enum { PSB_AGC_NONE = 0, PSB_AGC_MAX = 1, PSB_AGC_EMAX = 2, PSB_AGC_NOISE = 3 };   /* -agc (agc.h) */
 typedef struct psb_fe_opts_s {
     int32_t feat;                          /* PSB_FEAT_*; s2_4x and s3_1x39 need n_cep == 13 */
     int32_t cmn;                           /* PSB_CMN_* */
-    int32_t varnorm;                       /* -varnorm: must be 0 (not implemented; live CMN refuses it too) */
+    int32_t varnorm;                       /* -varnorm: 0 / 1, batch CMN only (live CMN refuses it) */
     int32_t dither;                        /* -dither: 0 / 1 */
     int32_t seed;                          /* -seed: the MT19937 seed, init_genrand((unsigned long)seed) */
     float cmn_init[PSB_FE_MAX_CEP];        /* -cmninit as cmn_set_repr parses it; unused entries 0 */
+    int32_t agc;                           /* PSB_AGC_*; emax carries its estimate across a session */
+    float agc_thresh;                      /* -agcthresh (agc_t.noise_thresh; the reference's default is 2.0),
+                                              read by PSB_AGC_NOISE only */
+    const float *lda;                      /* -lda: lda[0] of the feature_transform file, [lda_rows][lda_cols]
+                                              row-major, eigenvectors in rows; NULL = no transform.  Copied
+                                              by psb_fe_create_ex */
+    int32_t lda_rows, lda_cols;            /* lda_cols must be the feature dimension; not with s2_4x */
+    int32_t ldadim;                        /* -ldadim: rows used, if 0 < ldadim <= lda_rows; else lda_rows */
 } psb_fe_opts_t;
 int psb_fe_create_ex(const psb_fe_desc_t *d, const psb_fe_opts_t *o, int device, psb_fe_t **out);
 
-/* What a ps_decoder_t carries from one utterance to the next: the live-CMN state (cmn_t) and the
- * dither generator (genrand.c).  ps_start_stream resets neither. */
+/* What a ps_decoder_t carries from one utterance to the next: the live-CMN state (cmn_t), the
+ * dither generator (genrand.c) and the emax AGC estimate (agc_t).  ps_start_stream resets none. */
 typedef struct psb_fe_state_s {
     float cmn_mean[PSB_FE_MAX_CEP], cmn_sum[PSB_FE_MAX_CEP];
     int32_t cmn_nframe;
     int32_t mt_index;                      /* mti: 624 = a twist is due */
     uint32_t mt[624];
+    float agc_max, agc_obs_max, agc_obs_max_sum;   /* agc_t.max, obs_max, obs_max_sum */
+    int32_t agc_obs_frame, agc_obs_utt;            /* agc_t.obs_frame, obs_utt */
 } psb_fe_state_t;
-/* the state fe_init + cmn_set_repr leave: mean = cmn_init, sum = mean * 500, nframe = 500,
- * init_genrand(seed) */
+/* the state fe_init + cmn_set_repr + agc_init + agc_emax_set leave: mean = cmn_init, sum = mean * 500,
+ * nframe = 500, init_genrand(seed), agc_max = 5 (10 with CMN none), the other AGC fields 0 */
 int psb_fe_state_init(const psb_fe_t *fe, psb_fe_state_t *s);
 /* Names the sessions of the next psb_fe_process_* / psb_decode_batch_pcm_host call: session s is
  * utterances sess_off[s] .. sess_off[s + 1] - 1 (in decode order; sess_off[0] = 0, sess_off[n_sess]

@@ -39,12 +39,14 @@ class FeDesc(C.Structure):
 
 class FeOpts(C.Structure):
     _fields_ = [("feat", C.c_int32), ("cmn", C.c_int32), ("varnorm", C.c_int32), ("dither", C.c_int32), ("seed", C.c_int32),
-                ("cmn_init", C.c_float * 32)]
+                ("cmn_init", C.c_float * 32), ("agc", C.c_int32), ("agc_thresh", C.c_float), ("lda", C.c_void_p),
+                ("lda_rows", C.c_int32), ("lda_cols", C.c_int32), ("ldadim", C.c_int32)]
 
 
 class FeState(C.Structure):
     _fields_ = [("cmn_mean", C.c_float * 32), ("cmn_sum", C.c_float * 32), ("cmn_nframe", C.c_int32), ("mt_index", C.c_int32),
-                ("mt", C.c_uint32 * 624)]
+                ("mt", C.c_uint32 * 624), ("agc_max", C.c_float), ("agc_obs_max", C.c_float), ("agc_obs_max_sum", C.c_float),
+                ("agc_obs_frame", C.c_int32), ("agc_obs_utt", C.c_int32)]
 
 
 class FsgDesc(C.Structure):

@@ -654,8 +654,9 @@ def ngram_segments(info, model, bp, bss, entry, lm_arrays=None, second_pass=Fals
 class FrontEnd:
     """fe/ + feat/ for whole batches on the device.  `desc` is the dict of fe_tables.make_fe_desc() -- or the
     same arrays taken out of the reference's fe_t.  `opts` (fe_tables.make_fe_opts(), optional) selects the
-    feature type, CMN (including live), -cmninit and dither; without it every utterance is a fresh stream with
-    desc's 1s_c_d_dd features and CMN."""
+    feature type, CMN (including live, and -varnorm), -cmninit, AGC, an LDA transform and dither; without it every
+    utterance is a fresh stream with desc's 1s_c_d_dd features and CMN.  feat_dim is the LDA output dimension when
+    there is a transform.  The cepstra process_host returns (want_mfcc) are the ones after CMN and AGC."""
 
     def __init__(self, desc, device=0, opts=None):
         from ._lib import FeDesc, FeOpts
@@ -687,6 +688,12 @@ class FrontEnd:
             v = np.asarray(opts["cmn_init"], np.float32).ravel()[:32]
             ci[:v.size] = v
             o.cmn_init[:] = ci.tolist()
+            o.agc, o.agc_thresh = int(opts.get("agc", 0)), float(opts.get("agc_thresh", 2.0))
+            if opts.get("lda") is not None:
+                a = np.ascontiguousarray(opts["lda"], np.float32)
+                assert a.ndim == 2
+                self._keep["lda"] = a
+                o.lda, (o.lda_rows, o.lda_cols), o.ldadim = a.ctypes.data, a.shape, int(opts.get("ldadim", 0))
             check(lib().psb_fe_create_ex(C.byref(d), C.byref(o), device, C.byref(h)), "psb_fe_create_ex")
         self.h = h
         self.feat_dim = lib().psb_fe_feat_dim(h)
@@ -734,7 +741,7 @@ class FrontEnd:
 
     def process_host(self, pcm, samp_off, want_mfcc=False):
         """pcm int16 (utterances back to back), samp_off int64 [n_utt+1] -> (feats [T][feat_dim],
-        frame_off int32 [n_utt+1][, mfcc after CMN [T][n_cep]])."""
+        frame_off int32 [n_utt+1][, mfcc after CMN and AGC [T][n_cep]])."""
         pcm = np.ascontiguousarray(pcm, np.int16)
         samp_off = np.ascontiguousarray(samp_off, np.int64)
         n_utt = len(samp_off) - 1

@@ -9,11 +9,13 @@
 //   fe_remove_noise and its helpers                                  (fe_noise.c:109-364)
 //   fe_mel_cep, fe_spec2cep / fe_dct2, fe_lifter                     (:1244-1349)
 //   frame counting of fe_process_frames + fe_end_utt                 (fe_interface.c:352-545)
-//   cmn (batch)                                                      (feat/cmn.c:136-200)
+//   cmn (batch, with or without varnorm)                             (feat/cmn.c:165-232)
+//   agc_max / agc_emax + agc_emax_update / agc_noise on c0           (feat/agc.c:110-216, feat.c:941-966)
 //   feat_1s_c_d_dd_cep2feat with replicated edges                    (feat/feat.c:579-622, 1243-1330)
 //   feat_s2_4x_cep2feat / feat_s3_1x39_cep2feat                      (feat/feat.c:425-538)
 //   cmn_live + cmn_live_shiftwin + cmn_live_update over a session    (feat/cmn_live.c, feat.c:917-938)
 //   dither: MT19937 (util/genrand.c) in the draw order of fe_process_frames + fe_end_utt
+//   feat_lda_transform                                               (feat/lda.c:139-159)
 // All tables (window, twiddles, mel filters, DCT cosines, lifter) are INPUTS: the host builds
 // them with the reference's own init code / libm and passes them in psb_fe_desc_t.  The only
 // operation that is not bit-reproducible is log(): device libm vs glibc can differ in the last
@@ -45,6 +47,10 @@ struct psb_fe_s {
     int64_t *d_samp_off; int32_t *d_frame_off; int32_t *d_frame_utt; size_t utt_cap, fu_cap;
     // psb_fe_create_ex options and sessions
     int feat, feat_dim, dither, seed;
+    int varnorm, agc, stream_dim;             // stream_dim: the features' dimension before LDA
+    float agc_thresh;
+    float *d_lda;                             // [feat_dim][stream_dim], NULL without LDA
+    float *d_raw; size_t raw_cap;             // [frames][stream_dim]: the features LDA reads
     float cmn_init[PSB_FE_MAX_CEP];
     std::vector<int32_t> sess_off;            // set by psb_fe_set_sessions for the next call only
     std::vector<psb_fe_state_t> states;       // in: the next call's sessions; out: after it
@@ -201,7 +207,8 @@ fe_frame_kernel(FeDev p, const int16_t *__restrict__ pcm, const int64_t *__restr
 }
 
 // One CTA (64 threads) per utterance: noise removal (sequential over frames), log, cepstral
-// transform, lifter; then batch CMN; then the dynamic features.
+// transform, lifter; then batch CMN (VARNORM: with variance normalisation); then the dynamic features.
+template <bool VARNORM>
 __global__ void __launch_bounds__(64)
 fe_utt_kernel(FeDev p, const int32_t *__restrict__ frame_off, double *__restrict__ mfspec,
               float *__restrict__ mfcc, float *__restrict__ feats, int cmn, int window)
@@ -311,9 +318,29 @@ fe_utt_kernel(FeDev p, const int32_t *__restrict__ frame_off, double *__restrict
             mean_s[tid] = __fdiv_rn(sum, (float)cnt);
         }
         __syncthreads();
-        for (int i = tid; i < T * nc; i += blockDim.x) {
-            float *v = mfcc + (size_t)f0 * nc + i;
-            *v = __fsub_rn(*v, mean_s[i % nc]);
+        if constexpr (VARNORM) {
+            // cmn.c:209-231: the variance sums over every frame, c0 >= 0 or not, in frame order;
+            // inverse standard deviation (float)sqrt((double)n_frame / var)
+            __shared__ float istd_s[FE_MAX_CEP];
+            if (tid < nc) {
+                float var = 0.f;
+                for (int t = 0; t < T; ++t) {
+                    const float d = __fsub_rn(mfcc[(size_t)(f0 + t) * nc + tid], mean_s[tid]);
+                    var = __fadd_rn(var, __fmul_rn(d, d));
+                }
+                istd_s[tid] = __double2float_rn(__dsqrt_rn(__ddiv_rn((double)T, (double)var)));
+            }
+            __syncthreads();
+            for (int i = tid; i < T * nc; i += blockDim.x) {
+                float *v = mfcc + (size_t)f0 * nc + i;
+                *v = __fmul_rn(__fsub_rn(*v, mean_s[i % nc]), istd_s[i % nc]);
+            }
+        }
+        else {
+            for (int i = tid; i < T * nc; i += blockDim.x) {
+                float *v = mfcc + (size_t)f0 * nc + i;
+                *v = __fsub_rn(*v, mean_s[i % nc]);
+            }
         }
         __threadfence_block();
         __syncthreads();
@@ -484,6 +511,114 @@ __global__ void fe_feat_kernel(const int32_t *__restrict__ frame_off, const int3
 #undef CEP
 }
 
+// The extreme of c0 over T frames as the reference's sequential scans find it: the running value is
+// replaced only by a strictly greater (MAX) / smaller value, so ties keep the earliest frame and a NaN
+// never replaces it.  SEED: the scan starts from frame 0's value, as agc_max and agc_noise do (a NaN
+// there is kept); else it starts empty and skips NaNs (agc_emax compares against the running
+// obs_max instead).  Each lane scans a contiguous run of frames; the runs are combined in frame
+// order.  Returns in every lane whether any value was taken, and the value in *out.
+template <bool MAX, bool SEED>
+__device__ bool c0_extreme(const float *__restrict__ c0, int T, int nc, float *out)
+{
+    const int lane = threadIdx.x & 31, run = (T + 31) / 32;
+    const int lo = min(lane * run, T), hi = min(lo + run, T);
+    bool has = false;
+    float v = 0.f;
+    for (int t = lo; t < hi; ++t) {
+        const float x = c0[(size_t)t * nc];
+        if ((SEED && t == 0) || (!isnan(x) && (!has || (MAX ? x > v : x < v)))) { v = x; has = true; }
+    }
+    for (int s = 1; s < 32; s <<= 1) {
+        const float ov = __shfl_down_sync(0xffffffffu, v, s);
+        const bool oh = __shfl_down_sync(0xffffffffu, (int)has, s) != 0;
+        if ((lane & (2 * s - 1)) == 0 && lane + s < 32 && oh && (!has || (MAX ? ov > v : ov < v))) { v = ov; has = true; }
+    }
+    *out = __shfl_sync(0xffffffffu, v, 0);
+    return __shfl_sync(0xffffffffu, (int)has, 0) != 0;
+}
+
+// AGC on c0 after CMN (feat_agc with beginutt and endutt, feat.c:941-966), one warp per utterance
+// (max, noise) or per session (emax: its utterances in order, agc_emax then agc_emax_update each;
+// the update ps_end_utt repeats through feat_update_stats finds obs_frame 0 and changes nothing).
+template <int AGC>
+__global__ void __launch_bounds__(32)
+fe_agc_kernel(const int32_t *__restrict__ sess_off, const int32_t *__restrict__ frame_off, float *__restrict__ mfcc,
+              int nc, float thresh, psb_fe_state_t *__restrict__ state)
+{
+    const int lane = threadIdx.x;
+    int u0 = blockIdx.x, u1 = blockIdx.x + 1;
+    float emax = 0.f, obs_max = 0.f, obs_sum = 0.f;
+    int obs_frame = 0, obs_utt = 0;
+    if constexpr (AGC == PSB_AGC_EMAX) {
+        const psb_fe_state_t *st = state + blockIdx.x;
+        u0 = sess_off[blockIdx.x]; u1 = sess_off[blockIdx.x + 1];
+        emax = st->agc_max; obs_max = st->agc_obs_max; obs_sum = st->agc_obs_max_sum;
+        obs_frame = st->agc_obs_frame; obs_utt = st->agc_obs_utt;
+    }
+    for (int u = u0; u < u1; ++u) {
+        const int f0 = frame_off[u], T = frame_off[u + 1] - f0;
+        float *c0 = mfcc + (size_t)f0 * nc;
+        float sub = 0.f, m;
+        bool apply = T > 0;
+        if constexpr (AGC == PSB_AGC_MAX) {                              // agc_max (agc.c:110-127)
+            if (T > 0) c0_extreme<true, true>(c0, T, nc, &sub);
+        }
+        else if constexpr (AGC == PSB_AGC_NOISE) {                       // agc_noise (agc.c:181-216)
+            if (T > 0) {
+                c0_extreme<false, true>(c0, T, nc, &m);
+                const float lim = __fadd_rn(m, thresh);
+                float sum = 0.f;
+                int cnt = 0;
+                if (lane == 0)
+                    for (int t = 0; t < T; ++t) {
+                        const float x = c0[(size_t)t * nc];
+                        if (x < lim) { sum = __fadd_rn(sum, x); ++cnt; }
+                    }
+                cnt = __shfl_sync(0xffffffffu, cnt, 0);
+                sub = __shfl_sync(0xffffffffu, cnt > 0 ? __fdiv_rn(sum, (float)cnt) : 0.f, 0);
+                apply = cnt > 0;
+            }
+        }
+        else {                                                           // agc_emax + agc_emax_update (agc.c:143-178)
+            sub = emax;
+            if (T > 0 && c0_extreme<true, false>(c0, T, nc, &m) && m > obs_max) { obs_max = m; obs_frame = 1; }
+            if (obs_frame) {
+                obs_sum = __fadd_rn(obs_sum, obs_max);
+                ++obs_utt;
+                emax = __fdiv_rn(obs_sum, (float)obs_utt);
+                if (obs_utt == 16) { obs_sum = __fdiv_rn(obs_sum, 2.f); obs_utt = 8; }
+            }
+            obs_frame = 0;
+            obs_max = -1000.f;
+        }
+        if (apply)
+            for (int t = lane; t < T; t += 32) c0[(size_t)t * nc] = __fsub_rn(c0[(size_t)t * nc], sub);
+    }
+    if constexpr (AGC == PSB_AGC_EMAX)
+        if (lane == 0) {
+            psb_fe_state_t *st = state + blockIdx.x;
+            st->agc_max = emax; st->agc_obs_max = obs_max; st->agc_obs_max_sum = obs_sum;
+            st->agc_obs_frame = obs_frame; st->agc_obs_utt = obs_utt;
+        }
+}
+
+// feat_lda_transform (lda.c:139-159): out[j] = sum over ascending k of x[k] * lda[j][k] in float32,
+// one thread per (frame, output row), the rows used in shared memory.  in [total][n] -> out [total][m].
+__global__ void __launch_bounds__(256)
+fe_lda_kernel(const float *__restrict__ in, const float *__restrict__ lda, float *__restrict__ out, int n, int m,
+              int32_t total)
+{
+    extern __shared__ float a_s[];                                       // [m][n]
+    for (int i = threadIdx.x; i < m * n; i += blockDim.x) a_s[i] = lda[i];
+    __syncthreads();
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (int64_t)total * m) return;
+    const float *x = in + (size_t)(i / m) * n, *a = a_s + (i % m) * n;
+    float acc = 0.f;
+    for (int k = 0; k < n; ++k) acc = __fadd_rn(acc, __fmul_rn(x[k], a[k]));
+    out[i] = acc;
+}
+
 static FeDev dev_fe(const psb_fe_t *fe)
 {
     FeDev p;
@@ -528,6 +663,7 @@ extern "C" void psb_fe_free(psb_fe_t *fe)
     cudaFree(fe->d_lifter); cudaFree(fe->d_rev); cudaFree(fe->d_mfspec); cudaFree(fe->d_mfcc); cudaFree(fe->d_pcm);
     cudaFree(fe->d_feats); cudaFree(fe->d_samp_off); cudaFree(fe->d_frame_off); cudaFree(fe->d_frame_utt);
     cudaFree(fe->d_state); cudaFree(fe->d_sess_off); cudaFree(fe->d_draw); cudaFree(fe->d_dpcm); cudaFree(fe->d_tail);
+    cudaFree(fe->d_lda); cudaFree(fe->d_raw);
     if (fe->ev[0]) cudaEventDestroy(fe->ev[0]);
     if (fe->ev[1]) cudaEventDestroy(fe->ev[1]);
     if (fe->stream) cudaStreamDestroy(fe->stream);
@@ -557,9 +693,20 @@ extern "C" int psb_fe_create_ex(const psb_fe_desc_t *d, const psb_fe_opts_t *o, 
                     "psb_fe_create_ex: feat must be 0 (1s_c_d_dd), 1 (s2_4x) or 2 (s3_1x39)");
         PSB_REQUIRE(o->feat == PSB_FEAT_1S_C_D_DD || d->n_cep == 13, "psb_fe_create_ex: s2_4x and s3_1x39 need n_cep 13 (got %d)", d->n_cep);
         PSB_REQUIRE(o->cmn >= PSB_CMN_NONE && o->cmn <= PSB_CMN_LIVE, "psb_fe_create_ex: cmn must be 0 (none), 1 (batch) or 2 (live)");
-        PSB_REQUIRE(!o->varnorm, o->cmn == PSB_CMN_LIVE ? "psb_fe_create_ex: variance normalization is not implemented in live mode"
-                                                        : "psb_fe_create_ex: variance normalization is not implemented");
+        PSB_REQUIRE(o->varnorm == 0 || o->varnorm == 1, "psb_fe_create_ex: varnorm must be 0 or 1");
+        PSB_REQUIRE(!o->varnorm || o->cmn == PSB_CMN_BATCH,
+                    o->cmn == PSB_CMN_LIVE ? "psb_fe_create_ex: variance normalization is not implemented in live mode"
+                                           : "psb_fe_create_ex: variance normalization needs batch CMN");
         PSB_REQUIRE(o->dither == 0 || o->dither == 1, "psb_fe_create_ex: dither must be 0 or 1");
+        PSB_REQUIRE(o->agc >= PSB_AGC_NONE && o->agc <= PSB_AGC_NOISE, "psb_fe_create_ex: agc must be 0 (none), 1 (max), 2 (emax) or 3 (noise)");
+        if (o->lda) {
+            const int dim = o->feat == PSB_FEAT_1S_C_D_DD ? 3 * d->n_cep : 39;
+            PSB_REQUIRE(o->feat != PSB_FEAT_S2_4X, "psb_fe_create_ex: LDA needs single-stream features; s2_4x has four streams");
+            PSB_REQUIRE(o->lda_cols == dim, "psb_fe_create_ex: the LDA matrix has %d columns, the features %d dimensions", o->lda_cols, dim);
+            PSB_REQUIRE(o->lda_rows > 0, "psb_fe_create_ex: the LDA matrix has %d rows", o->lda_rows);
+            const int m = o->ldadim > 0 && o->ldadim <= o->lda_rows ? o->ldadim : o->lda_rows;
+            PSB_REQUIRE(m <= dim, "psb_fe_create_ex: %d LDA outputs from %d-dimensional features", m, dim);
+        }
     }
     PSB_REQUIRE(d->hamming && d->ccc && d->sss && d->spec_start && d->filt_start && d->filt_width && d->filt_coeffs &&
                 d->mel_cosine && (d->lifter_val == 0 || d->lifter), "psb_fe_create: missing table");
@@ -581,8 +728,10 @@ extern "C" int psb_fe_create_ex(const psb_fe_desc_t *d, const psb_fe_opts_t *o, 
         fe->feat = o->feat; fe->cmn = o->cmn; fe->dither = o->dither; fe->seed = o->seed;
         fe->window = o->feat == PSB_FEAT_S2_4X ? 4 : 3;
         memcpy(fe->cmn_init, o->cmn_init, sizeof(fe->cmn_init));
+        fe->varnorm = o->varnorm; fe->agc = o->agc; fe->agc_thresh = o->agc_thresh;
     }
-    fe->feat_dim = fe->feat == PSB_FEAT_S2_4X ? 51 : 3 * fe->n_cep;
+    fe->stream_dim = fe->feat_dim = fe->feat == PSB_FEAT_S2_4X ? 51 : 3 * fe->n_cep;
+    if (o && o->lda) fe->feat_dim = o->ldadim > 0 && o->ldadim <= o->lda_rows ? o->ldadim : o->lda_rows;   // feat_read_lda
     fe->n_coeffs = n_coeffs; fe->alpha = d->pre_emphasis_alpha; fe->sqrt_inv_n = d->sqrt_inv_n; fe->sqrt_inv_2n = d->sqrt_inv_2n;
     std::vector<int> rev((size_t)d->fft_size);
     for (int i = 0; i < d->fft_size; ++i) {
@@ -600,6 +749,7 @@ extern "C" int psb_fe_create_ex(const psb_fe_desc_t *d, const psb_fe_opts_t *o, 
     if (!rc) rc = up(&fe->d_mel_cosine, d->mel_cosine, (size_t)d->n_cep * d->n_filt);
     if (!rc) rc = up(&fe->d_lifter, d->lifter, d->lifter_val ? (size_t)d->n_cep : 0);
     if (!rc) rc = up(&fe->d_rev, rev.data(), rev.size());
+    if (!rc && o && o->lda) rc = up(&fe->d_lda, o->lda, (size_t)fe->feat_dim * fe->stream_dim);
     cudaError_t e = cudaSuccess;
     if (!rc) {
         e = cudaStreamCreateWithFlags(&fe->stream, cudaStreamNonBlocking);
@@ -635,6 +785,7 @@ static void state_init(const psb_fe_t *fe, psb_fe_state_t *s)
     s->mt[0] = (uint32_t)fe->seed;
     for (int i = 1; i < 624; ++i) s->mt[i] = 1812433253u * (s->mt[i - 1] ^ (s->mt[i - 1] >> 30)) + (uint32_t)i;
     s->mt_index = 624;
+    s->agc_max = fe->cmn != PSB_CMN_NONE ? 5.f : 10.f;                 // feat_init's agc_emax_set (feat.c:879)
 }
 
 static int fe_run(psb_fe_t *fe, const int16_t *d_pcm, const int64_t *samp_off, int32_t n_utt, float *d_feats,
@@ -652,7 +803,7 @@ static int fe_run(psb_fe_t *fe, const int16_t *d_pcm, const int64_t *samp_off, i
         fe->states.clear();
     }
     const int32_t n_sess = (int32_t)fe->sess_off.size() - 1;
-    const bool live = fe->cmn == PSB_CMN_LIVE, stateful = live || fe->dither;
+    const bool live = fe->cmn == PSB_CMN_LIVE, emax = fe->agc == PSB_AGC_EMAX, stateful = live || fe->dither || emax;
     if (stateful && fe->states.empty()) {
         fe->states.resize((size_t)n_sess);
         for (auto &st : fe->states) state_init(fe, &st);
@@ -668,8 +819,9 @@ static int fe_run(psb_fe_t *fe, const int16_t *d_pcm, const int64_t *samp_off, i
     const int32_t total = foff[(size_t)n_utt];
     if (frame_off) memcpy(frame_off, foff.data(), foff.size() * sizeof(int32_t));
     if (ms) *ms = 0.f;
-    // live CMN updates its state even after an utterance without frames (cmn_live_update)
-    if (total == 0 && !(live && n_sess > 0)) return PSB_OK;
+    // live CMN and emax AGC update their state even after an utterance without frames (cmn_live_update,
+    // agc_emax_update)
+    if (total == 0 && !((live || emax) && n_sess > 0)) return PSB_OK;
     std::vector<int32_t> futt((size_t)total);
     for (int u = 0; u < n_utt; ++u)
         for (int32_t f = foff[(size_t)u]; f < foff[(size_t)u + 1]; ++f) futt[(size_t)f] = u;
@@ -683,6 +835,7 @@ static int fe_run(psb_fe_t *fe, const int16_t *d_pcm, const int64_t *samp_off, i
         PSB_CUDA(cudaMalloc((void **)&fe->d_frame_off, fe->utt_cap * 4));
     }
     if (!rc) rc = grow(&fe->d_frame_utt, &fe->fu_cap, (size_t)std::max(total, 1));
+    if (!rc && fe->d_lda && d_feats) rc = grow(&fe->d_raw, &fe->raw_cap, (size_t)std::max(total, 1) * fe->stream_dim);
     // dither: per utterance the first sample of its last frame, where its copy goes, and the draws
     // of fe_process_frames (every sample the full frames read) and of fe_end_utt (the last frame's)
     std::vector<int64_t> draw;
@@ -719,9 +872,9 @@ static int fe_run(psb_fe_t *fe, const int16_t *d_pcm, const int64_t *samp_off, i
     }
     const FeDev p = dev_fe(fe);
     const size_t smem = ((size_t)fe->fft_size + fe->fft_size / 2 + 1) * sizeof(double);
-    // the features of 1s_c_d_dd without live CMN come out of fe_utt_kernel; every other
+    // the features of 1s_c_d_dd without live CMN, AGC or LDA come out of fe_utt_kernel; every other
     // configuration normalises and builds them in the kernels behind it
-    const bool utt_feats = fe->feat == PSB_FEAT_1S_C_D_DD && !live;
+    const bool utt_feats = fe->feat == PSB_FEAT_1S_C_D_DD && !live && fe->agc == PSB_AGC_NONE && !fe->d_lda;
     PSB_CUDA(cudaEventRecord(fe->ev[0], fe->stream));
     if (fe->dither && n_sess) {
         fe_dither_kernel<<<(unsigned)n_sess, FE_DITHER_THREADS, 0, fe->stream>>>(d_pcm, fe->d_samp_off, fe->d_sess_off, fe->d_draw,
@@ -736,19 +889,44 @@ static int fe_run(psb_fe_t *fe, const int16_t *d_pcm, const int64_t *samp_off, i
             fe_frame_kernel<false><<<(unsigned)total, 128, smem, fe->stream>>>(p, d_pcm, fe->d_samp_off, fe->d_frame_off,
                                                                              fe->d_frame_utt, fe->d_mfspec, nullptr, nullptr);
         PSB_LAUNCH_CHECK();
-        fe_utt_kernel<<<(unsigned)n_utt, 64, 0, fe->stream>>>(p, fe->d_frame_off, fe->d_mfspec, fe->d_mfcc,
-                                                             utt_feats ? d_feats : nullptr, live ? 0 : fe->cmn, fe->window);
+        if (fe->varnorm)
+            fe_utt_kernel<true><<<(unsigned)n_utt, 64, 0, fe->stream>>>(p, fe->d_frame_off, fe->d_mfspec, fe->d_mfcc,
+                                                                       utt_feats ? d_feats : nullptr, fe->cmn, fe->window);
+        else
+            fe_utt_kernel<false><<<(unsigned)n_utt, 64, 0, fe->stream>>>(p, fe->d_frame_off, fe->d_mfspec, fe->d_mfcc,
+                                                                        utt_feats ? d_feats : nullptr, live ? 0 : fe->cmn, fe->window);
         PSB_LAUNCH_CHECK();
     }
     if (live) {
         fe_cmn_live_kernel<<<(unsigned)n_sess, 32, 0, fe->stream>>>(fe->d_sess_off, fe->d_frame_off, fe->d_mfcc, fe->n_cep, fe->d_state);
         PSB_LAUNCH_CHECK();
     }
+    if (fe->agc == PSB_AGC_MAX && total) {
+        fe_agc_kernel<PSB_AGC_MAX><<<(unsigned)n_utt, 32, 0, fe->stream>>>(nullptr, fe->d_frame_off, fe->d_mfcc, fe->n_cep, 0.f, nullptr);
+        PSB_LAUNCH_CHECK();
+    }
+    else if (fe->agc == PSB_AGC_NOISE && total) {
+        fe_agc_kernel<PSB_AGC_NOISE><<<(unsigned)n_utt, 32, 0, fe->stream>>>(nullptr, fe->d_frame_off, fe->d_mfcc, fe->n_cep,
+                                                                           fe->agc_thresh, nullptr);
+        PSB_LAUNCH_CHECK();
+    }
+    else if (emax && n_sess) {
+        fe_agc_kernel<PSB_AGC_EMAX><<<(unsigned)n_sess, 32, 0, fe->stream>>>(fe->d_sess_off, fe->d_frame_off, fe->d_mfcc, fe->n_cep,
+                                                                           0.f, fe->d_state);
+        PSB_LAUNCH_CHECK();
+    }
     if (!utt_feats && d_feats && total) {
         const int64_t work = (int64_t)total * fe->n_cep;
-        fe_feat_kernel<<<(unsigned)((work + 255) / 256), 256, 0, fe->stream>>>(fe->d_frame_off, fe->d_frame_utt, fe->d_mfcc, d_feats,
-                                                                           fe->n_cep, fe->feat, fe->feat_dim, total);
+        fe_feat_kernel<<<(unsigned)((work + 255) / 256), 256, 0, fe->stream>>>(fe->d_frame_off, fe->d_frame_utt, fe->d_mfcc,
+                                                                           fe->d_lda ? fe->d_raw : d_feats, fe->n_cep, fe->feat,
+                                                                           fe->stream_dim, total);
         PSB_LAUNCH_CHECK();
+        if (fe->d_lda) {
+            const int64_t outs = (int64_t)total * fe->feat_dim;
+            fe_lda_kernel<<<(unsigned)((outs + 255) / 256), 256, (size_t)fe->feat_dim * fe->stream_dim * sizeof(float), fe->stream>>>(
+                fe->d_raw, fe->d_lda, d_feats, fe->stream_dim, fe->feat_dim, total);
+            PSB_LAUNCH_CHECK();
+        }
     }
     PSB_CUDA(cudaEventRecord(fe->ev[1], fe->stream));
     if (d_mfcc_out && total)

@@ -12,12 +12,13 @@ import os
 
 import numpy as np
 
-from . import api, lextree
-from .fe_tables import CMN_TYPES, FEAT_TYPES, make_fe_desc, make_fe_opts
+from . import api, lextree, s3io
+from .fe_tables import AGC_TYPES, CMN_TYPES, FEAT_TYPES, make_fe_desc, make_fe_opts
 from .model import PackedModel
 
 # config_macro.h (the reference's defaults for every front-end / feature key this class looks at)
-FE_REFERENCE_DEFAULTS = dict(feat="1s_c_d_dd", cmn="live", agc="none", varnorm="no", lda="", svspec="", dither="no",
+FE_REFERENCE_DEFAULTS = dict(feat="1s_c_d_dd", cmn="live", agc="none", agcthresh="2.0", varnorm="no", lda="", ldadim="0",
+                             svspec="", dither="no",
                              round_filters="yes", ncep="13", frate="100", nfft="0", cmninit="40,3,-1", seed="-1", samprate="16000",
                              wlen="0.025625", nfilt="40", lowerf="133.33334", upperf="6855.4976", alpha="0.97",
                              transform="legacy", lifter="0", remove_noise="no", remove_dc="no", unit_area="yes", doublebw="no")
@@ -42,24 +43,38 @@ class Decoder:
         unsupported = []
         if fp["feat"] not in FEAT_TYPES: unsupported.append("-feat " + fp["feat"])
         if fp["cmn"] not in CMN_TYPES: unsupported.append("-cmn " + fp["cmn"])
-        if fp["agc"] != "none": unsupported.append("-agc " + fp["agc"])
-        if fp["varnorm"] in yes: unsupported.append("-varnorm yes")
-        if fp["lda"]: unsupported.append("-lda")
+        if fp["agc"] not in AGC_TYPES: unsupported.append("-agc " + fp["agc"])
+        if fp["varnorm"] in yes and CMN_TYPES.get(fp["cmn"]) != 1: unsupported.append("-varnorm yes with -cmn " + fp["cmn"])
         if fp["svspec"] not in ("", "0-12/13-25/26-38"): unsupported.append("-svspec " + fp["svspec"])
         if int(fp["ncep"]) != 13: unsupported.append("-ncep " + fp["ncep"])
         if int(fp["frate"]) != 100: unsupported.append("-frate " + fp["frate"])
         if int(fp["nfft"]) != 0: unsupported.append("-nfft " + fp["nfft"])
         if unsupported:
             raise NotImplementedError("front end settings the device front end does not implement: " + ", ".join(unsupported))
+        # -lda defaults to the model's feature_transform when there is one (ps_expand_model_config, pocketsphinx.c:119)
+        if not fp["lda"] and os.path.exists(os.path.join(hmm, "feature_transform")):
+            fp["lda"] = os.path.join(hmm, "feature_transform")
+        if fp["lda"] and fp["svspec"]:
+            # feat_dimension2 is the LDA output for every subvector, which no model's streams match (acmod_init fails)
+            raise ValueError("-lda %s with -svspec %s: the reference cannot load this model either" % (fp["lda"], fp["svspec"]))
+        lda = s3io.read_lda(fp["lda"])[0] if fp["lda"] else None
         opts = make_fe_opts(feat=fp["feat"], cmn=fp["cmn"], cmninit=fp["cmninit"], dither=fp["dither"] in yes,
-                            seed=int(fp["seed"]), ncep=int(fp["ncep"]))
+                            seed=int(fp["seed"]), ncep=int(fp["ncep"]), varnorm=fp["varnorm"] in yes, agc=fp["agc"],
+                            agcthresh=float(fp["agcthresh"]), lda=lda, ldadim=int(fp["ldadim"]))
         desc = make_fe_desc(samprate=float(fp["samprate"]), wlen=float(fp["wlen"]), nfilt=int(fp["nfilt"]),
                             lowerf=float(fp["lowerf"]), upperf=float(fp["upperf"]), alpha=float(fp["alpha"]),
                             transform=fp["transform"], lifter=int(fp["lifter"]), remove_noise=fp["remove_noise"] in yes,
                             remove_dc=fp["remove_dc"] in yes, unit_area=fp["unit_area"] in yes,
                             round_filters=fp["round_filters"] in yes, doublebw=fp["doublebw"] in yes)
-        # 1s_c_d_dd with batch CMN and no dither is the front end desc alone describes
-        plain = (opts["feat"], opts["cmn"], opts["dither"]) == (0, 1, 0)
+        # 1s_c_d_dd with batch CMN and nothing else is the front end desc alone describes
+        plain = (opts["feat"], opts["cmn"], opts["dither"], opts["varnorm"], opts["agc"], lda is None) == (0, 1, 0, 0, 0, True)
+        # the dimension psb_fe_feat_dim will report: feat_read_lda's out_dim, else the feature type's
+        dim = 51 if opts["feat"] == 1 else 3 * int(fp["ncep"])
+        if lda is not None:
+            dim = opts["ldadim"] if 0 < opts["ldadim"] <= lda.shape[0] else lda.shape[0]
+        if dim != self.pm.sumlen:
+            raise ValueError("the front end makes %d-dimensional features (-feat %s%s), the model in %s wants %d"
+                             % (dim, fp["feat"], ", -lda %s" % fp["lda"] if fp["lda"] else "", hmm, self.pm.sumlen))
         self.fe = api.FrontEnd(desc, device) if plain else api.FrontEnd(desc, device, opts)
         search_cfg = {k: v for k, v in cfg.items() if k in lextree.DEFAULTS}
         self.search = lextree.ngram_search_from_files(hmm, dict_file, lm_file, **search_cfg)

@@ -12,6 +12,7 @@ F32 = np.float32
 TRANSFORMS = {"legacy": 0, "dct": 1, "htk": 2}       # fe_internal.h: LEGACY_DCT, DCT_II, DCT_HTK
 CMN_TYPES = {"none": 0, "batch": 1, "current": 1, "live": 2}   # feat/cmn.h: CMN_NONE, CMN_BATCH, CMN_LIVE (cmn_type_str)
 FEAT_TYPES = {"1s_c_d_dd": 0, "s2_4x": 1, "s3_1x39": 2, "1s_12c_12d_3p_12dd": 2}   # psb200.h: PSB_FEAT_*
+AGC_TYPES = {"none": 0, "max": 1, "emax": 2, "noise": 3}          # feat/agc.h: agc_type_str, psb200.h: PSB_AGC_*
 
 
 def _mel(x):
@@ -111,17 +112,20 @@ def make_fe_desc(samprate=16000.0, frate=100, wlen=0.025625, nfft=0, nfilt=25, l
     return d
 
 
-def make_fe_opts(feat="1s_c_d_dd", cmn="live", cmninit="40,3,-1", varnorm=False, dither=False, seed=-1, ncep=13):
-    """psb_fe_opts_t from the feat.params / command-line keys -feat, -cmn, -cmninit, -varnorm, -dither and
-    -seed; the defaults are config_macro.h's.  cmn_init is what cmn_set_repr (cmn.c:119-146) parses out of
-    -cmninit: up to ncep comma-separated values, the rest 0."""
+def make_fe_opts(feat="1s_c_d_dd", cmn="live", cmninit="40,3,-1", varnorm=False, dither=False, seed=-1, ncep=13,
+                 agc="none", agcthresh=2.0, lda=None, ldadim=0):
+    """psb_fe_opts_t from the feat.params / command-line keys -feat, -cmn, -cmninit, -varnorm, -dither, -seed,
+    -agc, -agcthresh and -ldadim; the defaults are config_macro.h's.  cmn_init is what cmn_set_repr
+    (cmn.c:119-146) parses out of -cmninit: up to ncep comma-separated values, the rest 0.  lda: None or the
+    transform matrix [m][n] (s3io.read_lda(path)[0])."""
     init = np.zeros(32, np.float32)
     vals = cmninit.split(",") if cmninit else []
     for i, v in enumerate(vals[:ncep]):
         if v != "":
             init[i] = F32(float(v))
     return dict(feat=FEAT_TYPES[feat], cmn=CMN_TYPES[cmn], varnorm=int(bool(varnorm)), dither=int(bool(dither)),
-                seed=int(seed), cmn_init=init)
+                seed=int(seed), cmn_init=init, agc=AGC_TYPES[agc], agc_thresh=F32(agcthresh),
+                lda=None if lda is None else np.ascontiguousarray(lda, np.float32), ldadim=int(ldadim))
 
 
 def n_frames(desc, n_samples):

@@ -240,9 +240,9 @@ def write_model_dir(path, *, kind, n_mgau, n_feat, n_density, featlen, mean, var
 # tests/test_s3io_read.py compares every array with what the compiled reference holds after
 # acmod_init on its three shipped models (PTM en-us, semi-continuous tidigits, continuous an4).
 
-def _read_s3(path):
+def _read_s3(path, verify=True):
     """bio_readhdr + payload (bio.c:188-262): "s3\\n", "key value" lines up to "endhdr", the byte-order
-    word, data, and (chksum0 yes) the trailing checksum of bio_fread's rotate-and-add (:266-296)."""
+    word, data, and (chksum0 yes, verify) the trailing checksum of bio_fread's rotate-and-add (:266-296)."""
     with open(path, "rb") as f:
         raw = f.read()
     if not raw.startswith(b"s3\n"):
@@ -265,7 +265,7 @@ def _read_s3(path):
     else:
         raise ValueError("%s: bad byte-order word %#x" % (path, magic))
     body = raw[pos + 4:]
-    if hdr.get("chksum0", "no") == "yes":
+    if verify and hdr.get("chksum0", "no") == "yes":
         body, tail = body[:-4], body[-4:]
         data = body if order == "<" else np.frombuffer(body, ">u4").astype("<u4").tobytes()
         if _chksum_fast(data) != struct.unpack(order + "I", tail)[0]:
@@ -295,6 +295,27 @@ def read_tmat(path):
     if n_tmat <= 0 or n_tmat >= 32767 or n_dst != n_src + 1 or n != n_tmat * n_src * n_dst:
         raise ValueError("%s: unsupported transition matrices %d x %d x %d" % (path, n_tmat, n_src, n_dst))
     return np.frombuffer(b, o + "f4", n, 16).astype(np.float32).reshape(n_tmat, n_src, n_dst)
+
+
+def read_lda(path):
+    """feature_transform / -lda (feat_read_lda, lda.c:61-137): float32 [n_lda][m][n]; the front end uses [0],
+    eigenvectors in rows.  The reference computes the checksum but never compares it, so neither does this."""
+    hdr, b, o = _read_s3(path, verify=False)
+    if len(b) < 16:
+        raise ValueError("%s: truncated transform header" % path)
+    d1, d2, d3, n = struct.unpack_from(o + "4I", b, 0)
+    if n == 0 or n != d1 * d2 * d3 or len(b) < 16 + 4 * n:
+        raise ValueError("%s: bad transform dimensions %d x %d x %d (%d values, %d bytes of data)"
+                         % (path, d1, d2, d3, n, len(b) - 16))
+    return np.frombuffer(b, o + "f4", n, 16).astype(np.float32).reshape(d1, d2, d3)
+
+
+def write_lda(path, lda):
+    """A feature_transform file (bio_fwrite_3d with its checksum) of float32 [n_lda][m][n]."""
+    a = np.ascontiguousarray(lda, "<f4")
+    assert a.ndim == 3
+    payload = struct.pack("<4I", *a.shape, a.size) + a.tobytes()
+    _write_s3(path, [("version", "0.1"), ("chksum0", "yes")], payload)
 
 
 def read_mixw(path):
