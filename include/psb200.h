@@ -374,6 +374,32 @@ int psb_allphone_lm_batch_device(psb_hmmctx_t *c, const int16_t *d_senscr, const
                                  int32_t pbeam, int32_t n_ci, const int32_t *node_ci, const int32_t *bg,
                                  const int32_t *tg, int32_t *hist, int32_t cap_per_utt, int32_t *n_hist);
 
+/* Phone decoding over a PHMM net of any size, the context-dependent one (-allphone_ci no: one node per
+ * distinct (CI phone, tmat, senone sequence) of the mdef, 29 324 on en-us) included, for whole
+ * batches, with or without a phone LM.  The net is given in the reference's factored form, not as
+ * links: node i (in the order of ci_phmm[], ci-major, list order) = (ssid[i], tmatid[i], node_ci[i],
+ * lc[i], rc[i]), lc / rc the context bit vectors phmm_build fills (allphone_search.c:259-308; bit a
+ * of lc: CI phone a may precede the node; a filler context sets every filler's bit; CI nodes have
+ * all n_ci bits).  phmm_link's rule (:167-215) -- p links to p2 iff ci(p2) is in rc(p) and ci(p) in
+ * lc(p2) -- is applied on the device.  n_ci <= 64; no mask bit at or above n_ci.  start = the
+ * silence node allphone_search_start enters; beam / pbeam / inspen as allphone_search_init computes
+ * them (inspen is ignored with an LM).  bg / tg: NULL for the unconstrained loop, else the phone LM's
+ * tables as for psb_allphone_lm_batch_device.
+ * The history table stays on the device (cap_per_utt rows of 16 bytes per utterance; at most
+ * n_nodes entries per frame) and allphone_backtrace (:774-837) runs there.  Per utterance u:
+ * res[u] = {status, n_hist, n_seg}, status 0 = ok, 1 = the history outgrew cap_per_utt (the search
+ * of that utterance stopped; no segments; the other utterances are unaffected), 2 = more than
+ * seg_cap segments (the first seg_cap are returned; T segments always suffice for T frames);
+ * segs [n_utt][seg_cap][5] = (ci, sf, ef, score, tscore) in time order, as the reference's phseg_t
+ * list.  hist: NULL, or [n_utt][cap_per_utt][4] host rows {ef, node, predecessor entry, score}
+ * (for hosts that keep their own backtrace). */
+int psb_allphone_net_batch_device(psb_hmmctx_t *c, const int16_t *d_senscr, const int32_t *utt_off,
+                                  int32_t n_utt, int32_t n_nodes, const int32_t *ssid, const int32_t *tmatid,
+                                  const int32_t *node_ci, const uint64_t *lc, const uint64_t *rc, int32_t n_ci,
+                                  int32_t start, int32_t beam, int32_t pbeam, int32_t inspen, const int32_t *bg,
+                                  const int32_t *tg, int32_t cap_per_utt, int32_t *res, int32_t *segs,
+                                  int32_t seg_cap, int32_t *hist);
+
 /* ------------------------------------------------------------------------------------ */
 /* STATUS of the search entry points below (psb_fsg_batch_device, psb_ngram_*_batch_device): their phase
  * code reproduces the reference's tables in host emulation and is race-checked (tests/emul/), the kernels

@@ -420,6 +420,48 @@ class HmmContext:
               "psb_allphone_lm_batch_device")
         return [hist[u, :min(int(n_hist[u]), cap)].copy() for u in range(n_utt)], n_hist[:n_utt].copy()
 
+    def allphone_net(self, d_senscr_ptr, utt_off, net, beam, pbeam, inspen=0, bg=None, tg=None, cap=None,
+                     want_hist=False, hist_budget=4 << 30):
+        """allphone_search over a batch on a factored PHMM net (allphone_net.build_net: ssid, tmatid, ci,
+        lc, rc, n_ci, start), with a phone LM when bg / tg are given.  The history table stays on the
+        device; its backtrace runs there.  cap: history rows per utterance (default: frames x nodes,
+        which cannot overflow).  Utterances go to the device in sub-batches whose history tables fit
+        hist_budget bytes.  Returns a dict: status [n_utt] (0 ok, 1 history overflow), n_hist [n_utt],
+        segs (list of [n][5] = (ci, sf, ef, score, tscore)), hist (list of [n][4] rows, if want_hist)."""
+        utt_off = np.ascontiguousarray(utt_off, np.int32)
+        n_utt = len(utt_off) - 1
+        H = len(net["ci"])
+        a = [np.ascontiguousarray(net[k], np.int32) for k in ("ssid", "tmatid", "ci")]
+        lc, rc = (np.ascontiguousarray(net[k], np.uint64) for k in ("lc", "rc"))
+        if (bg is None) != (tg is None):
+            raise ValueError("give both phone-LM tables or neither")
+        bg = None if bg is None else np.ascontiguousarray(bg, np.int32)
+        tg = None if tg is None else np.ascontiguousarray(tg, np.int32)
+        lens = np.diff(utt_off)
+        cap = int(cap or max(1, int(lens.max(initial=1)) * H))
+        per = max(1, int(hist_budget) // (cap * 16))
+        out = dict(status=np.zeros(n_utt, np.int32), n_hist=np.zeros(n_utt, np.int32), segs=[], hist=[] if want_hist else None)
+        for u0 in range(0, max(n_utt, 1), per):
+            u1 = min(n_utt, u0 + per)
+            m = u1 - u0
+            sub = utt_off[u0:u1 + 1] - utt_off[u0]
+            seg_cap = max(1, int(np.diff(sub).max(initial=1)))          # a segment spans at least one frame
+            res = np.zeros((max(m, 1), 3), np.int32)
+            segs = np.zeros((max(m, 1), seg_cap, 5), np.int32)
+            hist = np.zeros((max(m, 1), cap, 4), np.int32) if want_hist else None
+            ptr = d_senscr_ptr + int(utt_off[u0]) * self.n_sen * 2 if m else d_senscr_ptr
+            check(lib().psb_allphone_net_batch_device(self.h, C.c_void_p(ptr), _p(sub), m, H, _p(a[0]), _p(a[1]), _p(a[2]),
+                                                      _p(lc), _p(rc), int(net["n_ci"]), int(net["start"]), int(beam), int(pbeam),
+                                                      int(inspen), _p(bg) if bg is not None else None,
+                                                      _p(tg) if tg is not None else None, cap, _p(res), _p(segs), seg_cap,
+                                                      _p(hist) if want_hist else None), "psb_allphone_net_batch_device")
+            for j in range(m):
+                out["status"][u0 + j], out["n_hist"][u0 + j] = res[j, 0], res[j, 1]
+                out["segs"].append(segs[j, :res[j, 2]].copy())
+                if want_hist:
+                    out["hist"].append(hist[j, :min(int(res[j, 1]), cap)].copy())
+        return out
+
     def kws(self, d_senscr_ptr, utt_off, pl_ssid, pl_tmat, kp_off, kp_thresh, kp_ssid, kp_tmat, beam, plp, cap=None):
         """kws_search over a batch (scores on the device).  Returns a list of raw hit arrays
         [n][5] = (frame, keyphrase, start frame, prob, ascr), one per utterance."""

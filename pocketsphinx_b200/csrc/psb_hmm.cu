@@ -2086,3 +2086,138 @@ extern "C" int psb_allphone_lm_batch_device(psb_hmmctx_t *c, const int16_t *d_se
                            cap_per_utt, n_hist, n_ci, node_ci, bg, tg);
 }
 
+// ---------------------------------------------------------------------------------------
+// Phone decoding over the factored PHMM net (-allphone_ci no, or yes), for whole batches.  The
+// phases and why they equal the reference's link walks are in psb_apn_core.h, which a host harness
+// (tests/emul/apn_emul.cpp) runs against the reference's golden results.  One CTA per utterance:
+// the node state (~48 B per node at 3 states, 1.4 MB for the en-us CD net) and the history table
+// live in global memory, the frame's n_ci x n_ci class table and the scalars in shared memory.
+#include "psb_apn_core.h"
+
+namespace {
+
+struct ApnDevEval {
+    HmmCtxDev c;
+    const uint16_t *senid_g;
+    const int32_t *tmatid_g;
+    const int16_t *row;
+    int H;
+    __device__ __forceinline__ int operator()(const ApnWork &W, int p) const
+    {
+        const HmmSoA<> V{W.score, W.hist, W.out_score, W.out_hist, W.best, H};
+        const int N = c.n_emit;
+        HmmReg h;
+        V.load(h, p, N, senid_g + (size_t)p * N, 1);
+        const int b = hmm_step(h, c, tmatid_g[p], false, row);
+        V.store(h, p, N);
+        return b;
+    }
+};
+
+constexpr int APN_THREADS = 512;
+
+__global__ void __launch_bounds__(APN_THREADS)
+allphone_net_kernel(const int16_t *__restrict__ senscr, const int32_t *__restrict__ utt_off, HmmCtxDev c, ApnNet G,
+                    const uint16_t *__restrict__ senid_g, const int32_t *__restrict__ tmatid_g, int32_t *work,
+                    size_t work_words, int32_t *hist_out, int cap, int32_t *res, int32_t *segs, int seg_cap)
+{
+    extern __shared__ int32_t apn_tab[];                     // msc | mix [n_ci * n_ci]
+    __shared__ ApnScalars S;
+    const int u = (int)blockIdx.x;
+    const long long f0 = utt_off[u];
+    const int T = utt_off[u + 1] - utt_off[u];
+    ApnWork W;
+    apn_work_carve(work + (size_t)u * work_words, G, W);
+    W.msc = apn_tab; W.mix = apn_tab + G.n_ci * G.n_ci;
+    W.hist_out = hist_out + (size_t)u * cap * APN_ROW;
+    W.cap = cap;
+    ApnDevEval ev{c, senid_g, tmatid_g, nullptr, G.H};
+    apn_start(G, W, &S);
+    for (int t = 0; t < T; ++t) {
+        if (S.overflow) break;                               // uniform: written before the last barrier of the step
+        ev.row = senscr + (f0 + t) * c.n_sen;
+        apn_step(G, W, &S, t, ev);
+    }
+    const bool ovf = S.overflow != 0;
+    const int ns = ovf ? 0 : apn_backtrace(G, W, &S, segs + (size_t)u * seg_cap * APN_SEG, seg_cap);
+    FSG_IF_LEADER {
+        res[u * 3 + 0] = ovf ? 1 : ns > seg_cap ? 2 : 0;
+        res[u * 3 + 1] = S.n_hist;
+        res[u * 3 + 2] = ns < seg_cap ? ns : seg_cap;
+    }
+}
+
+}  // namespace
+
+extern "C" int psb_allphone_net_batch_device(psb_hmmctx_t *c, const int16_t *d_senscr, const int32_t *utt_off,
+                                             int32_t n_utt, int32_t n_nodes, const int32_t *ssid, const int32_t *tmatid,
+                                             const int32_t *node_ci, const uint64_t *lc, const uint64_t *rc, int32_t n_ci,
+                                             int32_t start, int32_t beam, int32_t pbeam, int32_t inspen, const int32_t *bg,
+                                             const int32_t *tg, int32_t cap_per_utt, int32_t *res, int32_t *segs,
+                                             int32_t seg_cap, int32_t *hist)
+{
+    static const char *fn = "psb_allphone_net_batch_device";
+    PSB_REQUIRE(c && utt_off && n_utt >= 0 && n_nodes > 0 && ssid && tmatid && node_ci && lc && rc && res && segs &&
+                cap_per_utt > 0 && seg_cap > 0, "%s: bad argument", fn);
+    PSB_REQUIRE(n_ci > 0 && n_ci <= 64, "%s: %d CI phones; the context sets are 64-bit masks (at most 64)", fn, n_ci);
+    PSB_REQUIRE(start >= 0 && start < n_nodes, "%s: start node %d out of range", fn, start);
+    PSB_REQUIRE((bg == nullptr) == (tg == nullptr), "%s: give both phone-LM tables or neither", fn);
+    const uint64_t outside = n_ci == 64 ? 0 : ~((1ull << n_ci) - 1);
+    for (int i = 0; i < n_nodes; ++i) {
+        PSB_REQUIRE(node_ci[i] >= 0 && node_ci[i] < n_ci, "%s: node_ci[%d] = %d out of range", fn, i, node_ci[i]);
+        PSB_REQUIRE(!(lc[i] & outside) && !(rc[i] & outside), "%s: node %d has a context bit at or above n_ci = %d", fn, i, n_ci);
+    }
+    if (n_utt == 0) return PSB_OK;
+    int rc_ = ctx_check_utts(fn, utt_off, n_utt, d_senscr);
+    if (rc_) return rc_;
+    const int N = c->n_emit, H = n_nodes;
+    std::vector<uint16_t> senid((size_t)H * N);
+    rc_ = ctx_senids(c, fn, H, ssid, tmatid, senid.data(), N, 1);
+    if (rc_) return rc_;
+    PSB_CUDA(cudaSetDevice(c->device));
+    // one int32 block: utt_off | tmatid[H] | node_ci[H] | res[n_utt][3] | bg | tg; the masks apart
+    std::vector<int32_t> ibuf(utt_off, utt_off + n_utt + 1);
+    const size_t o_tm = ibuf.size();
+    ibuf.insert(ibuf.end(), tmatid, tmatid + H);
+    const size_t o_ci = ibuf.size();
+    ibuf.insert(ibuf.end(), node_ci, node_ci + H);
+    const size_t o_res = ibuf.size();
+    ibuf.resize(o_res + (size_t)n_utt * 3, 0);
+    const size_t o_bg = ibuf.size();
+    if (bg) ibuf.insert(ibuf.end(), bg, bg + (size_t)n_ci * n_ci);
+    const size_t o_tg = ibuf.size();
+    if (tg) ibuf.insert(ibuf.end(), tg, tg + (size_t)n_ci * n_ci * n_ci);
+    std::vector<uint64_t> masks(lc, lc + H);
+    masks.insert(masks.end(), rc, rc + H);
+    const size_t work_words = apn_work_words(H, N);
+    const size_t hist_n = (size_t)n_utt * cap_per_utt * APN_ROW, seg_n = (size_t)n_utt * seg_cap * APN_SEG;
+    int32_t *d_i = nullptr, *d_hist = nullptr, *d_work = nullptr, *d_segs = nullptr;
+    uint16_t *d_senid = nullptr;
+    uint64_t *d_masks = nullptr;
+    cudaError_t e = srch_reserve(c, 0, ibuf.size(), &d_i);
+    if (e == cudaSuccess) e = srch_reserve(c, 1, hist_n, &d_hist);
+    if (e == cudaSuccess) e = srch_reserve(c, 2, senid.size(), &d_senid);
+    if (e == cudaSuccess) e = srch_reserve(c, 3, work_words * (size_t)n_utt, &d_work);
+    if (e == cudaSuccess) e = srch_reserve(c, 4, masks.size(), &d_masks);
+    if (e == cudaSuccess) e = srch_reserve(c, 5, seg_n, &d_segs);
+    cudaStream_t st = c->stream;
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_i, ibuf.data(), ibuf.size() * 4, cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_senid, senid.data(), senid.size() * 2, cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_masks, masks.data(), masks.size() * 8, cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess) {
+        ApnNet G;
+        memset(&G, 0, sizeof(G));
+        G.H = H; G.n_ci = n_ci; G.n_emit = N; G.start = start;
+        G.beam = beam; G.pbeam = pbeam; G.inspen = bg ? 0 : inspen;
+        G.ci = d_i + o_ci;
+        G.lc = (const unsigned long long *)d_masks; G.rc = (const unsigned long long *)d_masks + H;
+        G.bg = bg ? d_i + o_bg : nullptr; G.tg = tg ? d_i + o_tg : nullptr;
+        const size_t smem = 2 * (size_t)n_ci * n_ci * sizeof(int32_t);
+        allphone_net_kernel<<<(unsigned)n_utt, APN_THREADS, smem, st>>>(d_senscr, d_i, dev_ctx(c), G, d_senid, d_i + o_tm, d_work,
+                                                                        work_words, d_hist, cap_per_utt, d_i + o_res, d_segs,
+                                                                        seg_cap);
+    }
+    return ctx_finish(c, fn, e, 1, {{res, d_i + o_res, (size_t)n_utt * 3 * 4}, {segs, d_segs, seg_n * 4},
+                                    {hist, d_hist, hist ? hist_n * 4 : 0}});
+}
+

@@ -393,7 +393,8 @@ def read_mdef(path):
     file with the reference's pocketsphinx_mdef_convert).  Returns a dict: n_ciphone, n_phone,
     n_emit_state, n_ci_sen, n_sen, n_tmat, ciname, sseq [n_sseq][n_emit], phone_ssid, phone_tmat,
     phone_filler, sen2cimap, cd_tree (the triphone lookup tree: ctx, n_down, down / pid; None for a CI-only
-    text file), sil (the id of SIL or -1)."""
+    text file), sil (the id of SIL or -1), phone_ctx [n_phone][4] (a CD phone's info bytes wpos, base, left
+    and right context; (-1, ci, -1, -1) for a CI phone)."""
     with open(path, "rb") as f:
         raw = f.read()
     if raw[:4] in (b"BMDF", b"FDMB"):
@@ -424,6 +425,9 @@ def read_mdef(path):
         filler = ent["info"][:n_ci, 0].astype(np.uint8)
         # CD phones: info = {wpos, ctx[3]} with ctx[0] the base phone (bin_mdef.h:86-89)
         base = np.concatenate([np.arange(n_ci), ent["info"][n_ci:, 1].astype(np.int64)])
+        ctx = np.full((n_phone, 4), -1, np.int32)
+        ctx[:, 1] = base
+        ctx[n_ci:] = ent["info"][n_ci:].astype(np.int32)
     else:
         lines = [l.strip() for l in raw.decode("latin-1").split("\n")]
         lines = [l for l in lines if l and not l.startswith("#")]
@@ -451,6 +455,8 @@ def read_mdef(path):
         sseq = np.array(list(uniq), np.uint16).reshape(len(uniq), n_emit)
         ssid, tmat, filler = np.array(ssid, np.int32), np.array(tmat, np.int32), np.array(filler, np.uint8)
         n_phone, base = n_ci, np.arange(n_ci)
+        ctx = np.full((n_ci, 4), -1, np.int32)
+        ctx[:, 1] = base
         cd_tree = None
     if sseq.size and int(sseq.max()) >= n_sen:
         raise ValueError("%s: senone id out of range" % path)
@@ -461,7 +467,7 @@ def read_mdef(path):
         sen2ci[sseq[ssid[i]]] = base[i]
     return dict(n_ciphone=n_ci, n_phone=n_phone, n_emit_state=n_emit, n_ci_sen=n_ci_sen, n_sen=n_sen, n_tmat=n_tmat,
                 ciname=names, sseq=sseq, phone_ssid=ssid, phone_tmat=tmat, phone_filler=filler, sen2cimap=sen2ci,
-                cd_tree=cd_tree, sil=names.index("SIL") if "SIL" in names else -1)
+                cd_tree=cd_tree, sil=names.index("SIL") if "SIL" in names else -1, phone_ctx=ctx)
 
 
 def read_feat_params(path):
