@@ -28,7 +28,7 @@ typedef enum psb_status_e {
     PSB_OK = 0,
     PSB_ERR_ARG = -1,        /* bad argument / unsupported shape */
     PSB_ERR_CUDA = -2,       /* CUDA runtime error (message in psb_last_error) */
-    PSB_ERR_NOMEM = -3,
+    PSB_ERR_NOMEM = -3,      /* a device or pinned host allocation failed; the handle stays usable */
     PSB_ERR_STATE = -4       /* call not valid in the handle's current state */
 } psb_status_t;
 
@@ -689,6 +689,8 @@ int psb_vad_process_device(psb_vad_t *v, const int16_t *d_pcm, const int64_t *sa
 
 /* number of kernels launched by this library in the calling process so far */
 int64_t psb_kernel_launch_count(void);
+/* bytes of device and pinned host memory this library holds now, over all handles */
+int64_t psb_device_bytes_live(void);
 
 #ifdef __cplusplus
 }

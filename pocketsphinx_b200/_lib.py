@@ -161,6 +161,7 @@ SYMBOLS = [
     ("psb_vad_process_host", C.c_int, [_VP, _VP, _VP, _I32, _VP, _VP, _VP, _VP, _VP]),
     ("psb_vad_process_device", C.c_int, [_VP, _VP, _VP, _I32, _VP, _VP, _VP, _VP, _VP, C.POINTER(C.c_float)]),
     ("psb_kernel_launch_count", _I64, []),
+    ("psb_device_bytes_live", _I64, []),
 ]
 
 _lib = None

@@ -9,6 +9,7 @@
 #include <vector>
 
 std::atomic<long long> g_psb_launches{0};
+std::atomic<long long> g_psb_bytes_live{0};
 
 static thread_local char g_err[512] = "";
 
@@ -23,6 +24,7 @@ void psb_set_error(const char *fmt, ...)
 extern "C" const char *psb_last_error(void) { return g_err; }
 extern "C" int psb_abi_version(void) { return PSB_ABI_VERSION; }
 extern "C" int64_t psb_kernel_launch_count(void) { return g_psb_launches.load(); }
+extern "C" int64_t psb_device_bytes_live(void) { return g_psb_bytes_live.load(); }
 
 extern "C" int psb_device_count(void)
 {
@@ -37,11 +39,13 @@ extern "C" int psb_device_count(void)
 // ---------------------------------------------------------------------------------------
 // model
 
-static int upload(void **dst, const void *src, size_t bytes, bool src_on_device)
+template <class T>
+static int upload(DevBuf<T> &dst, const void *src, size_t n, bool src_on_device)
 {
-    PSB_CUDA(cudaMalloc(dst, bytes ? bytes : 1));
-    if (bytes)
-        PSB_CUDA(cudaMemcpy(*dst, src, bytes, src_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
+    const int rc = dst.reserve(n ? n : 1);
+    if (rc) return rc;
+    if (n)
+        PSB_CUDA(cudaMemcpy(dst, src, n * sizeof(T), src_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
     return PSB_OK;
 }
 
@@ -77,10 +81,10 @@ static int build_records(psb_model_t *m, const float *mean, const float *var, co
                 }
             }
         }
-    if (!m->d_rec) {
-        PSB_CUDA(cudaMalloc(&m->d_rec, total * sizeof(float)));
-        PSB_CUDA(cudaMalloc(&m->d_rec_off, m->K * sizeof(size_t)));
-        PSB_CUDA(cudaMemcpy(m->d_rec_off, m->rec_off.data(), m->K * sizeof(size_t), cudaMemcpyHostToDevice));
+    if (!m->d_rec_off) {
+        int rc = m->d_rec.reserve(total);
+        if (!rc) rc = upload(m->d_rec_off, m->rec_off.data(), m->K, false);
+        if (rc) return rc;
     }
     PSB_CUDA(cudaMemcpy(m->d_rec, rec.data(), total * sizeof(float), cudaMemcpyHostToDevice));
     if (m->kind != PSB_KIND_MS && m->n_density % 2 == 0 && !m->fixed_point) {
@@ -108,10 +112,10 @@ static int build_records(psb_model_t *m, const float *mean, const float *var, co
                     }
                 }
             }
-        if (!m->d_rec2) {
-            PSB_CUDA(cudaMalloc(&m->d_rec2, total2 * sizeof(float)));
-            PSB_CUDA(cudaMalloc(&m->d_rec2_off, m->K * sizeof(size_t)));
-            PSB_CUDA(cudaMemcpy(m->d_rec2_off, off2.data(), m->K * sizeof(size_t), cudaMemcpyHostToDevice));
+        if (!m->d_rec2_off) {
+            int rc = m->d_rec2.reserve(total2);
+            if (!rc) rc = upload(m->d_rec2_off, off2.data(), m->K, false);
+            if (rc) return rc;
         }
         PSB_CUDA(cudaMemcpy(m->d_rec2, rec2.data(), total2 * sizeof(float), cudaMemcpyHostToDevice));
     }
@@ -136,10 +140,9 @@ static int build_records(psb_model_t *m, const float *mean, const float *var, co
                     }
                 }
             }
-        if (!m->d_msT) {
-            PSB_CUDA(cudaMalloc(&m->d_msT, gT.size() * sizeof(float)));
-            PSB_CUDA(cudaMalloc(&m->d_msdetT, dT.size() * sizeof(float)));
-        }
+        int rc = m->d_msT.reserve(gT.size());
+        if (!rc) rc = m->d_msdetT.reserve(dT.size());
+        if (rc) return rc;
         PSB_CUDA(cudaMemcpy(m->d_msT, gT.data(), gT.size() * sizeof(float), cudaMemcpyHostToDevice));
         PSB_CUDA(cudaMemcpy(m->d_msdetT, dT.data(), dT.size() * sizeof(float), cudaMemcpyHostToDevice));
     }
@@ -155,7 +158,8 @@ extern "C" int psb_model_create(const psb_model_desc_t *d, int device, psb_model
     PSB_REQUIRE(d->topn >= 1 && d->topn <= PSB_MAX_TOPN, "topn %d out of range", d->topn);
     PSB_REQUIRE(d->mean && d->var && d->det && d->mixw && d->sen2cb, "missing model array");
     PSB_CUDA(cudaSetDevice(device));
-    psb_model_t *m = new psb_model_t();
+    PSB_REQUIRE(!(d->fixed_point && d->kind == PSB_KIND_MS), "fixed-point arithmetic is implemented for ptm and semi-continuous models only");
+    std::unique_ptr<psb_model_t> m(new psb_model_t());
     m->device = device;
     m->kind = d->kind; m->n_sen = d->n_sen; m->n_mgau = d->n_mgau; m->n_feat = d->n_feat;
     m->n_density = d->n_density; m->topn = d->topn;
@@ -170,42 +174,25 @@ extern "C" int psb_model_create(const psb_model_desc_t *d, int device, psb_model
     m->K = m->n_mgau * m->n_feat;
     m->mixw_4bit = d->mixw_cb != nullptr;
     m->fixed_point = d->fixed_point != 0;
-    if (m->fixed_point && d->kind == PSB_KIND_MS) {
-        psb_set_error("fixed-point arithmetic is implemented for ptm and semi-continuous models only");
-        delete m;
-        return PSB_ERR_ARG;
-    }
     m->logadd_ms_size = d->logadd_ms_size;
     m->logadd_ms_zero = d->logadd_ms_zero;
-    m->d_rec = nullptr; m->d_rec_off = nullptr; m->d_rec2 = nullptr; m->d_rec2_off = nullptr; m->d_mixw = nullptr; m->d_mixw_cb = nullptr;
-    m->d_sen2cb = nullptr; m->d_sen2cb32 = nullptr; m->d_quadcb = nullptr; m->d_bsen = nullptr; m->n_bsen = 0; m->d_logadd8 = nullptr; m->d_logadd_ms = nullptr;
-    m->has_topn_beam = false;
-    m->d_topn_beam = nullptr;
-    m->tc_ok = false;
-    m->d_tc_wumma = m->d_tc_cen = m->d_tc_bnd = nullptr;
-    m->d_msT = m->d_msdetT = nullptr; m->d_featlen = m->d_featoff = nullptr;
-    for (int f = 0; f < PSB_MAX_FEAT; ++f) m->topn_beam[f] = 0;
     const bool dev = d->on_device != 0;
-    int rc = build_records(m, d->mean, d->var, d->det, dev);
-    if (!rc) rc = upload((void **)&m->d_featlen, m->featlen, sizeof(m->featlen), false);
-    if (!rc) rc = upload((void **)&m->d_featoff, m->featoff, sizeof(m->featoff), false);
-    if (rc) { psb_model_free(m); return rc; }
+    const cudaMemcpyKind to_dev = dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+    int rc = build_records(m.get(), d->mean, d->var, d->det, dev);
+    if (!rc) rc = upload(m->d_featlen, m->featlen, PSB_MAX_FEAT, false);
+    if (!rc) rc = upload(m->d_featoff, m->featoff, PSB_MAX_FEAT, false);
+    if (rc) return rc;
 
     // senone -> codebook map
     std::vector<int32_t> s2c(m->n_sen);
     if (cudaMemcpy(s2c.data(), d->sen2cb, m->n_sen * sizeof(int32_t),
                    dev ? cudaMemcpyDeviceToHost : cudaMemcpyHostToHost) != cudaSuccess) {
         psb_set_error("copying sen2cb failed");
-        psb_model_free(m);
         return PSB_ERR_CUDA;
     }
     std::vector<uint16_t> s2c16(m->n_sen);
     for (int i = 0; i < m->n_sen; ++i) {
-        if (s2c[i] < 0 || s2c[i] >= m->n_mgau) {
-            psb_set_error("sen2cb[%d] = %d out of range", i, s2c[i]);
-            psb_model_free(m);
-            return PSB_ERR_ARG;
-        }
+        PSB_REQUIRE(s2c[i] >= 0 && s2c[i] < m->n_mgau, "sen2cb[%d] = %d out of range", i, s2c[i]);
         s2c16[i] = (uint16_t)s2c[i];
     }
     {
@@ -220,86 +207,67 @@ extern "C" int psb_model_create(const psb_model_desc_t *d, int device, psb_model
             else for (int i = 0; i < 4 && s0 + i < m->n_sen; ++i) bsen.push_back(s0 + i);
         }
         m->n_bsen = (int)bsen.size();
-        if ((rc = upload((void **)&m->d_quadcb, quadcb.data(), nq * sizeof(int16_t), false)) ||
-            (rc = upload((void **)&m->d_bsen, bsen.data(), bsen.size() * sizeof(int32_t), false))) {
-            psb_model_free(m);
+        if ((rc = upload(m->d_quadcb, quadcb.data(), nq, false)) || (rc = upload(m->d_bsen, bsen.data(), bsen.size(), false)))
             return rc;
-        }
     }
     m->sen_is_cb = m->n_mgau == m->n_sen;
     for (int i = 0; m->sen_is_cb && i < m->n_sen; ++i) m->sen_is_cb = s2c[i] == i;
-    if ((rc = upload((void **)&m->d_sen2cb, s2c16.data(), m->n_sen * sizeof(uint16_t), false)) ||
-        (rc = upload((void **)&m->d_sen2cb32, s2c.data(), m->n_sen * sizeof(int32_t), false))) {
-        psb_model_free(m);
+    if ((rc = upload(m->d_sen2cb, s2c16.data(), m->n_sen, false)) || (rc = upload(m->d_sen2cb32, s2c.data(), m->n_sen, false)))
         return rc;
-    }
 
     // mixture weights
     if (m->kind == PSB_KIND_MS) {
         m->mixw_row = m->n_sen;
         m->mixw_stride = m->n_sen;
-        rc = upload((void **)&m->d_mixw, d->mixw, (size_t)m->n_sen * m->n_feat * m->n_density, dev);
+        rc = upload(m->d_mixw, d->mixw, (size_t)m->n_sen * m->n_feat * m->n_density, dev);
     }
     else {
         m->mixw_row = m->mixw_4bit ? (m->n_sen + 1) / 2 : m->n_sen;
         m->mixw_stride = roundup(m->mixw_row, 128);
         const size_t rows = (size_t)m->n_feat * m->n_density;
-        rc = upload((void **)&m->d_mixw, nullptr, 0, false);
-        if (!rc) {
-            cudaFree(m->d_mixw);
-            m->d_mixw = nullptr;
-            if (cudaMalloc(&m->d_mixw, rows * m->mixw_stride) != cudaSuccess ||
-                cudaMemset(m->d_mixw, 0, rows * m->mixw_stride) != cudaSuccess ||
-                cudaMemcpy2D(m->d_mixw, m->mixw_stride, d->mixw, m->mixw_row, m->mixw_row, rows,
-                             dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice) != cudaSuccess) {
-                psb_set_error("uploading mixture weights failed: %s", cudaGetErrorString(cudaGetLastError()));
-                rc = PSB_ERR_CUDA;
-            }
+        rc = m->d_mixw.reserve(rows * m->mixw_stride);
+        if (!rc && (cudaMemset(m->d_mixw, 0, rows * m->mixw_stride) != cudaSuccess ||
+                    cudaMemcpy2D(m->d_mixw, m->mixw_stride, d->mixw, m->mixw_row, m->mixw_row, rows, to_dev) != cudaSuccess)) {
+            psb_set_error("uploading mixture weights failed: %s", cudaGetErrorString(cudaGetLastError()));
+            rc = PSB_ERR_CUDA;
         }
     }
-    if (!rc && m->mixw_4bit) rc = upload((void **)&m->d_mixw_cb, d->mixw_cb, 16, dev);
+    if (!rc && m->mixw_4bit) rc = upload(m->d_mixw_cb, d->mixw_cb, 16, dev);
     if (!rc && d->logadd8) {
         // 256 entries from the caller (logmath.c:116-120), continued with zeros: see logadd8()
-        if (cudaMalloc((void **)&m->d_logadd8, PSB_LOGADD8_N) != cudaSuccess ||
-            cudaMemset(m->d_logadd8, 0, PSB_LOGADD8_N) != cudaSuccess ||
-            cudaMemcpy(m->d_logadd8, d->logadd8, 256, dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice) != cudaSuccess) {
+        rc = m->d_logadd8.reserve(PSB_LOGADD8_N);
+        if (!rc && (cudaMemset(m->d_logadd8, 0, PSB_LOGADD8_N) != cudaSuccess ||
+                    cudaMemcpy(m->d_logadd8, d->logadd8, 256, to_dev) != cudaSuccess)) {
             psb_set_error("uploading the log-add table failed: %s", cudaGetErrorString(cudaGetLastError()));
             rc = PSB_ERR_CUDA;
         }
-        else {
+        else if (!rc) {
             uint8_t t[256];
             if (cudaMemcpy(t, m->d_logadd8, 256, cudaMemcpyDeviceToHost) == cudaSuccess)
                 for (int i = 0; i < 256; ++i) m->logadd8_max = std::max<int>(m->logadd8_max, t[i]);
         }
     }
-    if (!rc && m->kind != PSB_KIND_MS && !d->logadd8) {
-        psb_set_error("logadd8 table required for ptm/semi models");
-        rc = PSB_ERR_ARG;
+    if (rc) return rc;
+    PSB_REQUIRE(m->kind == PSB_KIND_MS || d->logadd8, "logadd8 table required for ptm/semi models");
+    if (m->kind == PSB_KIND_MS) {
+        PSB_REQUIRE(d->logadd_ms && d->logadd_ms_size > 0, "logadd_ms table required for ms models");
+        rc = upload(m->d_logadd_ms, d->logadd_ms, (size_t)d->logadd_ms_size, dev);
+        if (rc) return rc;
     }
-    if (!rc && m->kind == PSB_KIND_MS) {
-        if (!d->logadd_ms || d->logadd_ms_size <= 0) {
-            psb_set_error("logadd_ms table required for ms models");
-            rc = PSB_ERR_ARG;
-        }
-        else
-            rc = upload((void **)&m->d_logadd_ms, d->logadd_ms, (size_t)d->logadd_ms_size * sizeof(uint32_t), dev);
-    }
-    if (!rc && d->topn_beam) {
+    if (d->topn_beam) {
         uint8_t tb[PSB_MAX_FEAT] = {0};
         if (cudaMemcpy(tb, d->topn_beam, m->n_feat, dev ? cudaMemcpyDeviceToHost : cudaMemcpyHostToHost) != cudaSuccess)
-            rc = PSB_ERR_CUDA;
+            return PSB_ERR_CUDA;
         for (int f = 0; f < m->n_feat; ++f) {
             m->topn_beam[f] = tb[f];
             if (tb[f]) m->has_topn_beam = true;
         }
     }
-    if (!rc) {
-        int32_t tb[PSB_MAX_FEAT] = {0};
-        for (int f = 0; f < m->n_feat; ++f) tb[f] = m->has_topn_beam ? m->topn_beam[f] : 0;
-        rc = upload((void **)&m->d_topn_beam, tb, sizeof(tb), false);
-    }
-    if (rc) { psb_model_free(m); return rc; }
-    *out = m;
+    int32_t tb[PSB_MAX_FEAT] = {0};
+    for (int f = 0; f < m->n_feat; ++f) tb[f] = m->has_topn_beam ? m->topn_beam[f] : 0;
+    rc = upload(m->d_topn_beam, tb, PSB_MAX_FEAT, false);
+    if (rc) return rc;
+    *out = m.release();
     return PSB_OK;
 }
 
@@ -307,10 +275,6 @@ extern "C" void psb_model_free(psb_model_t *m)
 {
     if (!m) return;
     cudaSetDevice(m->device);
-    cudaFree(m->d_rec); cudaFree(m->d_rec_off); cudaFree(m->d_rec2); cudaFree(m->d_rec2_off); cudaFree(m->d_mixw); cudaFree(m->d_mixw_cb);
-    cudaFree(m->d_sen2cb); cudaFree(m->d_sen2cb32); cudaFree(m->d_quadcb); cudaFree(m->d_bsen); cudaFree(m->d_logadd8); cudaFree(m->d_logadd_ms);
-    cudaFree(m->d_topn_beam); cudaFree(m->d_msT); cudaFree(m->d_msdetT); cudaFree(m->d_featlen); cudaFree(m->d_featoff);
-    cudaFree(m->d_tc_wumma); cudaFree(m->d_tc_cen); cudaFree(m->d_tc_bnd);
     delete m;
 }
 
@@ -338,7 +302,7 @@ extern "C" int psb_batch_create(psb_model_t *m, int32_t max_utts, int64_t max_fr
                 "psb_batch_create: PSB_TOPN_VARIANT=%s; accepted values are 0, 2, 3, 4, 5 and 6 (default)", v);
     PSB_REQUIRE(!impl || !strcmp(impl, "wgmma"), "psb_batch_create: PSB_TC_IMPL=%s; the only accepted value is wgmma", impl);
     PSB_CUDA(cudaSetDevice(m->device));
-    psb_batch_t *b = new psb_batch_t();      // value-initialised: all pointers null, counters zero
+    std::unique_ptr<psb_batch_t> b(new psb_batch_t());
     b->m = m;
     b->max_utts = max_utts;
     b->max_frames = max_frames;
@@ -351,21 +315,21 @@ extern "C" int psb_batch_create(psb_model_t *m, int32_t max_utts, int64_t max_fr
         if (b->n_pipe < 0) b->n_pipe = 0;
         if (b->n_pipe > 8) b->n_pipe = 8;
     }
-    cudaError_t e = cudaStreamCreateWithFlags(&b->stream, cudaStreamNonBlocking);
-    if (e == cudaSuccess) e = cudaMalloc(&b->d_feats, (size_t)max_frames * m->sumlen * sizeof(float));
-    if (e == cudaSuccess) e = cudaMalloc(&b->d_senscr, (size_t)max_frames * m->n_sen * sizeof(int16_t));
-    if (e == cudaSuccess && m->kind != PSB_KIND_MS) e = cudaMalloc(&b->d_topn, (size_t)max_frames * m->K * sizeof(int4));
-    for (int i = 0; i < 4 && e == cudaSuccess; ++i) e = cudaEventCreate(&b->ev[i]);
-    for (int i = 0; i < 2 && e == cudaSuccess; ++i) e = cudaEventCreate(&b->tev[i]);
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&b->fork_ev, cudaEventDisableTiming);
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&b->join_ev, cudaEventDisableTiming);
+    cudaError_t e = b->stream.create();
+    for (int i = 0; i < 4 && e == cudaSuccess; ++i) e = b->ev[i].create();
+    for (int i = 0; i < 2 && e == cudaSuccess; ++i) e = b->tev[i].create();
+    if (e == cudaSuccess) e = b->fork_ev.create(cudaEventDisableTiming);
+    if (e == cudaSuccess) e = b->join_ev.create(cudaEventDisableTiming);
     if (e != cudaSuccess) {
         psb_set_error("psb_batch_create: %s", cudaGetErrorString(e));
-        psb_batch_free(b);
-        return e == cudaErrorMemoryAllocation ? PSB_ERR_NOMEM : PSB_ERR_CUDA;
+        return PSB_ERR_CUDA;
     }
-    b->have_ev = true;
-    *out = b;
+    int rc = b->d_feats.reserve((size_t)max_frames * m->sumlen);
+    if (!rc) rc = b->d_senscr.reserve((size_t)max_frames * m->n_sen);
+    if (!rc && m->kind != PSB_KIND_MS) rc = b->topn.reserve((size_t)max_frames * m->K);
+    if (rc) return rc;
+    b->d_topn = b->topn;
+    *out = b.release();
     return PSB_OK;
 }
 
@@ -373,31 +337,8 @@ extern "C" void psb_batch_free(psb_batch_t *b)
 {
     if (!b) return;
     cudaSetDevice(b->m->device);
-    if (b->stream) cudaStreamSynchronize(b->stream);
-    for (psb_batch_t *k : b->kids) {            // sub-batches own only their stream, tables, featT, events
-        cudaStreamSynchronize(k->stream);
-        if (k->h_off) cudaFreeHost(k->h_off);
-        cudaFree(k->d_featT); cudaFree(k->d_tab); cudaFree(k->d_off); cudaFree(k->d_msdist); cudaFree(k->d_msbest);
-        cudaFree(k->d_uttoff); cudaFree(k->d_semi_dist); cudaFree(k->d_tc_flags); cudaFree(k->d_tc_check); cudaFree(k->d_tc_items); cudaFree(k->d_tc_nitems);
-        if (k->h_tab) cudaFreeHost(k->h_tab);
-        for (int i = 0; i < 4; ++i) cudaEventDestroy(k->ev[i]);
-        cudaEventDestroy(k->join_ev);
-        cudaStreamDestroy(k->stream);
-        delete k;
-    }
-    if (b->fork_ev) cudaEventDestroy(b->fork_ev);
-    if (b->join_ev) cudaEventDestroy(b->join_ev);
-    cudaFree(b->d_feats); cudaFree(b->d_senscr); cudaFree(b->d_featT); cudaFree(b->d_topn); cudaFree(b->d_tab); cudaFree(b->d_semi_dist); cudaFree(b->d_uttoff);
-    cudaFree(b->d_best); cudaFree(b->d_pen); cudaFree(b->d_off); cudaFree(b->d_msdist); cudaFree(b->d_msbest);
-    cudaFree(b->d_tc_flags); cudaFree(b->d_tc_check); cudaFree(b->d_tc_items); cudaFree(b->d_tc_nitems);
-    if (b->h_tab) cudaFreeHost(b->h_tab);
-    if (b->h_feats) cudaFreeHost(b->h_feats);
-    if (b->h_senscr) cudaFreeHost(b->h_senscr);
-    if (b->h_best) cudaFreeHost(b->h_best);
-    if (b->h_pen) cudaFreeHost(b->h_pen);
-    if (b->have_ev) for (int i = 0; i < 4; ++i) cudaEventDestroy(b->ev[i]);
-    if (b->have_ev) for (int i = 0; i < 2; ++i) cudaEventDestroy(b->tev[i]);
-    if (b->stream) cudaStreamDestroy(b->stream);
+    cudaStreamSynchronize(b->stream);
+    for (auto &k : b->kids) cudaStreamSynchronize(k->stream);
     delete b;
 }
 
@@ -464,7 +405,7 @@ extern "C" int psb_batch_sync(psb_batch_t *b)
     return PSB_OK;
 }
 
-extern "C" int16_t *psb_batch_senscr_device(psb_batch_t *b) { return b ? b->d_senscr : nullptr; }
+extern "C" int16_t *psb_batch_senscr_device(psb_batch_t *b) { return b ? b->d_senscr.get() : nullptr; }
 
 extern "C" int psb_batch_last_kernel_ms(psb_batch_t *b, float *out3)
 {
@@ -476,7 +417,7 @@ extern "C" int psb_batch_last_kernel_ms(psb_batch_t *b, float *out3)
         // pipelined decode: sum of the sub-batches' own kernel intervals (they overlap in time)
         for (int q = 0; q < b->last_kids && q < (int)b->kids.size(); ++q)
             for (int i = 0; i < 3; ++i) {
-                psb_batch_t *k = b->kids[q];
+                const psb_batch_t *k = b->kids[q].get();
                 float ms = 0.f;
                 if (cudaEventElapsedTime(&ms, k->ev[i], k->ev[i + 1]) == cudaSuccess) out3[i] += ms;
                 else cudaGetLastError();
@@ -504,21 +445,19 @@ cudaStream_t psb_batch_stream(psb_batch_t *b) { return b->stream; }
 static int get_kid(psb_batch_t *b, int i, psb_batch_t **out)
 {
     while ((int)b->kids.size() <= i) {
-        psb_batch_t *k = new psb_batch_t();
+        std::unique_ptr<psb_batch_t> k(new psb_batch_t());
         k->m = b->m; k->max_utts = b->max_utts; k->max_frames = b->max_frames; k->topn_variant = b->topn_variant;
-        k->is_kid = true; k->n_pipe = 1;
-        cudaError_t e = cudaStreamCreateWithFlags(&k->stream, cudaStreamNonBlocking);
-        for (int j = 0; j < 4 && e == cudaSuccess; ++j) e = cudaEventCreate(&k->ev[j]);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&k->join_ev, cudaEventDisableTiming);
+        k->n_pipe = 1;
+        cudaError_t e = k->stream.create();
+        for (int j = 0; j < 4 && e == cudaSuccess; ++j) e = k->ev[j].create();
+        if (e == cudaSuccess) e = k->join_ev.create(cudaEventDisableTiming);
         if (e != cudaSuccess) {
             psb_set_error("pipelined decode: %s", cudaGetErrorString(e));
-            delete k;
             return PSB_ERR_CUDA;
         }
-        k->have_ev = true;
-        b->kids.push_back(k);
+        b->kids.push_back(std::move(k));
     }
-    *out = b->kids[i];
+    *out = b->kids[i].get();
     return PSB_OK;
 }
 
@@ -540,7 +479,7 @@ static int decode_common(psb_batch_t *b, psb_phoneloop_t *p, const float *feats,
 {
     const int rc = decode_common_body(b, p, feats, feats_on_host, utt_off, n_utt, h_best, h_pen, h_senscr, want_best, want_pen);
     if (rc != PSB_OK) {
-        for (psb_batch_t *k : b->kids) cudaStreamSynchronize(k->stream);
+        for (auto &k : b->kids) cudaStreamSynchronize(k->stream);
         cudaStreamSynchronize(b->stream);
     }
     return rc;
@@ -553,13 +492,9 @@ static int decode_common_body(psb_batch_t *b, psb_phoneloop_t *p, const float *f
     psb_model_t *m = b->m;
     const size_t H = psb_phoneloop_n_phones(p);
     const long long total = utt_off[n_utt];
-    if ((size_t)b->max_frames * H > b->pen_cap) {
-        cudaFree(b->d_best); cudaFree(b->d_pen);
-        b->d_best = b->d_pen = nullptr;
-        b->pen_cap = (size_t)b->max_frames * H;
-        PSB_CUDA(cudaMalloc(&b->d_best, (size_t)b->max_frames * 4));
-        PSB_CUDA(cudaMalloc(&b->d_pen, b->pen_cap * 4));
-    }
+    int rc = b->d_best.reserve((size_t)b->max_frames);
+    if (!rc) rc = b->d_pen.reserve((size_t)b->max_frames * H);
+    if (rc) return rc;
     // auto: two ranges when the features come from the host (the copies of one overlap the
     // kernels of the other), one when they are resident (two concurrent top-N kernels only add
     // launch and tail overhead; PSB_PIPELINE overrides)
@@ -575,19 +510,12 @@ static int decode_common_body(psb_batch_t *b, psb_phoneloop_t *p, const float *f
         if (s == S - 1) u1 = n_utt;
         if (u1 == u0) continue;
         psb_batch_t *k;
-        int rc = get_kid(b, s, &k);
+        rc = get_kid(b, s, &k);
         if (rc) return rc;
         const long long f0 = utt_off[u0], nf = utt_off[u1] - f0;
         const int nu = u1 - u0;
-        if ((size_t)nu + 1 > k->off_cap) {
-            cudaFree(k->d_off);
-            if (k->h_off) cudaFreeHost(k->h_off);
-            k->d_off = nullptr; k->h_off = nullptr;
-            k->off_cap = (size_t)nu + 1 + 256;
-            PSB_CUDA(cudaMalloc(&k->d_off, k->off_cap * 4));
-            PSB_CUDA(cudaMallocHost(&k->h_off, k->off_cap * 4));
-        }
         PSB_CUDA(cudaStreamSynchronize(k->stream));          // the previous call's copy from h_off is done
+        if ((rc = k->d_off.reserve((size_t)nu + 1, 256)) || (rc = k->h_off.reserve((size_t)nu + 1, 256))) return rc;
         int32_t *off = k->h_off;
         for (int i = 0; i <= nu; ++i) off[i] = utt_off[u0 + i] - (int32_t)f0;
         PSB_CUDA(cudaStreamWaitEvent(k->stream, b->fork_ev, 0));
@@ -598,7 +526,7 @@ static int decode_common_body(psb_batch_t *b, psb_phoneloop_t *p, const float *f
             d_f = b->d_feats + f0 * m->sumlen;
         }
         PSB_CUDA(cudaMemcpyAsync(k->d_off, off, (size_t)(nu + 1) * 4, cudaMemcpyHostToDevice, k->stream));
-        k->d_topn = b->d_topn ? b->d_topn + f0 * m->K : nullptr;
+        k->d_topn = b->topn ? b->topn + f0 * m->K : nullptr;
         rc = score_dispatch(k, d_f, off, nu, b->d_senscr + f0 * m->n_sen);
         if (rc) return rc;
         rc = psb_phoneloop_launch(p, b->d_senscr + f0 * m->n_sen, k->d_off, nu, want_best ? b->d_best + f0 : nullptr,

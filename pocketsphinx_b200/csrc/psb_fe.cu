@@ -33,33 +33,33 @@ struct psb_fe_s {
     int frame_size, frame_shift, fft_size, fft_order, n_filt, n_cep;
     int remove_dc, remove_noise, transform, lifter_val, window, cmn, n_coeffs;
     float alpha, sqrt_inv_n, sqrt_inv_2n;
-    double *d_hamming, *d_ccc, *d_sss;
-    int16_t *d_spec_start, *d_filt_start, *d_filt_width;
-    float *d_filt_coeffs, *d_mel_cosine, *d_lifter;
-    int *d_rev;                   // bit-reversal permutation [fft_size]
-    cudaStream_t stream;
-    cudaEvent_t ev[2];
+    Stream stream;                // declared first: destroyed after the buffers below
+    Event ev[2];
+    DevBuf<double> d_hamming, d_ccc, d_sss;
+    DevBuf<int16_t> d_spec_start, d_filt_start, d_filt_width;
+    DevBuf<float> d_filt_coeffs, d_mel_cosine, d_lifter;
+    DevBuf<int> d_rev;            // bit-reversal permutation [fft_size]
     // workspace
-    double *d_mfspec; size_t mfspec_cap;      // [frames][n_filt]
-    float *d_mfcc; size_t mfcc_cap;           // [frames][n_cep]
-    int16_t *d_pcm; size_t pcm_cap;
-    float *d_feats; size_t feats_cap;
-    int64_t *d_samp_off; int32_t *d_frame_off; int32_t *d_frame_utt; size_t utt_cap, fu_cap;
+    DevBuf<double> d_mfspec;      // [frames][n_filt]
+    DevBuf<float> d_mfcc;         // [frames][n_cep]
+    DevBuf<int16_t> d_pcm;
+    DevBuf<float> d_feats;
+    DevBuf<int64_t> d_samp_off; DevBuf<int32_t> d_frame_off, d_frame_utt;
     // psb_fe_create_ex options and sessions
     int feat, feat_dim, dither, seed;
     int varnorm, agc, stream_dim;             // stream_dim: the features' dimension before LDA
     float agc_thresh;
-    float *d_lda;                             // [feat_dim][stream_dim], NULL without LDA
-    float *d_raw; size_t raw_cap;             // [frames][stream_dim]: the features LDA reads
+    DevBuf<float> d_lda;                      // [feat_dim][stream_dim], NULL without LDA
+    DevBuf<float> d_raw;                      // [frames][stream_dim]: the features LDA reads
     float cmn_init[PSB_FE_MAX_CEP];
     std::vector<int32_t> sess_off;            // set by psb_fe_set_sessions for the next call only
     std::vector<psb_fe_state_t> states;       // in: the next call's sessions; out: after it
     bool sess_pending;
-    psb_fe_state_t *d_state; size_t state_cap;
-    int32_t *d_sess_off; size_t sess_cap;
-    int64_t *d_draw; size_t draw_cap;         // per utterance: first tail sample, tail offset, main draws, tail draws
-    int16_t *d_dpcm; size_t dpcm_cap;         // dithered samples of the full frames
-    int16_t *d_tail; size_t tail_cap;         // freshly dithered samples of each utterance's last frame
+    DevBuf<psb_fe_state_t> d_state;
+    DevBuf<int32_t> d_sess_off;
+    DevBuf<int64_t> d_draw;                   // per utterance: first tail sample, tail offset, main draws, tail draws
+    DevBuf<int16_t> d_dpcm;                   // dithered samples of the full frames
+    DevBuf<int16_t> d_tail;                   // freshly dithered samples of each utterance's last frame
 };
 
 namespace {
@@ -633,22 +633,19 @@ static FeDev dev_fe(const psb_fe_t *fe)
 }
 
 template <typename T>
-static int up(T **dst, const T *src, size_t n)
+static int up(DevBuf<T> &dst, const T *src, size_t n)
 {
-    PSB_CUDA(cudaMalloc((void **)dst, std::max<size_t>(n, 1) * sizeof(T)));
-    if (n) PSB_CUDA(cudaMemcpy(*dst, src, n * sizeof(T), cudaMemcpyHostToDevice));
+    const int rc = dst.reserve(std::max<size_t>(n, 1));
+    if (rc) return rc;
+    if (n) PSB_CUDA(cudaMemcpy(dst, src, n * sizeof(T), cudaMemcpyHostToDevice));
     return PSB_OK;
 }
 
+// the workspace's growth rule
 template <typename T>
-static int grow(T **p, size_t *cap, size_t need)
+static int grow(DevBuf<T> &b, size_t need)
 {
-    if (need <= *cap) return PSB_OK;
-    if (*p) cudaFree(*p);
-    *p = nullptr;
-    *cap = need + need / 8 + 64;
-    PSB_CUDA(cudaMalloc((void **)p, *cap * sizeof(T)));
-    return PSB_OK;
+    return b.reserve(need, need / 8 + 64);
 }
 
 }  // namespace
@@ -658,15 +655,6 @@ extern "C" void psb_fe_free(psb_fe_t *fe)
     if (!fe) return;
     cudaSetDevice(fe->device);
     if (fe->stream) cudaStreamSynchronize(fe->stream);
-    cudaFree(fe->d_hamming); cudaFree(fe->d_ccc); cudaFree(fe->d_sss); cudaFree(fe->d_spec_start);
-    cudaFree(fe->d_filt_start); cudaFree(fe->d_filt_width); cudaFree(fe->d_filt_coeffs); cudaFree(fe->d_mel_cosine);
-    cudaFree(fe->d_lifter); cudaFree(fe->d_rev); cudaFree(fe->d_mfspec); cudaFree(fe->d_mfcc); cudaFree(fe->d_pcm);
-    cudaFree(fe->d_feats); cudaFree(fe->d_samp_off); cudaFree(fe->d_frame_off); cudaFree(fe->d_frame_utt);
-    cudaFree(fe->d_state); cudaFree(fe->d_sess_off); cudaFree(fe->d_draw); cudaFree(fe->d_dpcm); cudaFree(fe->d_tail);
-    cudaFree(fe->d_lda); cudaFree(fe->d_raw);
-    if (fe->ev[0]) cudaEventDestroy(fe->ev[0]);
-    if (fe->ev[1]) cudaEventDestroy(fe->ev[1]);
-    if (fe->stream) cudaStreamDestroy(fe->stream);
     delete fe;
 }
 
@@ -718,7 +706,7 @@ extern "C" int psb_fe_create_ex(const psb_fe_desc_t *d, const psb_fe_opts_t *o, 
     }
     PSB_REQUIRE(n_coeffs == d->n_coeffs, "psb_fe_create: n_coeffs %d != sum of filter widths %d", d->n_coeffs, n_coeffs);
     PSB_CUDA(cudaSetDevice(device));
-    psb_fe_t *fe = new psb_fe_t();
+    std::unique_ptr<psb_fe_t> fe(new psb_fe_t());
     fe->device = device;
     fe->frame_size = d->frame_size; fe->frame_shift = d->frame_shift; fe->fft_size = d->fft_size; fe->fft_order = d->fft_order;
     fe->n_filt = d->n_filt; fe->n_cep = d->n_cep; fe->remove_dc = d->remove_dc; fe->remove_noise = d->remove_noise;
@@ -739,29 +727,26 @@ extern "C" int psb_fe_create_ex(const psb_fe_desc_t *d, const psb_fe_opts_t *o, 
         for (int b = 0; b < d->fft_order; ++b) r |= ((i >> b) & 1) << (d->fft_order - 1 - b);
         rev[(size_t)i] = r;
     }
-    int rc = up(&fe->d_hamming, d->hamming, (size_t)d->frame_size / 2);
-    if (!rc) rc = up(&fe->d_ccc, d->ccc, (size_t)d->fft_size / 4);
-    if (!rc) rc = up(&fe->d_sss, d->sss, (size_t)d->fft_size / 4);
-    if (!rc) rc = up(&fe->d_spec_start, d->spec_start, (size_t)d->n_filt);
-    if (!rc) rc = up(&fe->d_filt_start, d->filt_start, (size_t)d->n_filt);
-    if (!rc) rc = up(&fe->d_filt_width, d->filt_width, (size_t)d->n_filt);
-    if (!rc) rc = up(&fe->d_filt_coeffs, d->filt_coeffs, (size_t)n_coeffs);
-    if (!rc) rc = up(&fe->d_mel_cosine, d->mel_cosine, (size_t)d->n_cep * d->n_filt);
-    if (!rc) rc = up(&fe->d_lifter, d->lifter, d->lifter_val ? (size_t)d->n_cep : 0);
-    if (!rc) rc = up(&fe->d_rev, rev.data(), rev.size());
-    if (!rc && o && o->lda) rc = up(&fe->d_lda, o->lda, (size_t)fe->feat_dim * fe->stream_dim);
-    cudaError_t e = cudaSuccess;
-    if (!rc) {
-        e = cudaStreamCreateWithFlags(&fe->stream, cudaStreamNonBlocking);
-        if (e == cudaSuccess) e = cudaEventCreate(&fe->ev[0]);
-        if (e == cudaSuccess) e = cudaEventCreate(&fe->ev[1]);
+    int rc = up(fe->d_hamming, d->hamming, (size_t)d->frame_size / 2);
+    if (!rc) rc = up(fe->d_ccc, d->ccc, (size_t)d->fft_size / 4);
+    if (!rc) rc = up(fe->d_sss, d->sss, (size_t)d->fft_size / 4);
+    if (!rc) rc = up(fe->d_spec_start, d->spec_start, (size_t)d->n_filt);
+    if (!rc) rc = up(fe->d_filt_start, d->filt_start, (size_t)d->n_filt);
+    if (!rc) rc = up(fe->d_filt_width, d->filt_width, (size_t)d->n_filt);
+    if (!rc) rc = up(fe->d_filt_coeffs, d->filt_coeffs, (size_t)n_coeffs);
+    if (!rc) rc = up(fe->d_mel_cosine, d->mel_cosine, (size_t)d->n_cep * d->n_filt);
+    if (!rc) rc = up(fe->d_lifter, d->lifter, d->lifter_val ? (size_t)d->n_cep : 0);
+    if (!rc) rc = up(fe->d_rev, rev.data(), rev.size());
+    if (!rc && o && o->lda) rc = up(fe->d_lda, o->lda, (size_t)fe->feat_dim * fe->stream_dim);
+    if (rc) return rc;
+    cudaError_t e = fe->stream.create();
+    if (e == cudaSuccess) e = fe->ev[0].create();
+    if (e == cudaSuccess) e = fe->ev[1].create();
+    if (e != cudaSuccess) {
+        psb_set_error("psb_fe_create: %s", cudaGetErrorString(e));
+        return PSB_ERR_CUDA;
     }
-    if (rc || e != cudaSuccess) {
-        if (!rc) psb_set_error("psb_fe_create: %s", cudaGetErrorString(e));
-        psb_fe_free(fe);
-        return rc ? rc : PSB_ERR_CUDA;
-    }
-    *out = fe;
+    *out = fe.release();
     return PSB_OK;
 }
 
@@ -825,17 +810,12 @@ static int fe_run(psb_fe_t *fe, const int16_t *d_pcm, const int64_t *samp_off, i
     std::vector<int32_t> futt((size_t)total);
     for (int u = 0; u < n_utt; ++u)
         for (int32_t f = foff[(size_t)u]; f < foff[(size_t)u + 1]; ++f) futt[(size_t)f] = u;
-    int rc = grow(&fe->d_mfspec, &fe->mfspec_cap, (size_t)total * fe->n_filt);
-    if (!rc) rc = grow(&fe->d_mfcc, &fe->mfcc_cap, (size_t)total * fe->n_cep);
-    if (!rc && (size_t)n_utt + 1 > fe->utt_cap) {
-        cudaFree(fe->d_samp_off); cudaFree(fe->d_frame_off);
-        fe->d_samp_off = nullptr; fe->d_frame_off = nullptr;
-        fe->utt_cap = (size_t)n_utt + 1 + 64;
-        PSB_CUDA(cudaMalloc((void **)&fe->d_samp_off, fe->utt_cap * 8));
-        PSB_CUDA(cudaMalloc((void **)&fe->d_frame_off, fe->utt_cap * 4));
-    }
-    if (!rc) rc = grow(&fe->d_frame_utt, &fe->fu_cap, (size_t)std::max(total, 1));
-    if (!rc && fe->d_lda && d_feats) rc = grow(&fe->d_raw, &fe->raw_cap, (size_t)std::max(total, 1) * fe->stream_dim);
+    int rc = grow(fe->d_mfspec, (size_t)total * fe->n_filt);
+    if (!rc) rc = grow(fe->d_mfcc, (size_t)total * fe->n_cep);
+    if (!rc) rc = fe->d_samp_off.reserve((size_t)n_utt + 1, 64);
+    if (!rc) rc = fe->d_frame_off.reserve((size_t)n_utt + 1, 64);
+    if (!rc) rc = grow(fe->d_frame_utt, (size_t)std::max(total, 1));
+    if (!rc && fe->d_lda && d_feats) rc = grow(fe->d_raw, (size_t)std::max(total, 1) * fe->stream_dim);
     // dither: per utterance the first sample of its last frame, where its copy goes, and the draws
     // of fe_process_frames (every sample the full frames read) and of fe_end_utt (the last frame's)
     std::vector<int64_t> draw;
@@ -853,13 +833,13 @@ static int fe_run(psb_fe_t *fe, const int16_t *d_pcm, const int64_t *samp_off, i
             draw[4 * (size_t)u + 3] = n > 0 ? n - t0 : 0;
             n_tail += draw[4 * (size_t)u + 3];
         }
-        if (!rc) rc = grow(&fe->d_draw, &fe->draw_cap, draw.size() + 1);
-        if (!rc) rc = grow(&fe->d_dpcm, &fe->dpcm_cap, (size_t)std::max<int64_t>(samp_off[n_utt], 1));
-        if (!rc) rc = grow(&fe->d_tail, &fe->tail_cap, (size_t)std::max<int64_t>(n_tail, 1));
+        if (!rc) rc = grow(fe->d_draw, draw.size() + 1);
+        if (!rc) rc = grow(fe->d_dpcm, (size_t)std::max<int64_t>(samp_off[n_utt], 1));
+        if (!rc) rc = grow(fe->d_tail, (size_t)std::max<int64_t>(n_tail, 1));
     }
     if (stateful) {
-        if (!rc) rc = grow(&fe->d_state, &fe->state_cap, (size_t)n_sess);
-        if (!rc) rc = grow(&fe->d_sess_off, &fe->sess_cap, (size_t)n_sess + 1);
+        if (!rc) rc = grow(fe->d_state, (size_t)n_sess);
+        if (!rc) rc = grow(fe->d_sess_off, (size_t)n_sess + 1);
     }
     if (rc) return rc;
     PSB_CUDA(cudaMemcpyAsync(fe->d_samp_off, samp_off, ((size_t)n_utt + 1) * 8, cudaMemcpyHostToDevice, fe->stream));
@@ -957,8 +937,8 @@ extern "C" int psb_fe_process_host(psb_fe_t *fe, const int16_t *pcm, const int64
     PSB_REQUIRE(ns == 0 || pcm, "psb_fe_process_host: pcm is null");
     int64_t total = 0;
     for (int u = 0; u < n_utt; ++u) total += psb_fe_n_frames(fe, samp_off[u + 1] - samp_off[u]);
-    int rc = grow(&fe->d_pcm, &fe->pcm_cap, (size_t)std::max<int64_t>(ns, 1));
-    if (!rc) rc = grow(&fe->d_feats, &fe->feats_cap, (size_t)std::max<int64_t>(total, 1) * fe->feat_dim);
+    int rc = grow(fe->d_pcm, (size_t)std::max<int64_t>(ns, 1));
+    if (!rc) rc = grow(fe->d_feats, (size_t)std::max<int64_t>(total, 1) * fe->feat_dim);
     if (rc) return rc;
     if (ns) PSB_CUDA(cudaMemcpyAsync(fe->d_pcm, pcm, (size_t)ns * 2, cudaMemcpyHostToDevice, fe->stream));
     rc = fe_run(fe, fe->d_pcm, samp_off, n_utt, fe->d_feats, nullptr, frame_off, nullptr);
@@ -970,7 +950,7 @@ extern "C" int psb_fe_process_host(psb_fe_t *fe, const int16_t *pcm, const int64
 
 extern "C" const float *psb_fe_device_feats(const psb_fe_t *fe)
 {
-    return fe ? fe->d_feats : nullptr;
+    return fe ? fe->d_feats.get() : nullptr;
 }
 
 extern "C" int32_t psb_fe_feat_dim(const psb_fe_t *fe)

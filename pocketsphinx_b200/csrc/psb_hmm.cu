@@ -13,10 +13,10 @@ struct psb_phoneloop_s {
     psb_hmmctx_t *c;
     int n_phones, window, beam, pbeam, pip;
     double penalty_weight;
-    int32_t *d_ssid, *d_tmatid;
-    uint16_t *d_senid;            // [n_emit][n_phones]
-    cudaStream_t stream;
-    int32_t *d_flags;             // [1] pathological-regime counter
+    Stream stream;                // declared first: destroyed after the buffers below
+    DevBuf<int32_t> d_ssid, d_tmatid;
+    DevBuf<uint16_t> d_senid;     // [n_emit][n_phones]
+    DevBuf<int32_t> d_flags;      // [1] pathological-regime counter
 };
 
 namespace {
@@ -247,28 +247,27 @@ extern "C" int psb_hmmctx_create(int32_t n_emit_state, const uint8_t *tp, int32_
     PSB_REQUIRE(out && tp && n_emit_state >= 1 && n_emit_state <= PSB_HMM_MAX_NSTATE && n_tmat > 0 && n_sen > 0,
                 "psb_hmmctx_create: bad argument");
     PSB_CUDA(cudaSetDevice(device));
-    psb_hmmctx_t *c = new psb_hmmctx_t();
-    memset(c, 0, sizeof(*c));
+    std::unique_ptr<psb_hmmctx_t> c(new psb_hmmctx_t());
     c->device = device; c->n_emit = n_emit_state; c->n_tmat = n_tmat; c->n_sseq = n_sseq; c->n_sen = n_sen;
     size_t tpb = (size_t)n_tmat * n_emit_state * (n_emit_state + 1);
-    const size_t sseq_bytes = std::max<size_t>(2, (size_t)n_sseq * n_emit_state * 2);
-    cudaError_t e = cudaMalloc(&c->d_tp, tpb);
-    if (e == cudaSuccess) e = cudaMemcpy(c->d_tp, tp, tpb, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMalloc(&c->d_sseq, sseq_bytes);
-    if (e == cudaSuccess && !(c->h_sseq = (uint16_t *)calloc(sseq_bytes, 1))) e = cudaErrorMemoryAllocation;
-    if (e == cudaSuccess && n_sseq > 0 && sseq) memcpy(c->h_sseq, sseq, (size_t)n_sseq * n_emit_state * 2);
-    if (e == cudaSuccess) e = cudaMemcpy(c->d_sseq, c->h_sseq, sseq_bytes, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking);
-    if (e == cudaSuccess) e = cudaMalloc(&c->d_senscr, (size_t)n_sen * 2);
-    if (e == cudaSuccess) e = cudaMallocHost(&c->h_senscr, (size_t)n_sen * 2);
-    if (e == cudaSuccess) e = cudaMalloc(&c->d_best, 4);
-    if (e == cudaSuccess) e = cudaMallocHost(&c->h_best, 4);
+    const size_t n_sseq_el = std::max<size_t>(1, (size_t)n_sseq * n_emit_state);
+    c->h_sseq.assign(n_sseq_el, 0);
+    if (n_sseq > 0 && sseq) memcpy(c->h_sseq.data(), sseq, (size_t)n_sseq * n_emit_state * 2);
+    int rc = c->d_tp.reserve(tpb);
+    if (!rc) rc = c->d_sseq.reserve(n_sseq_el);
+    if (!rc) rc = c->d_senscr.reserve((size_t)n_sen);
+    if (!rc) rc = c->h_senscr.reserve((size_t)n_sen);
+    if (!rc) rc = c->d_best.reserve(1);
+    if (!rc) rc = c->h_best.reserve(1);
+    if (rc) return rc;
+    cudaError_t e = cudaMemcpy(c->d_tp, tp, tpb, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(c->d_sseq, c->h_sseq.data(), n_sseq_el * 2, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = c->stream.create();
     if (e != cudaSuccess) {
         psb_set_error("psb_hmmctx_create: %s", cudaGetErrorString(e));
-        psb_hmmctx_free(c);
         return PSB_ERR_CUDA;
     }
-    *out = c;
+    *out = c.release();
     return PSB_OK;
 }
 
@@ -276,16 +275,7 @@ extern "C" void psb_hmmctx_free(psb_hmmctx_t *c)
 {
     if (!c) return;
     cudaSetDevice(c->device);
-    if (c->stream) cudaStreamSynchronize(c->stream);
-    cudaFree(c->d_tp); cudaFree(c->d_sseq); cudaFree(c->d_hmms); cudaFree(c->d_senscr); cudaFree(c->d_best);
-    free(c->h_sseq);
-    for (void *p : c->d_srch) cudaFree(p);
-    if (c->al_ev[0]) cudaEventDestroy(c->al_ev[0]);
-    if (c->al_ev[1]) cudaEventDestroy(c->al_ev[1]);
-    if (c->h_hmms) cudaFreeHost(c->h_hmms);
-    if (c->h_senscr) cudaFreeHost(c->h_senscr);
-    if (c->h_best) cudaFreeHost(c->h_best);
-    if (c->stream) cudaStreamDestroy(c->stream);
+    cudaStreamSynchronize(c->stream);
     delete c;
 }
 
@@ -306,14 +296,8 @@ static int validate_hmm(const psb_hmmctx_t *c, const psb_hmm_t *h, int i)
 
 static int ensure_hmm_cap(psb_hmmctx_t *c, size_t n)
 {
-    if (n <= c->hmm_cap) return PSB_OK;
-    if (c->d_hmms) cudaFree(c->d_hmms);
-    if (c->h_hmms) cudaFreeHost(c->h_hmms);
-    c->d_hmms = nullptr; c->h_hmms = nullptr;
-    c->hmm_cap = n + n / 2 + 256;
-    PSB_CUDA(cudaMalloc(&c->d_hmms, c->hmm_cap * sizeof(psb_hmm_t)));
-    PSB_CUDA(cudaMallocHost(&c->h_hmms, c->hmm_cap * sizeof(psb_hmm_t)));
-    return PSB_OK;
+    const int rc = c->d_hmms.reserve(n, n / 2 + 256);
+    return rc ? rc : c->h_hmms.reserve(n, n / 2 + 256);
 }
 
 static int eval_staged(psb_hmmctx_t *c, int32_t n, const int16_t *senscr, int32_t *best)
@@ -389,27 +373,26 @@ extern "C" int psb_phoneloop_create(psb_hmmctx_t *c, int32_t n_phones, const int
     PSB_REQUIRE(c && out && n_phones > 0 && ssid && tmatid && window >= 0, "psb_phoneloop_create: bad argument");
     PSB_CUDA(cudaSetDevice(c->device));
     std::vector<uint16_t> senid((size_t)c->n_emit * n_phones);          // [state][phone]: coalesced reads in the kernel
-    const int rc = ctx_senids(c, "psb_phoneloop_create", n_phones, ssid, tmatid, senid.data(), 1, n_phones);
+    int rc = ctx_senids(c, "psb_phoneloop_create", n_phones, ssid, tmatid, senid.data(), 1, n_phones);
     if (rc) return rc;
-    psb_phoneloop_t *p = new psb_phoneloop_t();
-    memset(p, 0, sizeof(*p));
+    std::unique_ptr<psb_phoneloop_t> p(new psb_phoneloop_t());
     p->c = c; p->n_phones = n_phones; p->window = window; p->beam = beam; p->pbeam = pbeam; p->pip = pip;
     p->penalty_weight = penalty_weight;
-    cudaError_t e = cudaMalloc(&p->d_senid, senid.size() * 2);
-    if (e == cudaSuccess) e = cudaMemcpy(p->d_senid, senid.data(), senid.size() * 2, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMalloc(&p->d_tmatid, (size_t)n_phones * 4);
+    rc = p->d_senid.reserve(senid.size());
+    if (!rc) rc = p->d_tmatid.reserve((size_t)n_phones);
+    if (!rc) rc = p->d_ssid.reserve((size_t)n_phones);
+    if (!rc) rc = p->d_flags.reserve(1);
+    if (rc) return rc;
+    cudaError_t e = cudaMemcpy(p->d_senid, senid.data(), senid.size() * 2, cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaMemcpy(p->d_tmatid, tmatid, (size_t)n_phones * 4, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMalloc(&p->d_ssid, (size_t)n_phones * 4);
     if (e == cudaSuccess) e = cudaMemcpy(p->d_ssid, ssid, (size_t)n_phones * 4, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMalloc(&p->d_flags, 4);
     if (e == cudaSuccess) e = cudaMemset(p->d_flags, 0, 4);
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking);
+    if (e == cudaSuccess) e = p->stream.create();
     if (e != cudaSuccess) {
         psb_set_error("psb_phoneloop_create: %s", cudaGetErrorString(e));
-        psb_phoneloop_free(p);
         return PSB_ERR_CUDA;
     }
-    *out = p;
+    *out = p.release();
     return PSB_OK;
 }
 
@@ -417,9 +400,7 @@ extern "C" void psb_phoneloop_free(psb_phoneloop_t *p)
 {
     if (!p) return;
     cudaSetDevice(p->c->device);
-    if (p->stream) cudaStreamSynchronize(p->stream);
-    cudaFree(p->d_senid); cudaFree(p->d_tmatid); cudaFree(p->d_ssid); cudaFree(p->d_flags);
-    if (p->stream) cudaStreamDestroy(p->stream);
+    cudaStreamSynchronize(p->stream);
     delete p;
 }
 
@@ -452,11 +433,11 @@ extern "C" int psb_phoneloop_run_device(psb_phoneloop_t *p, const int16_t *d_sen
     if (rc) return rc;
     PSB_CUDA(cudaSetDevice(p->c->device));
     cudaStream_t st = batch ? psb_batch_stream((psb_batch_t *)batch) : p->stream;
-    int32_t *d_off = nullptr;
-    psb_hmm_t *d_final = nullptr;
-    PSB_CUDA(cudaMalloc(&d_off, (size_t)(n_utt + 1) * 4));
+    DevBuf<int32_t> d_off;
+    DevBuf<psb_hmm_t> d_final;
+    if ((rc = d_off.reserve((size_t)n_utt + 1))) return rc;
+    if (final_hmms && (rc = d_final.reserve((size_t)n_utt * p->n_phones))) return rc;
     PSB_CUDA(cudaMemcpyAsync(d_off, utt_off, (size_t)(n_utt + 1) * 4, cudaMemcpyHostToDevice, st));
-    if (final_hmms) PSB_CUDA(cudaMalloc(&d_final, (size_t)n_utt * p->n_phones * sizeof(psb_hmm_t)));
     rc = psb_phoneloop_launch(p, d_senscr, d_off, n_utt, d_best, d_pen, d_final, nullptr, st);
     if (!rc && final_hmms) {
         cudaError_t e = cudaMemcpyAsync(final_hmms, d_final, (size_t)n_utt * p->n_phones * sizeof(psb_hmm_t),
@@ -464,8 +445,6 @@ extern "C" int psb_phoneloop_run_device(psb_phoneloop_t *p, const int16_t *d_sen
         if (e != cudaSuccess) { psb_set_error("%s", cudaGetErrorString(e)); rc = PSB_ERR_CUDA; }
     }
     cudaStreamSynchronize(st);
-    cudaFree(d_off);
-    cudaFree(d_final);
     return rc;
 }
 
@@ -478,14 +457,15 @@ extern "C" int psb_phoneloop_run_host(psb_phoneloop_t *p, const int16_t *senscr,
     if (rc) return rc;
     PSB_CUDA(cudaSetDevice(p->c->device));
     const size_t total = utt_off[n_utt], H = p->n_phones;
-    int16_t *d_scr = nullptr; int32_t *d_off = nullptr, *d_best = nullptr, *d_pen = nullptr; psb_hmm_t *d_tr = nullptr;
-    cudaError_t e = cudaMalloc(&d_scr, std::max<size_t>(2, total * p->c->n_sen * 2));
-    if (e == cudaSuccess) e = cudaMemcpy(d_scr, senscr, total * p->c->n_sen * 2, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMalloc(&d_off, (size_t)(n_utt + 1) * 4);
+    DevBuf<int16_t> d_scr;
+    DevBuf<int32_t> d_off, d_best, d_pen;
+    DevBuf<psb_hmm_t> d_tr;
+    if ((rc = d_scr.reserve(std::max<size_t>(1, total * p->c->n_sen))) || (rc = d_off.reserve((size_t)n_utt + 1)) ||
+        (best && (rc = d_best.reserve(std::max<size_t>(1, total)))) || (pen && (rc = d_pen.reserve(std::max<size_t>(1, total * H)))) ||
+        (hmm_trace && (rc = d_tr.reserve(std::max<size_t>(1, total * H)))))
+        return rc;
+    cudaError_t e = cudaMemcpy(d_scr, senscr, total * p->c->n_sen * 2, cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaMemcpy(d_off, utt_off, (size_t)(n_utt + 1) * 4, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess && best) e = cudaMalloc(&d_best, std::max<size_t>(4, total * 4));
-    if (e == cudaSuccess && pen) e = cudaMalloc(&d_pen, std::max<size_t>(4, total * H * 4));
-    if (e == cudaSuccess && hmm_trace) e = cudaMalloc(&d_tr, std::max<size_t>(4, total * H * sizeof(psb_hmm_t)));
     if (e == cudaSuccess) {
         rc = psb_phoneloop_launch(p, d_scr, d_off, n_utt, d_best, d_pen, nullptr, d_tr, p->stream);
         if (!rc) e = cudaStreamSynchronize(p->stream);
@@ -495,7 +475,6 @@ extern "C" int psb_phoneloop_run_host(psb_phoneloop_t *p, const int16_t *senscr,
             e = cudaMemcpy(hmm_trace, d_tr, total * H * sizeof(psb_hmm_t), cudaMemcpyDeviceToHost);
     }
     if (e != cudaSuccess) { psb_set_error("psb_phoneloop_run_host: %s", cudaGetErrorString(e)); rc = PSB_ERR_CUDA; }
-    cudaFree(d_scr); cudaFree(d_off); cudaFree(d_best); cudaFree(d_pen); cudaFree(d_tr);
     return rc;
 }
 
@@ -522,15 +501,16 @@ struct psb_hmmset_s {
     int32_t n_seg_max, n_seg;
     int64_t max_seg_len;
     bool any_mpx;                 // some instance is multiplexed (hmm_t.mpx): the fused sweep leaves those to the per-frame kernel
-    int32_t *d_i32;               // [pitch / HS_TS][2*NS + 4][HS_TS]: score[NS] hist[NS] out_score out_hist best frame
-    uint16_t *d_u16;              // [pitch / HS_TS][NS + 2][HS_TS]: senid[NS] ssid tmatid(int16)
-    uint8_t *d_mpx;               // [pitch]
-    int64_t *d_seg_off;           // [n_seg_max + 1] caller's offsets (AoS order)
-    int64_t *d_seg_base;          // [n_seg_max + 1] padded offsets inside the set
-    psb_hmm_t *d_aos;             // staging for upload / download
-    int32_t *d_snap_i32;          // psb_hmmset_snapshot: copy of the mutable state (scores, histories, exits)
-    cudaStream_t stream, own_stream;
-    cudaEvent_t ev[2];
+    Stream own_stream;            // declared first: destroyed after the buffers below
+    cudaStream_t stream;          // own_stream, or a batch's after psb_hmmset_use_batch_stream
+    DevBuf<int32_t> d_i32;        // [pitch / HS_TS][2*NS + 4][HS_TS]: score[NS] hist[NS] out_score out_hist best frame
+    DevBuf<uint16_t> d_u16;       // [pitch / HS_TS][NS + 2][HS_TS]: senid[NS] ssid tmatid(int16)
+    DevBuf<uint8_t> d_mpx;        // [pitch]
+    DevBuf<int64_t> d_seg_off;    // [n_seg_max + 1] caller's offsets (AoS order)
+    DevBuf<int64_t> d_seg_base;   // [n_seg_max + 1] padded offsets inside the set
+    DevBuf<psb_hmm_t> d_aos;      // staging for upload / download
+    DevBuf<int32_t> d_snap_i32;   // psb_hmmset_snapshot: copy of the mutable state (scores, histories, exits)
+    Event ev[2];
 };
 
 namespace {
@@ -1091,11 +1071,6 @@ extern "C" void psb_hmmset_free(psb_hmmset_t *s)
     if (!s) return;
     cudaSetDevice(s->c->device);
     if (s->stream) cudaStreamSynchronize(s->stream);
-    cudaFree(s->d_i32); cudaFree(s->d_u16); cudaFree(s->d_mpx); cudaFree(s->d_seg_off); cudaFree(s->d_seg_base); cudaFree(s->d_aos);
-    cudaFree(s->d_snap_i32);
-    if (s->ev[0]) cudaEventDestroy(s->ev[0]);
-    if (s->ev[1]) cudaEventDestroy(s->ev[1]);
-    if (s->own_stream) cudaStreamDestroy(s->own_stream);
     delete s;
 }
 
@@ -1103,25 +1078,25 @@ extern "C" int psb_hmmset_create(psb_hmmctx_t *c, int64_t n_max, int32_t n_seg_m
 {
     PSB_REQUIRE(c && out && n_max > 0 && n_seg_max > 0 && n_seg_max <= 65535, "psb_hmmset_create: bad argument");
     PSB_CUDA(cudaSetDevice(c->device));
-    psb_hmmset_t *s = new psb_hmmset_t();
+    std::unique_ptr<psb_hmmset_t> s(new psb_hmmset_t());
     s->c = c; s->n_max = n_max; s->n_seg_max = n_seg_max;
     s->pitch = ((n_max + (int64_t)(HS_V - 1) * n_seg_max + HS_TS - 1) / HS_TS) * HS_TS;   // every segment may pad up to 3
     const int ns = c->n_emit;
-    cudaError_t e = cudaMalloc(&s->d_i32, (size_t)(2 * ns + 4) * s->pitch * 4);
-    if (e == cudaSuccess) e = cudaMalloc(&s->d_u16, (size_t)(ns + 2) * s->pitch * 2);
-    if (e == cudaSuccess) e = cudaMalloc(&s->d_mpx, (size_t)s->pitch);
-    if (e == cudaSuccess) e = cudaMalloc(&s->d_seg_off, (size_t)(n_seg_max + 1) * 8);
-    if (e == cudaSuccess) e = cudaMalloc(&s->d_seg_base, (size_t)(n_seg_max + 1) * 8);
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&s->own_stream, cudaStreamNonBlocking);
+    int rc = s->d_i32.reserve((size_t)(2 * ns + 4) * s->pitch);
+    if (!rc) rc = s->d_u16.reserve((size_t)(ns + 2) * s->pitch);
+    if (!rc) rc = s->d_mpx.reserve((size_t)s->pitch);
+    if (!rc) rc = s->d_seg_off.reserve((size_t)n_seg_max + 1);
+    if (!rc) rc = s->d_seg_base.reserve((size_t)n_seg_max + 1);
+    if (rc) return rc;
+    cudaError_t e = s->own_stream.create();
     s->stream = s->own_stream;
-    if (e == cudaSuccess) e = cudaEventCreate(&s->ev[0]);
-    if (e == cudaSuccess) e = cudaEventCreate(&s->ev[1]);
+    if (e == cudaSuccess) e = s->ev[0].create();
+    if (e == cudaSuccess) e = s->ev[1].create();
     if (e != cudaSuccess) {
         psb_set_error("psb_hmmset_create: %s", cudaGetErrorString(e));
-        psb_hmmset_free(s);
         return PSB_ERR_CUDA;
     }
-    *out = s;
+    *out = s.release();
     return PSB_OK;
 }
 
@@ -1141,7 +1116,8 @@ extern "C" int psb_hmmset_snapshot(psb_hmmset_t *s)
     PSB_REQUIRE(s && !s->any_mpx, "psb_hmmset_snapshot: null set or multiplexed instances");
     PSB_CUDA(cudaSetDevice(s->c->device));
     const size_t nb = (size_t)(2 * s->c->n_emit + 4) * s->pitch * 4;
-    if (!s->d_snap_i32) PSB_CUDA(cudaMalloc(&s->d_snap_i32, nb));
+    const int rc = s->d_snap_i32.reserve(nb / 4);
+    if (rc) return rc;
     PSB_CUDA(cudaMemcpyAsync(s->d_snap_i32, s->d_i32, nb, cudaMemcpyDeviceToDevice, s->stream));
     return PSB_OK;
 }
@@ -1156,8 +1132,7 @@ extern "C" int psb_hmmset_restore(psb_hmmset_t *s)
 
 static int hmmset_staging(psb_hmmset_t *s)
 {
-    if (!s->d_aos) PSB_CUDA(cudaMalloc(&s->d_aos, (size_t)s->n_max * sizeof(psb_hmm_t)));
-    return PSB_OK;
+    return s->d_aos.reserve((size_t)s->n_max);
 }
 
 extern "C" int psb_hmmset_upload(psb_hmmset_t *s, const psb_hmm_t *hmms, int64_t n, const int64_t *seg_off, int32_t n_seg)
@@ -1399,18 +1374,17 @@ extern "C" int psb_hmmset_eval_host(psb_hmmset_t *s, const int16_t *senscr, int3
     // one frame, host rows [n_seg][n_sen] in, host best[n_seg] out (tests and small callers)
     PSB_REQUIRE(s && senscr && best, "psb_hmmset_eval_host: bad argument");
     PSB_CUDA(cudaSetDevice(s->c->device));
-    int16_t *d_scr = nullptr;
-    int32_t *d_best = nullptr;
+    DevBuf<int16_t> d_scr;
+    DevBuf<int32_t> d_best;
     const size_t nb = (size_t)s->n_seg * s->c->n_sen * 2;
-    PSB_CUDA(cudaMalloc(&d_scr, nb));
-    cudaError_t e = cudaMalloc(&d_best, (size_t)s->n_seg * 4);
-    if (e == cudaSuccess) e = cudaMemcpy(d_scr, senscr, nb, cudaMemcpyHostToDevice);
-    int rc = PSB_OK;
+    int rc = d_scr.reserve(nb / 2);
+    if (!rc) rc = d_best.reserve((size_t)s->n_seg);
+    if (rc) return rc;
+    cudaError_t e = cudaMemcpy(d_scr, senscr, nb, cudaMemcpyHostToDevice);
     if (e == cudaSuccess) {
         rc = psb_hmmset_eval_frames_device(s, d_scr, nullptr, nullptr, 1, d_best, nullptr);
         if (!rc) e = cudaMemcpy(best, d_best, (size_t)s->n_seg * 4, cudaMemcpyDeviceToHost);
     }
-    cudaFree(d_scr); cudaFree(d_best);
     if (e != cudaSuccess) {
         psb_set_error("psb_hmmset_eval_host: %s", cudaGetErrorString(e));
         return PSB_ERR_CUDA;
@@ -1599,12 +1573,14 @@ extern "C" int psb_align_batch_device(psb_hmmctx_t *c, const int16_t *d_senscr, 
     int32_t *d_i32 = nullptr, *d_tok = nullptr;
     uint16_t *d_senid = nullptr;
     int64_t *d_tokoff = nullptr;
-    cudaError_t e = srch_reserve(c, 0, n_i32, &d_i32);
-    if (e == cudaSuccess) e = srch_reserve(c, 1, n_tok, &d_tok);
-    if (e == cudaSuccess) e = srch_reserve(c, 2, senid.size(), &d_senid);
-    if (e == cudaSuccess) e = srch_reserve(c, 3, tok_off.size(), &d_tokoff);
-    if (e == cudaSuccess && !c->al_ev[0]) e = cudaEventCreate(&c->al_ev[0]);
-    if (e == cudaSuccess && !c->al_ev[1]) e = cudaEventCreate(&c->al_ev[1]);
+    rc = srch_reserve(c, 0, n_i32, &d_i32);
+    if (!rc) rc = srch_reserve(c, 1, n_tok, &d_tok);
+    if (!rc) rc = srch_reserve(c, 2, senid.size(), &d_senid);
+    if (!rc) rc = srch_reserve(c, 3, tok_off.size(), &d_tokoff);
+    if (rc) return rc;
+    cudaError_t e = cudaSuccess;
+    if (!c->al_ev[0]) e = c->al_ev[0].create();
+    if (e == cudaSuccess && !c->al_ev[1]) e = c->al_ev[1].create();
     cudaStream_t st = c->stream;
     if (e == cudaSuccess) e = cudaMemcpyAsync(d_i32 + o_utt, utt_off, ((size_t)n_utt + 1) * 4, cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess) e = cudaMemcpyAsync(d_i32 + o_ph, ph_off, ((size_t)n_utt + 1) * 4, cudaMemcpyHostToDevice, st);
@@ -1650,12 +1626,11 @@ extern "C" int psb_align_batch_host(psb_hmmctx_t *c, const int16_t *senscr, cons
     if (rc) return rc;
     PSB_CUDA(cudaSetDevice(c->device));
     const size_t nb = (size_t)utt_off[n_utt] * c->n_sen * 2;
-    int16_t *d = nullptr;
-    PSB_CUDA(cudaMalloc((void **)&d, std::max<size_t>(nb, 2)));
+    DevBuf<int16_t> d;
+    if ((rc = d.reserve(std::max<size_t>(nb / 2, 1)))) return rc;
     cudaError_t e = nb ? cudaMemcpy(d, senscr, nb, cudaMemcpyHostToDevice) : cudaSuccess;
     if (e == cudaSuccess)
         rc = psb_align_batch_device(c, d, utt_off, n_utt, ph_off, ssid, tmatid, sf, ef, st_start, st_dur, st_score, status);
-    cudaFree(d);
     if (e != cudaSuccess) {
         psb_set_error("psb_align_batch_host: %s", cudaGetErrorString(e));
         return PSB_ERR_CUDA;
@@ -1826,11 +1801,12 @@ extern "C" int psb_kws_batch_device(psb_hmmctx_t *c, const int16_t *d_senscr, co
     int32_t *d_i = nullptr, *d_hits = nullptr;
     uint16_t *d_senid = nullptr;
     const size_t hits_n = (size_t)n_utt * cap_per_utt * 5;
-    cudaError_t e = srch_reserve(c, 0, ibuf.size(), &d_i);
-    if (e == cudaSuccess) e = srch_reserve(c, 1, hits_n, &d_hits);
-    if (e == cudaSuccess) e = srch_reserve(c, 2, senid.size(), &d_senid);
+    rc = srch_reserve(c, 0, ibuf.size(), &d_i);
+    if (!rc) rc = srch_reserve(c, 1, hits_n, &d_hits);
+    if (!rc) rc = srch_reserve(c, 2, senid.size(), &d_senid);
+    if (rc) return rc;
     cudaStream_t st = c->stream;
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_i, ibuf.data(), ibuf.size() * 4, cudaMemcpyHostToDevice, st);
+    cudaError_t e = cudaMemcpyAsync(d_i, ibuf.data(), ibuf.size() * 4, cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess) e = cudaMemcpyAsync(d_senid, senid.data(), senid.size() * 2, cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(kws_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e == cudaSuccess)
@@ -2044,11 +2020,12 @@ static int allphone_common(psb_hmmctx_t *c, const int16_t *d_senscr, const int32
     int32_t *d_i = nullptr, *d_hist = nullptr;
     uint16_t *d_senid = nullptr;
     const size_t hist_n = (size_t)n_utt * cap_per_utt * ROW;
-    cudaError_t e = srch_reserve(c, 0, ibuf.size(), &d_i);
-    if (e == cudaSuccess) e = srch_reserve(c, 1, hist_n, &d_hist);
-    if (e == cudaSuccess) e = srch_reserve(c, 2, senid.size(), &d_senid);
+    rc = srch_reserve(c, 0, ibuf.size(), &d_i);
+    if (!rc) rc = srch_reserve(c, 1, hist_n, &d_hist);
+    if (!rc) rc = srch_reserve(c, 2, senid.size(), &d_senid);
+    if (rc) return rc;
     cudaStream_t st = c->stream;
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_i, ibuf.data(), ibuf.size() * 4, cudaMemcpyHostToDevice, st);
+    cudaError_t e = cudaMemcpyAsync(d_i, ibuf.data(), ibuf.size() * 4, cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess) e = cudaMemcpyAsync(d_senid, senid.data(), senid.size() * 2, cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(allphone_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(allphone_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -2194,14 +2171,15 @@ extern "C" int psb_allphone_net_batch_device(psb_hmmctx_t *c, const int16_t *d_s
     int32_t *d_i = nullptr, *d_hist = nullptr, *d_work = nullptr, *d_segs = nullptr;
     uint16_t *d_senid = nullptr;
     uint64_t *d_masks = nullptr;
-    cudaError_t e = srch_reserve(c, 0, ibuf.size(), &d_i);
-    if (e == cudaSuccess) e = srch_reserve(c, 1, hist_n, &d_hist);
-    if (e == cudaSuccess) e = srch_reserve(c, 2, senid.size(), &d_senid);
-    if (e == cudaSuccess) e = srch_reserve(c, 3, work_words * (size_t)n_utt, &d_work);
-    if (e == cudaSuccess) e = srch_reserve(c, 4, masks.size(), &d_masks);
-    if (e == cudaSuccess) e = srch_reserve(c, 5, seg_n, &d_segs);
+    int ret = srch_reserve(c, 0, ibuf.size(), &d_i);
+    if (!ret) ret = srch_reserve(c, 1, hist_n, &d_hist);
+    if (!ret) ret = srch_reserve(c, 2, senid.size(), &d_senid);
+    if (!ret) ret = srch_reserve(c, 3, work_words * (size_t)n_utt, &d_work);
+    if (!ret) ret = srch_reserve(c, 4, masks.size(), &d_masks);
+    if (!ret) ret = srch_reserve(c, 5, seg_n, &d_segs);
+    if (ret) return ret;
     cudaStream_t st = c->stream;
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_i, ibuf.data(), ibuf.size() * 4, cudaMemcpyHostToDevice, st);
+    cudaError_t e = cudaMemcpyAsync(d_i, ibuf.data(), ibuf.size() * 4, cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess) e = cudaMemcpyAsync(d_senid, senid.data(), senid.size() * 2, cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess) e = cudaMemcpyAsync(d_masks, masks.data(), masks.size() * 8, cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess) {

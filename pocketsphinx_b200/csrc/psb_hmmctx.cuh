@@ -11,19 +11,21 @@
 struct psb_hmmctx_s {
     int device;
     int n_emit, n_tmat, n_sseq, n_sen;
-    uint8_t *d_tp;
-    uint16_t *d_sseq, *h_sseq;    // [n_sseq][n_emit], on the device and on the host
-    cudaStream_t stream;
+    Stream stream;                // declared first: destroyed after the buffers below
+    DevBuf<uint8_t> d_tp;
+    DevBuf<uint16_t> d_sseq;      // [n_sseq][n_emit], on the device and on the host
+    std::vector<uint16_t> h_sseq;
     // staging for psb_hmm_vit_eval_batch
-    psb_hmm_t *d_hmms, *h_hmms;
-    size_t hmm_cap;
-    int16_t *d_senscr, *h_senscr;
-    int32_t *d_best, *h_best;
-    cudaEvent_t al_ev[2];         // around the last psb_align_batch_* kernel
+    DevBuf<psb_hmm_t> d_hmms;
+    HostBuf<psb_hmm_t> h_hmms;
+    DevBuf<int16_t> d_senscr;
+    HostBuf<int16_t> h_senscr;
+    DevBuf<int32_t> d_best;
+    HostBuf<int32_t> h_best;
+    Event al_ev[2];               // around the last psb_align_batch_* kernel
     float last_align_ms;
     // grow-only device workspace of the whole-utterance entry points (srch_reserve)
-    void *d_srch[10];
-    size_t srch_cap[10];
+    DevBuf<unsigned char> srch[10];
 };
 
 static inline HmmCtxDev dev_ctx(const psb_hmmctx_t *c)
@@ -34,20 +36,14 @@ static inline HmmCtxDev dev_ctx(const psb_hmmctx_t *c)
 }
 
 // Grow-only device workspace kept in the context: repeated calls (one per batch) do not pay
-// cudaMalloc / cudaFree again.
+// an allocation again.
 template <class T>
-static cudaError_t srch_reserve(psb_hmmctx_t *c, int slot, size_t count, T **out)
+static int srch_reserve(psb_hmmctx_t *c, int slot, size_t count, T **out)
 {
     const size_t bytes = (count > 0 ? count : 1) * sizeof(T);
-    if (bytes > c->srch_cap[slot]) {
-        cudaFree(c->d_srch[slot]);
-        c->d_srch[slot] = nullptr; c->srch_cap[slot] = 0;
-        const cudaError_t e = cudaMalloc(&c->d_srch[slot], bytes + bytes / 4);
-        if (e != cudaSuccess) return e;
-        c->srch_cap[slot] = bytes + bytes / 4;
-    }
-    *out = (T *)c->d_srch[slot];
-    return cudaSuccess;
+    const int rc = c->srch[slot].reserve(bytes, bytes / 4);
+    *out = reinterpret_cast<T *>(c->srch[slot].get());
+    return rc;
 }
 
 // The utterances of a whole-utterance entry point: offsets from 0 that never decrease, and scores wherever

@@ -6,10 +6,12 @@
 #include <stdio.h>
 
 #include <atomic>
+#include <memory>
 #include <string>
 #include <vector>
 
 #include "../../include/psb200.h"
+#include "psb_mem.cuh"
 
 #define PSB_SENSCR_SHIFT 10      // hmm.h:72
 #define PSB_MAX_NEG_ASCR 96      // tied_mgau_common.h:91
@@ -89,80 +91,72 @@ struct psb_model_s {
     int mixw_stride;              // padded row pitch on the device (multiple of 128)
     int logadd_ms_size, logadd_ms_zero;
     // device buffers
-    float *d_rec;                 // records; (cb, f) block at rec_off[cb * n_feat + f]
+    DevBuf<float> d_rec;          // records; (cb, f) block at rec_off[cb * n_feat + f]
     std::vector<size_t> rec_off;  // float offsets, host copy
-    size_t *d_rec_off;
-    float *d_rec2;                // pair-interleaved, negated records for the codeword-pair kernels
-    size_t *d_rec2_off;
-    uint8_t *d_mixw;              // [n_feat][n_density][mixw_stride] (ptm/semi) or raw pdf (ms)
-    uint8_t *d_mixw_cb;           // 16 bytes or null
-    uint16_t *d_sen2cb;           // [n_sen] (ptm)
-    int32_t *d_sen2cb32;          // [n_sen] (ms)
+    DevBuf<size_t> d_rec_off;
+    DevBuf<float> d_rec2;         // pair-interleaved, negated records for the codeword-pair kernels
+    DevBuf<size_t> d_rec2_off;
+    DevBuf<uint8_t> d_mixw;       // [n_feat][n_density][mixw_stride] (ptm/semi) or raw pdf (ms)
+    DevBuf<uint8_t> d_mixw_cb;    // 16 bytes or null
+    DevBuf<uint16_t> d_sen2cb;    // [n_sen] (ptm)
+    DevBuf<int32_t> d_sen2cb32;   // [n_sen] (ms)
     bool sen_is_cb;               // ms: senone s uses codebook s (continuous models): distances and mixtures in one kernel
-    int16_t *d_quadcb;            // [ceil(n_sen/4)] codebook of a uniform senone quad, else -1
-    int32_t *d_bsen;              // senones of the non-uniform quads
+    DevBuf<int16_t> d_quadcb;     // [ceil(n_sen/4)] codebook of a uniform senone quad, else -1
+    DevBuf<int32_t> d_bsen;       // senones of the non-uniform quads
     int n_bsen;
     int logadd8_max;              // largest entry of the 8-bit add table (bias bound of the 16x2 senone kernel)
-    uint8_t *d_logadd8;           // [PSB_LOGADD8_N]: the 256-entry table continued with zeros
-    uint32_t *d_logadd_ms;
-    float *d_msT, *d_msdetT;      // ms back-end: codebook-minor Gaussians (see psb_ms.cu)
-    int32_t *d_featlen, *d_featoff;
+    DevBuf<uint8_t> d_logadd8;    // [PSB_LOGADD8_N]: the 256-entry table continued with zeros
+    DevBuf<uint32_t> d_logadd_ms;
+    DevBuf<float> d_msT, d_msdetT;   // ms back-end: codebook-minor Gaussians (see psb_ms.cu)
+    DevBuf<int32_t> d_featlen, d_featoff;
     uint8_t topn_beam[PSB_MAX_FEAT];
-    int32_t *d_topn_beam;         // [PSB_MAX_FEAT]
+    DevBuf<int32_t> d_topn_beam;  // [PSB_MAX_FEAT]
     bool has_topn_beam;
     // tensor-core filter path (psb_ptm_tc.cu): W in the wgmma operand layout, centres, error-bound coefficients
     bool tc_ok;
-    float *d_tc_wumma, *d_tc_cen, *d_tc_bnd;
+    DevBuf<float> d_tc_wumma, d_tc_cen, d_tc_bnd;
 };
 
+// A batch, or one sub-batch of its pipelined decode.  A sub-batch borrows the parent's d_feats, d_senscr, d_best,
+// d_pen and a range of its top-N records; every batch reads its records through the d_topn view.
 struct psb_batch_s {
     psb_model_t *m;
-    cudaStream_t stream;
+    Stream stream;                // declared first: destroyed after the buffers below
     int max_utts;
     long long max_frames;
     // device
-    float *d_feats;               // [max_frames][sumlen] staging for the _host path
-    int16_t *d_senscr;            // [max_frames][n_sen]
-    float *d_featT;               // transposed groups
-    size_t featT_cap;             // floats
-    int4 *d_topn;                 // [max_frames][K]
-    int32_t *d_tab;               // per-call lane/group tables
-    size_t tab_cap;
-    int32_t *h_tab;               // pinned
-    // pinned host staging for the _host path
-    float *h_feats;
-    int16_t *h_senscr;
-    cudaEvent_t ev[4];
-    cudaEvent_t tev[2];           // user stopwatch (psb_batch_event_record)
-    bool have_ev;
+    DevBuf<float> d_feats;        // [max_frames][sumlen] staging for the _host path
+    DevBuf<int16_t> d_senscr;     // [max_frames][n_sen]
+    DevBuf<float> d_featT;        // transposed groups
+    DevBuf<int4> topn;            // [max_frames][K] (parent only)
+    int4 *d_topn;                 // view: topn, or a sub-batch's range of its parent's
+    DevBuf<int32_t> d_tab;        // per-call lane/group tables
+    HostBuf<int32_t> h_tab;
+    Event ev[4];
+    Event tev[2];                 // user stopwatch (psb_batch_event_record)
     long long last_frames;
-    float2 *d_semi_dist; size_t semi_cap;      // semi-continuous split path: {d, partial} per (stream, frame, codeword)
-    int32_t *d_uttoff; size_t uttoff_cap;
+    DevBuf<float2> d_semi_dist;   // semi-continuous split path: {d, partial} per (stream, frame, codeword)
+    DevBuf<int32_t> d_uttoff;
     int topn_variant;             // PSB_TOPN_VARIANT: 0 scalar, 2 codeword pairs, 3 two utterances per lane,
                                   // 4/5 pairs + deferred insertion (2 / 1 utterances per lane),
                                   // 6 (default) tensor-core filter + exact rescoring where the model allows, else 5
-    unsigned *d_tc_flags; size_t tc_flag_cap, tc_flag_words;   // [K][words]: frames the tie fix-up redoes
-    float *d_tc_check;            // debug (PSB_TC_CHECK=1): max |a - d| / eps, max candidates, decision-path counters
+    DevBuf<unsigned> d_tc_flags; size_t tc_flag_words;   // [K][words]: frames the tie fix-up redoes
+    DevBuf<float> d_tc_check;     // debug (PSB_TC_CHECK=1): max |a - d| / eps, max candidates, decision-path counters
     int tc_last_tpc;              // the last filter launch: tiles per CTA and CTAs per pair
     long long tc_last_ctas;
-    uint4 *d_tc_items; unsigned *d_tc_nitems; unsigned tc_item_cap;   // rows the filter left in doubt (ptm_tc_exact_kernel)
+    DevBuf<uint4> d_tc_items; DevBuf<unsigned> d_tc_nitems; unsigned tc_item_cap;   // rows the filter left in doubt (ptm_tc_exact_kernel)
     // phone-loop outputs for psb_decode_batch_host
-    int32_t *d_best, *d_pen;
-    int32_t *h_best, *h_pen;
-    size_t pen_cap;
-    int32_t *d_off;               // utt_off on the device for the phone loop
-    void *d_msdist;               // ms back-end: per-chunk top-N distance lists
-    int32_t *d_msbest;
-    size_t ms_cap;
-    size_t off_cap;
+    DevBuf<int32_t> d_best, d_pen;
+    DevBuf<int32_t> d_off;        // utt_off on the device for the phone loop
+    DevBuf<unsigned char> d_msdist;   // ms back-end: per-chunk top-N distance lists
+    DevBuf<int32_t> d_msbest;
     // pipelined decode: sub-batches on their own streams sharing this batch's big buffers
-    std::vector<psb_batch_t *> kids;
-    cudaEvent_t fork_ev, join_ev;
+    std::vector<std::unique_ptr<psb_batch_t>> kids;
+    Event fork_ev, join_ev;
     int n_pipe;                   // PSB_PIPELINE: 0 = auto (default), 1 = everything on `stream`, n = n ranges
-    bool is_kid;
     bool last_pipelined;
     int last_kids;                // sub-batches used by the last decode call
-    int32_t *h_off;               // pinned copy of a sub-batch's utterance offsets
+    HostBuf<int32_t> h_off;       // pinned copy of a sub-batch's utterance offsets
 };
 
 // ---- launchers implemented in the .cu files ----

@@ -363,20 +363,16 @@ int psb_launch_ms_batch(psb_batch_t *b, const float *d_feats, const int32_t *utt
     const size_t budget = (size_t)2 << 30;
     long long chunk = std::max<long long>(FT, std::min<long long>(total, (long long)(budget / per_frame) / FT * FT));
     chunk = std::min<long long>(chunk, 65535);              // gridDim.y
-    if (b->ms_cap < (size_t)chunk * per_frame) {
-        cudaFree(b->d_msdist); cudaFree(b->d_msbest);
-        b->d_msdist = nullptr; b->d_msbest = nullptr;
-        b->ms_cap = (size_t)chunk * per_frame;
-        PSB_CUDA(cudaMalloc(&b->d_msdist, b->ms_cap));
-        PSB_CUDA(cudaMalloc(&b->d_msbest, 65536 * sizeof(int32_t)));
-    }
-    if (b->have_ev) PSB_CUDA(cudaEventRecord(b->ev[0], b->stream));
-    if (b->have_ev) PSB_CUDA(cudaEventRecord(b->ev[1], b->stream));
+    int rc = b->d_msdist.reserve((size_t)chunk * per_frame);
+    if (!rc) rc = b->d_msbest.reserve(65536);
+    if (rc) return rc;
+    PSB_CUDA(cudaEventRecord(b->ev[0], b->stream));
+    PSB_CUDA(cudaEventRecord(b->ev[1], b->stream));
     for (long long f0 = 0; f0 < total; f0 += chunk) {
         const long long n = std::min(chunk, total - f0);
         dim3 g1((m->n_mgau + 127) / 128, (unsigned)((n + FT - 1) / FT));
         size_t smem = (size_t)FT * m->sumlen * sizeof(float);
-        int2 *dist = reinterpret_cast<int2 *>(b->d_msdist);
+        int2 *dist = reinterpret_cast<int2 *>(b->d_msdist.get());
         const size_t tile_smem = ((size_t)m->n_density * m->sumlen * 2 + (size_t)m->n_feat * m->n_density) * MS_TCB * sizeof(float)
                                  + (size_t)m->sumlen * MS_TFB * sizeof(float);
         const bool tile = tile_smem <= 100 * 1024;           // else the untiled kernel (parameters streamed from L2)
@@ -424,8 +420,8 @@ int psb_launch_ms_batch(psb_batch_t *b, const float *d_feats, const int32_t *utt
         ms_norm_kernel<<<g2, 256, 0, b->stream>>>(d_senscr, b->d_msbest, f0, m->n_sen, nullptr, m->n_sen);
         PSB_LAUNCH_CHECK();
     }
-    if (b->have_ev) PSB_CUDA(cudaEventRecord(b->ev[2], b->stream));
-    if (b->have_ev) PSB_CUDA(cudaEventRecord(b->ev[3], b->stream));
+    PSB_CUDA(cudaEventRecord(b->ev[2], b->stream));
+    PSB_CUDA(cudaEventRecord(b->ev[3], b->stream));
     return PSB_OK;
 }
 

@@ -1496,13 +1496,9 @@ int psb_launch_ptm_batch(psb_batch_t *b, const float *d_feats, const int32_t *ut
     size_t n32 = (size_t)n_groups * 64 + n_groups + K + PSB_MAX_FEAT;
     n32 = (n32 + 1) & ~(size_t)1;
     size_t need = n32 + 2 * (size_t)(2 * n_groups + 1);
-    if (need > b->tab_cap) {
-        if (b->d_tab) cudaFree(b->d_tab);
-        if (b->h_tab) cudaFreeHost(b->h_tab);
-        b->tab_cap = need * 2;
-        PSB_CUDA(cudaMalloc(&b->d_tab, b->tab_cap * sizeof(int32_t)));
-        PSB_CUDA(cudaMallocHost(&b->h_tab, b->tab_cap * sizeof(int32_t)));
-    }
+    int rc = b->d_tab.reserve(need, need);
+    if (!rc) rc = b->h_tab.reserve(need, need);
+    if (rc) return rc;
     int32_t *lane_len = b->h_tab, *lane_off = lane_len + n_groups * 32, *grp_maxT = lane_off + n_groups * 32;
     int32_t *klist = grp_maxT + n_groups, *featoff = klist + K;
     long long *grp_base = reinterpret_cast<long long *>(b->h_tab + n32), *warp_base = grp_base + n_groups;
@@ -1527,11 +1523,7 @@ int psb_launch_ptm_batch(psb_batch_t *b, const float *d_feats, const int32_t *ut
     }
     warp_base[n_groups] = items;
     for (int f = 0; f < PSB_MAX_FEAT; ++f) featoff[f] = f < m->n_feat ? m->featoff[f] : 0;
-    if ((size_t)featT_floats > b->featT_cap) {
-        if (b->d_featT) cudaFree(b->d_featT);
-        b->featT_cap = (size_t)featT_floats + (featT_floats >> 3);
-        PSB_CUDA(cudaMalloc(&b->d_featT, b->featT_cap * sizeof(float)));
-    }
+    if ((rc = b->d_featT.reserve((size_t)featT_floats, (size_t)featT_floats >> 3))) return rc;
     // k lists per distinct feature length
     std::vector<std::vector<int>> byfl;
     std::vector<int> fls;
@@ -1554,7 +1546,7 @@ int psb_launch_ptm_batch(psb_batch_t *b, const float *d_feats, const int32_t *ut
     const long long *d_warp_base = tabs.grp_base + n_groups;
 
     const bool use_tc = !semi && psb_tc_usable(b);
-    if (b->have_ev) PSB_CUDA(cudaEventRecord(b->ev[0], b->stream));
+    PSB_CUDA(cudaEventRecord(b->ev[0], b->stream));
     if (!use_tc) {
         int warps = 8;
         while (warps > 1 && (size_t)warps * 32 * (D + 1) * sizeof(float) > 48 * 1024) warps >>= 1;
@@ -1565,29 +1557,18 @@ int psb_launch_ptm_batch(psb_batch_t *b, const float *d_feats, const int32_t *ut
             d_feats, b->d_featT, tabs, d_warp_base, n_groups, D);
         PSB_LAUNCH_CHECK();
     }
-    if (b->have_ev) PSB_CUDA(cudaEventRecord(b->ev[1], b->stream));
+    PSB_CUDA(cudaEventRecord(b->ev[1], b->stream));
     // semi-continuous: distances out of the time loop, one warp per (utterance, stream)
     const bool semi_split = semi && !m->fixed_point && m->n_mgau == 1 && b->topn_variant != 0 && m->n_density <= 256 &&
                             (m->n_density == 64 || m->n_density == 128 || m->n_density == 256);
     if (use_tc) {
         // no recurrence over time: tensor-core filter, exact rescoring of the survivors, tie fix-up (psb_ptm_tc.cu)
-        int rc = psb_launch_ptm_tc(b, d_feats, utt_off, n_utt, d_klist, d_featoff);
+        rc = psb_launch_ptm_tc(b, d_feats, utt_off, n_utt, d_klist, d_featoff);
         if (rc) return rc;
     }
     else if (semi_split) {
         const size_t need_d = (size_t)K * total * m->n_density;
-        if (need_d > b->semi_cap) {
-            if (b->d_semi_dist) cudaFree(b->d_semi_dist);
-            b->d_semi_dist = nullptr;
-            b->semi_cap = need_d + need_d / 8;
-            PSB_CUDA(cudaMalloc(&b->d_semi_dist, b->semi_cap * sizeof(float2)));
-        }
-        if ((size_t)n_utt + 1 > b->uttoff_cap) {
-            if (b->d_uttoff) cudaFree(b->d_uttoff);
-            b->d_uttoff = nullptr;
-            b->uttoff_cap = (size_t)n_utt + 1 + 64;
-            PSB_CUDA(cudaMalloc(&b->d_uttoff, b->uttoff_cap * sizeof(int32_t)));
-        }
+        if ((rc = b->d_semi_dist.reserve(need_d, need_d / 8)) || (rc = b->d_uttoff.reserve((size_t)n_utt + 1, 64))) return rc;
         PSB_CUDA(cudaMemcpyAsync(b->d_uttoff, utt_off, ((size_t)n_utt + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, b->stream));
         PSB_REQUIRE(total <= 0x7fffffffLL, "too many frames for one launch");
         int pos = 0;
@@ -1633,7 +1614,7 @@ int psb_launch_ptm_batch(psb_batch_t *b, const float *d_feats, const int32_t *ut
             pos += n_k;
         }
     }
-    if (b->have_ev) PSB_CUDA(cudaEventRecord(b->ev[2], b->stream));
+    PSB_CUDA(cudaEventRecord(b->ev[2], b->stream));
     if (semi) {
         size_t smem = (size_t)K * 32 + PSB_LOGADD8_N + 16;
         PSB_REQUIRE(K <= 512, "semi_senone_kernel handles at most 512 streams (got %d)", K);
@@ -1683,6 +1664,6 @@ int psb_launch_ptm_batch(psb_batch_t *b, const float *d_feats, const int32_t *ut
         }
         PSB_LAUNCH_CHECK();
     }
-    if (b->have_ev) PSB_CUDA(cudaEventRecord(b->ev[3], b->stream));
+    PSB_CUDA(cudaEventRecord(b->ev[3], b->stream));
     return PSB_OK;
 }

@@ -815,11 +815,10 @@ int psb_tc_prepare(psb_model_t *m, const float *hm, const float *hv, const float
             for (int i = 0; i < 32; ++i)
                 if (!std::isfinite(bb[i])) return PSB_OK;    // degenerate model: keep the scan kernels
         }
-    if (!m->d_tc_wumma) {
-        PSB_CUDA(cudaMalloc(&m->d_tc_wumma, wu.size() * sizeof(float)));
-        PSB_CUDA(cudaMalloc(&m->d_tc_cen, cen.size() * sizeof(float)));
-        PSB_CUDA(cudaMalloc(&m->d_tc_bnd, bnd.size() * sizeof(float)));
-    }
+    int rc = m->d_tc_wumma.reserve(wu.size());
+    if (!rc) rc = m->d_tc_cen.reserve(cen.size());
+    if (!rc) rc = m->d_tc_bnd.reserve(bnd.size());
+    if (rc) return rc;
     PSB_CUDA(cudaMemcpy(m->d_tc_wumma, wu.data(), wu.size() * sizeof(float), cudaMemcpyHostToDevice));
     PSB_CUDA(cudaMemcpy(m->d_tc_cen, cen.data(), cen.size() * sizeof(float), cudaMemcpyHostToDevice));
     PSB_CUDA(cudaMemcpy(m->d_tc_bnd, bnd.data(), bnd.size() * sizeof(float), cudaMemcpyHostToDevice));
@@ -840,31 +839,22 @@ int psb_launch_ptm_tc(psb_batch_t *b, const float *d_feats, const int32_t *utt_o
     psb_model_t *m = b->m;
     const long long total = utt_off[n_utt];
     const size_t fw = (size_t)((total + 31) / 32) + 1;
-    if (fw * m->K > b->tc_flag_cap) {
-        cudaFree(b->d_tc_flags);
-        b->d_tc_flags = nullptr;
-        b->tc_flag_cap = fw * m->K + fw * m->K / 8;
-        PSB_CUDA(cudaMalloc(&b->d_tc_flags, b->tc_flag_cap * 4));
+    int rc = b->d_tc_flags.reserve(fw * m->K, fw * m->K / 8);
+    if (!rc) rc = b->d_uttoff.reserve((size_t)n_utt + 1, 64);
+    if (!rc && !b->d_tc_check) {                              // float[2] check values, then (16-byte offset) ST_N 64-bit counters
+        rc = b->d_tc_check.reserve(TC_CHECK_BYTES / sizeof(float));
+        if (!rc) PSB_CUDA(cudaMemsetAsync(b->d_tc_check, 0, TC_CHECK_BYTES, b->stream));
     }
-    if ((size_t)n_utt + 1 > b->uttoff_cap) {
-        if (b->d_uttoff) cudaFree(b->d_uttoff);
-        b->d_uttoff = nullptr;
-        b->uttoff_cap = (size_t)n_utt + 1 + 64;
-        PSB_CUDA(cudaMalloc(&b->d_uttoff, b->uttoff_cap * sizeof(int32_t)));
-    }
-    if (!b->d_tc_check) {                                     // float[2] check values, then (16-byte offset) ST_N 64-bit counters
-        PSB_CUDA(cudaMalloc(&b->d_tc_check, TC_CHECK_BYTES));
-        PSB_CUDA(cudaMemsetAsync(b->d_tc_check, 0, TC_CHECK_BYTES, b->stream));
-    }
+    if (!rc) rc = b->d_tc_nitems.reserve(1);
+    if (rc) return rc;
     {
         // work list of the rows the filter leaves in doubt: room for a quarter of all (frame, pair) rows, 32 bytes each
         const size_t want = std::max<size_t>(4096, (size_t)total * m->K / 4);
-        if (want > b->tc_item_cap || !b->d_tc_items) {
-            cudaFree(b->d_tc_items);
-            b->d_tc_items = nullptr;
-            if (!b->d_tc_nitems) PSB_CUDA(cudaMalloc(&b->d_tc_nitems, 4));
-            b->tc_item_cap = (unsigned)std::min<size_t>(want + want / 8, 0x7fffffffu);
-            PSB_CUDA(cudaMalloc(&b->d_tc_items, (size_t)b->tc_item_cap * 32));
+        if (want > b->tc_item_cap) {
+            const unsigned cap = (unsigned)std::min<size_t>(want + want / 8, 0x7fffffffu);
+            b->tc_item_cap = 0;
+            if ((rc = b->d_tc_items.reserve(2 * (size_t)cap))) return rc;     // two uint4 per item
+            b->tc_item_cap = cap;
         }
         PSB_CUDA(cudaMemsetAsync(b->d_tc_nitems, 0, 4, b->stream));
     }
@@ -872,7 +862,6 @@ int psb_launch_ptm_tc(psb_batch_t *b, const float *d_feats, const int32_t *utt_o
     PSB_CUDA(cudaMemsetAsync(b->d_tc_flags, 0, fw * m->K * 4, b->stream));
     PSB_CUDA(cudaMemcpyAsync(b->d_uttoff, utt_off, ((size_t)n_utt + 1) * sizeof(int32_t), cudaMemcpyHostToDevice, b->stream));
     static const bool check = [] { const char *v = getenv("PSB_TC_CHECK"); return v && atoi(v) != 0; }();
-    int rc;
     switch (m->n_density) {
     case 256: rc = launch_wgmma<13, 256>(b, d_feats, total, d_klist, m->K, d_featoff, check); break;
     case 128: rc = launch_wgmma<13, 128>(b, d_feats, total, d_klist, m->K, d_featoff, check); break;
@@ -919,7 +908,7 @@ extern "C" int psb_batch_tc_counters(psb_batch_t *b, int64_t *out, int32_t n)
     if (b->d_tc_check) {
         PSB_CUDA(cudaSetDevice(b->m->device));
         PSB_CUDA(cudaStreamSynchronize(b->stream));
-        PSB_CUDA(cudaMemcpy(v, reinterpret_cast<unsigned char *>(b->d_tc_check) + 16, 8 * ST_N, cudaMemcpyDeviceToHost));
+        PSB_CUDA(cudaMemcpy(v, reinterpret_cast<unsigned char *>(b->d_tc_check.get()) + 16, 8 * ST_N, cudaMemcpyDeviceToHost));
     }
     v[ST_N] = b->tc_last_tpc;
     v[ST_N + 1] = b->tc_last_ctas;

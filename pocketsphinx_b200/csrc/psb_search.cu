@@ -104,12 +104,13 @@ extern "C" int psb_fsg_batch_device(psb_hmmctx_t *c, const psb_fsg_desc_t *g, co
     const size_t hist_n = (size_t)n_utt * cap_per_utt * FSG_ROW;
     int32_t *d_i = nullptr, *d_hist = nullptr, *d_work = nullptr;
     uint16_t *d_senid = nullptr;
-    cudaError_t e = srch_reserve(c, 0, ibuf.size(), &d_i);
-    if (e == cudaSuccess) e = srch_reserve(c, 1, hist_n, &d_hist);
-    if (e == cudaSuccess) e = srch_reserve(c, 2, work_words * (size_t)n_utt, &d_work);
-    if (e == cudaSuccess) e = srch_reserve(c, 3, senid.size(), &d_senid);
+    rc = srch_reserve(c, 0, ibuf.size(), &d_i);
+    if (!rc) rc = srch_reserve(c, 1, hist_n, &d_hist);
+    if (!rc) rc = srch_reserve(c, 2, work_words * (size_t)n_utt, &d_work);
+    if (!rc) rc = srch_reserve(c, 3, senid.size(), &d_senid);
+    if (rc) return rc;
     cudaStream_t st = c->stream;
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_i, ibuf.data(), ibuf.size() * 4, cudaMemcpyHostToDevice, st);
+    cudaError_t e = cudaMemcpyAsync(d_i, ibuf.data(), ibuf.size() * 4, cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess) e = cudaMemcpyAsync(d_senid, senid.data(), senid.size() * 2, cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess) {
         FsgGraph G;
@@ -208,7 +209,7 @@ extern "C" int psb_ngram_fwdtree_batch_device(psb_hmmctx_t *c, const psb_ngram_d
     const int N = c->n_emit;
     NgsFlat flat;
     std::string err;
-    if (ngs_flatten(g->info, g->model, (long long)g->model_len, g->lm_arrays, (long long)g->lm_arrays_len, g->ci_tmat, c->h_sseq, c->n_sseq, N, c->n_tmat, c->n_sen, flat, err) != 0) {
+    if (ngs_flatten(g->info, g->model, (long long)g->model_len, g->lm_arrays, (long long)g->lm_arrays_len, g->ci_tmat, c->h_sseq.data(), c->n_sseq, N, c->n_tmat, c->n_sen, flat, err) != 0) {
         psb_set_error("psb_ngram_fwdtree_batch_device: %s", err.c_str());
         return PSB_ERR_ARG;
     }
@@ -222,13 +223,14 @@ extern "C" int psb_ngram_fwdtree_batch_device(psb_hmmctx_t *c, const psb_ngram_d
     const size_t n_bp = (size_t)n_utt * bp_cap_per_utt * NGS_BP_ROW, n_bss = (size_t)n_utt * bss_cap_per_utt,
                  n_idx = total_frames + (size_t)n_utt;
     int32_t *d_i = nullptr, *d_work = nullptr, *d_bp = nullptr, *d_bss = nullptr, *d_idx = nullptr;
-    cudaError_t e = srch_reserve(c, 0, ibuf.size(), &d_i);
-    if (e == cudaSuccess) e = srch_reserve(c, 1, work_words * (size_t)n_utt, &d_work);
-    if (e == cudaSuccess) e = srch_reserve(c, 2, n_bp, &d_bp);
-    if (e == cudaSuccess) e = srch_reserve(c, 3, n_bss, &d_bss);
-    if (e == cudaSuccess) e = srch_reserve(c, 4, n_idx, &d_idx);
+    rc = srch_reserve(c, 0, ibuf.size(), &d_i);
+    if (!rc) rc = srch_reserve(c, 1, work_words * (size_t)n_utt, &d_work);
+    if (!rc) rc = srch_reserve(c, 2, n_bp, &d_bp);
+    if (!rc) rc = srch_reserve(c, 3, n_bss, &d_bss);
+    if (!rc) rc = srch_reserve(c, 4, n_idx, &d_idx);
+    if (rc) return rc;
     cudaStream_t st = c->stream;
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_i, ibuf.data(), ibuf.size() * 4, cudaMemcpyHostToDevice, st);
+    cudaError_t e = cudaMemcpyAsync(d_i, ibuf.data(), ibuf.size() * 4, cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess) e = cudaMemsetAsync(d_idx, 0, n_idx * 4, st);
     if (e == cudaSuccess) {
         ngs_bind(flat, d_i);
@@ -322,7 +324,7 @@ extern "C" int psb_ngram_fwdflat_batch_device(psb_hmmctx_t *c, const psb_ngram_d
     const int N = c->n_emit;
     NgfFlat flat;
     std::string err;
-    if (ngf_flatten(g->info, g->model, (long long)g->model_len, g->lm_arrays, (long long)g->lm_arrays_len, g->ci_tmat, g->ci_ssid, c->h_sseq, c->n_sseq, N, c->n_tmat, c->n_sen, flat, err) != 0) {
+    if (ngf_flatten(g->info, g->model, (long long)g->model_len, g->lm_arrays, (long long)g->lm_arrays_len, g->ci_tmat, g->ci_ssid, c->h_sseq.data(), c->n_sseq, N, c->n_tmat, c->n_sen, flat, err) != 0) {
         psb_set_error("psb_ngram_fwdflat_batch_device: %s", err.c_str());
         return PSB_ERR_ARG;
     }
@@ -338,14 +340,15 @@ extern "C" int psb_ngram_fwdflat_batch_device(psb_hmmctx_t *c, const psb_ngram_d
     const size_t n_in = (size_t)n_utt * first_cap_per_utt * NGS_BP_ROW, n_bp = (size_t)n_utt * bp_cap_per_utt * NGS_BP_ROW,
                  n_bss = (size_t)n_utt * bss_cap_per_utt, n_idx = total_frames + (size_t)n_utt;
     int32_t *d_i = nullptr, *d_work = nullptr, *d_in = nullptr, *d_bp = nullptr, *d_bss = nullptr, *d_idx = nullptr;
-    cudaError_t e = srch_reserve(c, 0, ibuf.size(), &d_i);
-    if (e == cudaSuccess) e = srch_reserve(c, 1, work_words * (size_t)n_utt, &d_work);
-    if (e == cudaSuccess) e = srch_reserve(c, 2, n_in, &d_in);
-    if (e == cudaSuccess) e = srch_reserve(c, 3, n_bp, &d_bp);
-    if (e == cudaSuccess) e = srch_reserve(c, 4, n_bss, &d_bss);
-    if (e == cudaSuccess) e = srch_reserve(c, 5, n_idx, &d_idx);
+    rc = srch_reserve(c, 0, ibuf.size(), &d_i);
+    if (!rc) rc = srch_reserve(c, 1, work_words * (size_t)n_utt, &d_work);
+    if (!rc) rc = srch_reserve(c, 2, n_in, &d_in);
+    if (!rc) rc = srch_reserve(c, 3, n_bp, &d_bp);
+    if (!rc) rc = srch_reserve(c, 4, n_bss, &d_bss);
+    if (!rc) rc = srch_reserve(c, 5, n_idx, &d_idx);
+    if (rc) return rc;
     cudaStream_t st = c->stream;
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_i, ibuf.data(), ibuf.size() * 4, cudaMemcpyHostToDevice, st);
+    cudaError_t e = cudaMemcpyAsync(d_i, ibuf.data(), ibuf.size() * 4, cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess) e = cudaMemcpyAsync(d_in, bp_first, n_in * 4, cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess) e = cudaMemsetAsync(d_idx, 0, n_idx * 4, st);
     if (e == cudaSuccess) {
@@ -390,8 +393,8 @@ extern "C" int psb_ngram_two_pass_batch_device(psb_hmmctx_t *c, const psb_ngram_
     NgsFlat f1;
     NgfFlat f2;
     std::string err;
-    if (ngs_flatten(g->info, g->model, (long long)g->model_len, g->lm_arrays, (long long)g->lm_arrays_len, g->ci_tmat, c->h_sseq, c->n_sseq, N, c->n_tmat, c->n_sen, f1, err) != 0 ||
-        ngf_flatten(g->info, g->model, (long long)g->model_len, g->lm_arrays, (long long)g->lm_arrays_len, g->ci_tmat, g->ci_ssid, c->h_sseq, c->n_sseq, N, c->n_tmat, c->n_sen, f2, err) != 0) {
+    if (ngs_flatten(g->info, g->model, (long long)g->model_len, g->lm_arrays, (long long)g->lm_arrays_len, g->ci_tmat, c->h_sseq.data(), c->n_sseq, N, c->n_tmat, c->n_sen, f1, err) != 0 ||
+        ngf_flatten(g->info, g->model, (long long)g->model_len, g->lm_arrays, (long long)g->lm_arrays_len, g->ci_tmat, g->ci_ssid, c->h_sseq.data(), c->n_sseq, N, c->n_tmat, c->n_sen, f2, err) != 0) {
         psb_set_error("psb_ngram_two_pass_batch_device: %s", err.c_str());
         return PSB_ERR_ARG;
     }
@@ -410,16 +413,17 @@ extern "C" int psb_ngram_two_pass_batch_device(psb_hmmctx_t *c, const psb_ngram_
                  n_bp2 = (size_t)n_utt * bp_cap_per_utt * NGS_BP_ROW, n_bss2 = (size_t)n_utt * bss_cap_per_utt;
     int32_t *d_i = nullptr, *d_work = nullptr, *d_bp1 = nullptr, *d_bss1 = nullptr, *d_idx1 = nullptr, *d_bp2 = nullptr, *d_bss2 = nullptr,
             *d_idx2 = nullptr;
-    cudaError_t e = srch_reserve(c, 0, ibuf.size(), &d_i);
-    if (e == cudaSuccess) e = srch_reserve(c, 1, ww * (size_t)n_utt, &d_work);
-    if (e == cudaSuccess) e = srch_reserve(c, 2, n_bp1, &d_bp1);
-    if (e == cudaSuccess) e = srch_reserve(c, 3, n_bss1, &d_bss1);
-    if (e == cudaSuccess) e = srch_reserve(c, 4, n_idx, &d_idx1);
-    if (e == cudaSuccess) e = srch_reserve(c, 5, n_bp2, &d_bp2);
-    if (e == cudaSuccess) e = srch_reserve(c, 6, n_bss2, &d_bss2);
-    if (e == cudaSuccess) e = srch_reserve(c, 7, n_idx, &d_idx2);
+    rc = srch_reserve(c, 0, ibuf.size(), &d_i);
+    if (!rc) rc = srch_reserve(c, 1, ww * (size_t)n_utt, &d_work);
+    if (!rc) rc = srch_reserve(c, 2, n_bp1, &d_bp1);
+    if (!rc) rc = srch_reserve(c, 3, n_bss1, &d_bss1);
+    if (!rc) rc = srch_reserve(c, 4, n_idx, &d_idx1);
+    if (!rc) rc = srch_reserve(c, 5, n_bp2, &d_bp2);
+    if (!rc) rc = srch_reserve(c, 6, n_bss2, &d_bss2);
+    if (!rc) rc = srch_reserve(c, 7, n_idx, &d_idx2);
+    if (rc) return rc;
     cudaStream_t st = c->stream;
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_i, ibuf.data(), ibuf.size() * 4, cudaMemcpyHostToDevice, st);
+    cudaError_t e = cudaMemcpyAsync(d_i, ibuf.data(), ibuf.size() * 4, cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess) e = cudaMemsetAsync(d_idx1, 0, n_idx * 4, st);
     if (e == cudaSuccess) e = cudaMemsetAsync(d_idx2, 0, n_idx * 4, st);
     if (e == cudaSuccess) {
@@ -466,8 +470,9 @@ extern "C" int psb_selftest_block_scan(int device, int32_t *a, int32_t n, int32_
 {
     PSB_REQUIRE(a && total && n >= 0, "psb_selftest_block_scan: bad argument");
     PSB_CUDA(cudaSetDevice(device));
-    int32_t *d = nullptr;
-    PSB_CUDA(cudaMalloc((void **)&d, ((size_t)n + 2) * 4));
+    DevBuf<int32_t> d;
+    const int rc = d.reserve((size_t)n + 2);
+    if (rc) return rc;
     cudaError_t e = cudaMemcpy(d, a, (size_t)n * 4, cudaMemcpyHostToDevice);
     if (e == cudaSuccess) {
         exscan_selftest_kernel<<<1, NGS_THREADS>>>(d, n, d + n);
@@ -476,7 +481,6 @@ extern "C" int psb_selftest_block_scan(int device, int32_t *a, int32_t n, int32_
     }
     if (e == cudaSuccess) e = cudaMemcpy(a, d, (size_t)n * 4, cudaMemcpyDeviceToHost);
     if (e == cudaSuccess) e = cudaMemcpy(total, d + n, 8, cudaMemcpyDeviceToHost);
-    cudaFree(d);
     if (e != cudaSuccess) {
         psb_set_error("psb_selftest_block_scan: %s", cudaGetErrorString(e));
         return PSB_ERR_CUDA;

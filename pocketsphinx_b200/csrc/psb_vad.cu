@@ -43,21 +43,22 @@ struct psb_vad_s {
     int device;
     int mode, sample_rate, closest, frame_size, maxlen, start_frames, end_frames, warmup;
     double frame_length, window, ratio;
-    cudaStream_t stream;
-    cudaEvent_t ev[2];
-    int16_t *d_pcm; size_t pcm_cap;
-    int16_t *d_feat; size_t feat_cap;              // [frames][8]
-    int8_t *d_flags; size_t flags_cap;
-    int64_t *d_segs; size_t segs_cap;            // [frames][2]: a stream has at most one segment per frame
-    double *d_times; size_t times_cap;
-    int32_t *d_seg_n; size_t segn_cap;
-    int64_t *d_samp_off; size_t so_cap;
-    int32_t *d_frame_off; size_t fo_cap;
-    int32_t *d_chunk_off; size_t co_cap;
-    int32_t *d_chunk_stream; size_t cs_cap;
-    psb_vad_filt_t *d_st_start, *d_st_end[2]; size_t sts_cap, ste_cap[2];
-    unsigned long long *d_repairs;
-    int *d_changed, *h_changed;   // repair pass flag, device and pinned host copy
+    Stream stream;                // declared first: destroyed after the buffers below
+    Event ev[2];
+    DevBuf<int16_t> d_pcm;
+    DevBuf<int16_t> d_feat;       // [frames][8]
+    DevBuf<int8_t> d_flags;
+    DevBuf<int64_t> d_segs;       // [frames][2]: a stream has at most one segment per frame
+    DevBuf<double> d_times;
+    DevBuf<int32_t> d_seg_n;
+    DevBuf<int64_t> d_samp_off;
+    DevBuf<int32_t> d_frame_off;
+    DevBuf<int32_t> d_chunk_off;
+    DevBuf<int32_t> d_chunk_stream;
+    DevBuf<psb_vad_filt_t> d_st_start, d_st_end[2];
+    DevBuf<unsigned long long> d_repairs;
+    DevBuf<int> d_changed;        // repair pass flag, device and pinned host copy
+    HostBuf<int> h_changed;
     int64_t last_repairs, last_passes;
 };
 
@@ -221,19 +222,6 @@ __global__ void __launch_bounds__(GMM_WARPS * 32, 1) vad_gmm_kernel(const int16_
     }
 }
 
-template <typename T>
-int vgrow(T **p, size_t *cap, size_t need)
-{
-    need = std::max<size_t>(need, 1);
-    if (*cap >= need) return PSB_OK;
-    if (*p) cudaFree(*p);
-    *p = nullptr;
-    *cap = 0;
-    PSB_CUDA(cudaMalloc(p, need * sizeof(T)));
-    *cap = need;
-    return PSB_OK;
-}
-
 size_t feat_smem(int closest) { return (size_t)FEAT_THREADS * psb_vad_scratch_elems(closest) * sizeof(int16_t); }
 
 // Stage A + B over streams whose samples are at d_pcm; frame_off (host) is filled here.
@@ -254,14 +242,14 @@ int vad_run(psb_vad_t *v, const int16_t *d_pcm, const int64_t *samp_off, int32_t
         chunk_stream.insert(chunk_stream.end(), (size_t)nc, s);
     }
     const int32_t total = frame_off[n], n_chunks = chunk_off[n];
-    int rc = vgrow(&v->d_feat, &v->feat_cap, (size_t)total * 8);
-    if (!rc) rc = vgrow(&v->d_samp_off, &v->so_cap, (size_t)n + 1);
-    if (!rc) rc = vgrow(&v->d_frame_off, &v->fo_cap, (size_t)n + 1);
-    if (!rc) rc = vgrow(&v->d_chunk_off, &v->co_cap, (size_t)n + 1);
-    if (!rc) rc = vgrow(&v->d_chunk_stream, &v->cs_cap, (size_t)n_chunks);
-    if (!rc) rc = vgrow(&v->d_st_start, &v->sts_cap, (size_t)n_chunks);
-    if (!rc) rc = vgrow(&v->d_st_end[0], &v->ste_cap[0], (size_t)n_chunks);
-    if (!rc) rc = vgrow(&v->d_st_end[1], &v->ste_cap[1], (size_t)n_chunks);
+    int rc = v->d_feat.reserve(std::max<size_t>((size_t)total * 8, 1));
+    if (!rc) rc = v->d_samp_off.reserve((size_t)n + 1);
+    if (!rc) rc = v->d_frame_off.reserve((size_t)n + 1);
+    if (!rc) rc = v->d_chunk_off.reserve((size_t)n + 1);
+    if (!rc) rc = v->d_chunk_stream.reserve(std::max<size_t>((size_t)n_chunks, 1));
+    if (!rc) rc = v->d_st_start.reserve(std::max<size_t>((size_t)n_chunks, 1));
+    if (!rc) rc = v->d_st_end[0].reserve(std::max<size_t>((size_t)n_chunks, 1));
+    if (!rc) rc = v->d_st_end[1].reserve(std::max<size_t>((size_t)n_chunks, 1));
     if (rc) return rc;
     cudaStream_t st = v->stream;
     PSB_CUDA(cudaMemcpyAsync(v->d_samp_off, samp_off, ((size_t)n + 1) * 8, cudaMemcpyHostToDevice, st));
@@ -324,14 +312,6 @@ extern "C" void psb_vad_free(psb_vad_t *v)
 {
     if (!v) return;
     cudaSetDevice(v->device);
-    cudaFree(v->d_pcm); cudaFree(v->d_feat); cudaFree(v->d_flags); cudaFree(v->d_segs); cudaFree(v->d_times);
-    cudaFree(v->d_seg_n); cudaFree(v->d_samp_off); cudaFree(v->d_frame_off); cudaFree(v->d_chunk_off);
-    cudaFree(v->d_chunk_stream); cudaFree(v->d_st_start); cudaFree(v->d_st_end[0]); cudaFree(v->d_st_end[1]);
-    cudaFree(v->d_repairs); cudaFree(v->d_changed);
-    if (v->h_changed) cudaFreeHost(v->h_changed);
-    if (v->stream) cudaStreamDestroy(v->stream);
-    for (auto &e : v->ev)
-        if (e) cudaEventDestroy(e);
     delete v;
 }
 
@@ -367,7 +347,7 @@ extern "C" int psb_vad_create(const psb_vad_opts_t *o, int device, psb_vad_t **o
     PSB_REQUIRE(o->warmup >= -1, "psb_vad_create: warmup must be >= -1 (got %d)", o->warmup);
     PSB_REQUIRE(maxlen + 1 <= GMM_RING_MAX, "psb_vad_create: window of %d frames; at most %d are implemented", maxlen, GMM_RING_MAX - 1);
     PSB_CUDA(cudaSetDevice(device));
-    psb_vad_t *v = new psb_vad_t();
+    std::unique_ptr<psb_vad_t> v(new psb_vad_t());
     v->device = device;
     v->mode = o->mode, v->sample_rate = rate, v->closest = closest, v->frame_size = frame_size;
     v->frame_length = flen, v->window = window, v->ratio = ratio;
@@ -375,18 +355,18 @@ extern "C" int psb_vad_create(const psb_vad_opts_t *o, int device, psb_vad_t **o
     // default warm-up: the frames of 0.5 s of audio (a 0.2 s warm-up left 12 % of the 64-frame chunks of an hour of
     // speech and silence to repair at 10 ms frames; see DESIGN)
     v->warmup = o->warmup == 0 ? (int)ceil(0.5 / flen - 1e-9) : o->warmup < 0 ? 0 : o->warmup;
-    cudaError_t e = cudaStreamCreateWithFlags(&v->stream, cudaStreamNonBlocking);
-    if (e == cudaSuccess) e = cudaEventCreate(&v->ev[0]);
-    if (e == cudaSuccess) e = cudaEventCreate(&v->ev[1]);
-    if (e == cudaSuccess) e = cudaMalloc(&v->d_repairs, sizeof(unsigned long long));
-    if (e == cudaSuccess) e = cudaMalloc(&v->d_changed, sizeof(int));
-    if (e == cudaSuccess) e = cudaMallocHost(&v->h_changed, sizeof(int));
+    cudaError_t e = v->stream.create();
+    if (e == cudaSuccess) e = v->ev[0].create();
+    if (e == cudaSuccess) e = v->ev[1].create();
     if (e != cudaSuccess) {
         psb_set_error("psb_vad_create: %s", cudaGetErrorString(e));
-        psb_vad_free(v);
         return PSB_ERR_CUDA;
     }
-    *out = v;
+    int rc = v->d_repairs.reserve(1);
+    if (!rc) rc = v->d_changed.reserve(1);
+    if (!rc) rc = v->h_changed.reserve(1);
+    if (rc) return rc;
+    *out = v.release();
     return PSB_OK;
 }
 
@@ -423,11 +403,11 @@ extern "C" int psb_vad_process_host(psb_vad_t *v, const int16_t *pcm, const int6
     PSB_CUDA(cudaSetDevice(v->device));
     int64_t total = 0;
     for (int s = 0; s < n_streams; ++s) total += std::max<int64_t>(samp_off[s + 1] - samp_off[s], 0) / v->frame_size;
-    int rc = vgrow(&v->d_pcm, &v->pcm_cap, (size_t)ns);
-    if (!rc) rc = vgrow(&v->d_flags, &v->flags_cap, (size_t)total);
-    if (!rc) rc = vgrow(&v->d_seg_n, &v->segn_cap, (size_t)n_streams);
-    if (!rc) rc = vgrow(&v->d_segs, &v->segs_cap, (size_t)total * 2);
-    if (!rc) rc = vgrow(&v->d_times, &v->times_cap, (size_t)total * 2);
+    int rc = v->d_pcm.reserve(std::max<size_t>((size_t)ns, 1));
+    if (!rc) rc = v->d_flags.reserve(std::max<size_t>((size_t)total, 1));
+    if (!rc) rc = v->d_seg_n.reserve(std::max<size_t>((size_t)n_streams, 1));
+    if (!rc) rc = v->d_segs.reserve(std::max<size_t>((size_t)total * 2, 1));
+    if (!rc) rc = v->d_times.reserve(std::max<size_t>((size_t)total * 2, 1));
     if (rc) return rc;
     if (ns) PSB_CUDA(cudaMemcpyAsync(v->d_pcm, pcm, (size_t)ns * 2, cudaMemcpyHostToDevice, v->stream));
     rc = vad_run(v, v->d_pcm, samp_off, n_streams, v->d_flags, frame_off, v->d_seg_n, v->d_segs, v->d_times, nullptr);
