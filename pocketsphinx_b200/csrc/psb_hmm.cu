@@ -5,6 +5,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <type_traits>
 
 #include <vector>
 
@@ -492,7 +493,7 @@ extern "C" int psb_phoneloop_run_host(psb_phoneloop_t *p, const int16_t *senscr,
 // never reach the best score.
 constexpr int HS_V = 4;                     // instances per thread
 constexpr int HS_TS = 512;                  // storage tile: [tile][field][HS_TS], so a CTA's fields are one contiguous block
-constexpr int SWEEP_FR = 2;                 // hmmset_sweep_kernel: frames per block barrier (2 * SWEEP_FR score rows in flight)
+constexpr int SWEEP_FR = 4;                 // hmmset_sweep_kernel: frames per block barrier (2 * SWEEP_FR score rows in flight)
 // threads per CTA: 128 (default) or 256 (PSB_HMMSET_THREADS)
 
 struct psb_hmmset_s {
@@ -761,8 +762,11 @@ hmmset_eval_kernel(HmmSetDev s, HmmCtxDev c, const int16_t *__restrict__ senscr,
 // that nothing past the allocation is touched.  Per frame one warp max (REDUX) into a shared slot;
 // one block barrier per SWEEP_FR frames, after which warp 0 reduces the slots and issues one
 // atomicMax per frame and CTA into best[t][segment].  The 3-state step runs on per-instance
-// constants decoded before the frame loop (hmm_step_3st_dec).  Results are bit-identical
-// to n_frames calls of hmmset_eval_kernel (tests/test_gpu_parity.py).
+// constants decoded before the frame loop (hmm_step_3st_dec); a CTA's slots past the segment's
+// end carry transitions that keep them on the floor (hmm_tp3_padding).  Results are bit-identical
+// to n_frames calls of hmmset_eval_kernel (tests/test_gpu_parity.py).  The plain sweep runs
+// 512 threads x 4 instances, one CTA per SM; FRP, LIVE_TEST and FAST take other values only in
+// the build of tools/sweep_time.py, which times them against the library's.
 //
 // BEAM: the same sweep with the beam pruning of prune_channels between frames (ngram_search_fwdtree.c:1130-1181 and the
 // keep-or-hmm_clear decision of prune_nonroot_chan, :811, :823-827, :872-874, without the lexicon-tree transitions): an instance is active
@@ -797,8 +801,8 @@ __device__ __forceinline__ void cluster_sync_all()
     asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
-template <int NS, int V, int THREADS, bool BEAM>
-__global__ void __launch_bounds__(THREADS, BEAM ? 1 : 2)
+template <int NS, int V, int THREADS, bool BEAM, int FRP = SWEEP_FR, bool LIVE_TEST = (NS != 3), bool FAST = (NS == 3 && !BEAM)>
+__global__ void __launch_bounds__(THREADS, BEAM || THREADS >= 512 || V > 4 ? 1 : 512 / THREADS)
 hmmset_sweep_kernel(HmmSetDev s, HmmCtxDev c, const int16_t *__restrict__ senscr, long long rows_total,
                     const int64_t *__restrict__ row0, const int32_t *__restrict__ n_rows, int n_frames,
                     int32_t *__restrict__ best_out, int n_tmat, int buf_bytes, int frame0, int beam, int maxhmmpf,
@@ -807,7 +811,7 @@ hmmset_sweep_kernel(HmmSetDev s, HmmCtxDev c, const int16_t *__restrict__ senscr
     static_assert(!BEAM || THREADS == 256, "the histogram walk maps one bin to one thread");
     // frames per block barrier: FR for the plain sweep (its warps run FR frames apart at most and leave their per-frame
     // maxima in double-buffered slots), one under the beam, whose pruning needs every frame's segment maximum
-    constexpr int FR = BEAM ? 1 : SWEEP_FR;
+    constexpr int FR = BEAM ? 1 : FRP;
     // score rows in flight: 2 * FR for the plain sweep (the copies of the next FR frames run while the current FR are
     // evaluated), six under the beam, where a CTA whose instances have mostly left runs ahead of the copies (the floor
     // of the pruned sweep is the per-frame exchange, DESIGN 4.19)
@@ -878,7 +882,7 @@ hmmset_sweep_kernel(HmmSetDev s, HmmCtxDev c, const int16_t *__restrict__ senscr
     __syncthreads();                                      // the transition matrices are staged
     if (NS == 3) {
 #pragma unroll
-        for (int v = 0; v < V; ++v) tk[v] = hmm_tp3_decode(tps + tmo[v]);
+        for (int v = 0; v < V; ++v) tk[v] = live[v] ? hmm_tp3_decode(tps + tmo[v]) : hmm_tp3_padding();
     }
     const int64_t r0 = row0 ? row0[seg] : seg;
     const int64_t rstep = row0 ? 1 : gridDim.y;
@@ -929,6 +933,16 @@ hmmset_sweep_kernel(HmmSetDev s, HmmCtxDev c, const int16_t *__restrict__ senscr
         const unsigned char *srowb = reinterpret_cast<const unsigned char *>(srow);
         auto score_at = [&](int off) { return (int)*reinterpret_cast<const int16_t *>(srowb + off); };
         int best = PSB_WORST_SCORE, cnt = 0;
+        // FAST: when every instance of the warp evaluates its exit state this frame (state 1 above the floor: every
+        // frame but an instance's first few), the step runs without the selects that serve the other case
+        bool s1_live = false;
+        if (NS == 3 && FAST) {
+            bool all = true;
+#pragma unroll
+            for (int v = 0; v < V; ++v) all &= sc[v][1] - score_at(sid[v][1]) > PSB_WORST_SCORE;
+            s1_live = __all_sync(0xffffffffu, all);
+        }
+        auto frame_steps = [&](auto s1_known) {
 #pragma unroll
         for (int v = 0; v < V; ++v) {
             if (BEAM && !act[v]) continue;
@@ -937,7 +951,7 @@ hmmset_sweep_kernel(HmmSetDev s, HmmCtxDev c, const int16_t *__restrict__ senscr
             if (NS == 3) {
                 int (&s3)[3] = *reinterpret_cast<int (*)[3]>(sc[v]);
                 int (&h3)[3] = *reinterpret_cast<int (*)[3]>(hi[v]);
-                bb = hmm_step_3st_dec(s3, h3, osc[v], ohi[v], tk[v], score_at(sid[v][0]), score_at(sid[v][1]),
+                bb = hmm_step_3st_dec<decltype(s1_known)::value>(s3, h3, osc[v], ohi[v], tk[v], score_at(sid[v][0]), score_at(sid[v][1]),
                                       score_at(sid[v][NS > 2 ? 2 : 0]));
             }
             else {
@@ -956,9 +970,13 @@ hmmset_sweep_kernel(HmmSetDev s, HmmCtxDev c, const int16_t *__restrict__ senscr
                 for (int k = 0; k < NS; ++k) { sc[v][k] = h.score[k]; hi[v][k] = h.hist[k]; }
                 osc[v] = h.out_score; ohi[v] = h.out_hist;
             }
-            if (v * THREADS < rem) best = max(best, bb);                // live[v], one compare
+            // a 3-state padding slot stays at WORST_SCORE by its transitions (hmm_tp3_padding); 5-state: live[v], one compare
+            if (!LIVE_TEST || v * THREADS < rem) best = max(best, bb);
             best_final[v] = bb;
         }
+        };
+        if (NS == 3 && FAST && s1_live) frame_steps(std::true_type());
+        else frame_steps(std::false_type());
         best = __reduce_max_sync(0xffffffffu, best);
         if (BEAM) cnt = __reduce_add_sync(0xffffffffu, cnt);
         const int slot = t % (2 * FR);
@@ -1258,8 +1276,30 @@ extern "C" int psb_hmmset_eval_frames_device(psb_hmmset_t *s, const int16_t *d_s
     return PSB_OK;
 }
 
-extern "C" int psb_hmmset_sweep_device(psb_hmmset_t *s, const int16_t *d_senscr, int64_t rows_total, const int64_t *d_row0,
-                                       const int32_t *d_n_rows, int32_t n_frames, int32_t *d_best, float *ms)
+// One launch of the plain sweep in the given CTA shape, between the set's two events.
+template <int NS, int V, int THREADS, int FR, bool LIVE_TEST = (NS != 3), bool FAST = (NS == 3)>
+static int sweep_launch(psb_hmmset_t *s, const int16_t *d_senscr, int64_t rows_total, const int64_t *d_row0,
+                        const int32_t *d_n_rows, int32_t n_frames, int32_t *d_best)
+{
+    const HmmCtxDev cd = dev_ctx(s->c);
+    const int buf_bytes = (int)(((size_t)cd.n_sen * 2 + 32 + 127) & ~(size_t)127);
+    const int tp_bytes = s->c->n_tmat * NS * (NS + 1);
+    const size_t smem = 2 * FR * (size_t)buf_bytes + tp_bytes;                  // NBUF of the plain instantiation
+    PSB_REQUIRE(smem <= 200 * 1024, "psb_hmmset_sweep: %d senones / %d transition matrices do not fit shared memory", cd.n_sen, s->c->n_tmat);
+    auto kern = hmmset_sweep_kernel<NS, V, THREADS, false, FR, LIVE_TEST, FAST>;
+    PSB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const dim3 grid((unsigned)((s->max_seg_len + THREADS * V - 1) / (THREADS * V)), (unsigned)s->n_seg);
+    PSB_CUDA(cudaEventRecord(s->ev[0], s->stream));
+    kern<<<grid, THREADS, smem, s->stream>>>(dev_set(s), cd, d_senscr, (long long)rows_total, d_row0, d_n_rows, n_frames, d_best,
+                                            s->c->n_tmat, buf_bytes, 0, 0, -1, nullptr);
+    PSB_LAUNCH_CHECK();
+    PSB_CUDA(cudaEventRecord(s->ev[1], s->stream));
+    return PSB_OK;
+}
+
+// candidate 0 is the library's sweep; the others exist only in the build of tools/sweep_time.py (PSB_SWEEP_CANDIDATES)
+static int sweep_device(psb_hmmset_t *s, const int16_t *d_senscr, int64_t rows_total, const int64_t *d_row0,
+                        const int32_t *d_n_rows, int32_t n_frames, int32_t *d_best, int candidate, float *ms)
 {
     PSB_REQUIRE(s && d_senscr && d_best && n_frames >= 0 && rows_total > 0, "psb_hmmset_sweep_device: bad argument");
     const HmmCtxDev cd = dev_ctx(s->c);
@@ -1275,32 +1315,44 @@ extern "C" int psb_hmmset_sweep_device(psb_hmmset_t *s, const int16_t *d_senscr,
         if (ms) PSB_CUDA(cudaStreamSynchronize(s->stream));
         return PSB_OK;
     }
-    const int buf_bytes = (int)(((size_t)cd.n_sen * 2 + 32 + 127) & ~(size_t)127);
-    const int tp_bytes = s->c->n_tmat * cd.n_emit * (cd.n_emit + 1);
-    const size_t smem = 2 * SWEEP_FR * (size_t)buf_bytes + tp_bytes;            // NBUF of the plain instantiation
-    PSB_REQUIRE(smem <= 200 * 1024, "psb_hmmset_sweep: %d senones / %d transition matrices do not fit shared memory", cd.n_sen, s->c->n_tmat);
-    const HmmSetDev sd = dev_set(s);
-    PSB_CUDA(cudaEventRecord(s->ev[0], s->stream));
-#define PSB_SWEEP(NS, V, THREADS)                                                                                               \
-    do {                                                                                                                       \
-        auto kern = hmmset_sweep_kernel<NS, V, THREADS, false>;                                                                \
-        PSB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));                          \
-        const dim3 grid((unsigned)((s->max_seg_len + THREADS * V - 1) / (THREADS * V)), (unsigned)s->n_seg);                   \
-        kern<<<grid, THREADS, smem, s->stream>>>(sd, cd, d_senscr, (long long)rows_total, d_row0, d_n_rows, n_frames, d_best,  \
-                                                s->c->n_tmat, buf_bytes, 0, 0, -1, nullptr);                                   \
-    } while (0)
-    // one CTA shape, 256 threads x 4 instances (the beam sweep's; the shapes timed against it are in DESIGN 4.14)
-    if (cd.n_emit == 3) PSB_SWEEP(3, 4, 256);
-    else PSB_SWEEP(5, 4, 256);
-#undef PSB_SWEEP
-    PSB_LAUNCH_CHECK();
-    PSB_CUDA(cudaEventRecord(s->ev[1], s->stream));
+    int rc;
+    // one CTA shape, 512 threads x 4 instances: one CTA of 16 warps per SM, half the copies of a segment's score row
+    // that 256 x 4 (the beam sweep's shape) makes; the shapes timed against it are in DESIGN 4.14
+    if (cd.n_emit == 5) rc = sweep_launch<5, 4, 512, SWEEP_FR>(s, d_senscr, rows_total, d_row0, d_n_rows, n_frames, d_best);
+#ifdef PSB_SWEEP_CANDIDATES
+    else if (candidate == 1) rc = sweep_launch<3, 4, 256, 2>(s, d_senscr, rows_total, d_row0, d_n_rows, n_frames, d_best);
+    else if (candidate == 2) rc = sweep_launch<3, 4, 512, 1>(s, d_senscr, rows_total, d_row0, d_n_rows, n_frames, d_best);
+    else if (candidate == 3) rc = sweep_launch<3, 4, 512, 4, false, false>(s, d_senscr, rows_total, d_row0, d_n_rows, n_frames, d_best);
+    else if (candidate == 4) rc = sweep_launch<3, 4, 512, 8>(s, d_senscr, rows_total, d_row0, d_n_rows, n_frames, d_best);
+    else if (candidate == 5) rc = sweep_launch<3, 4, 256, 2, true, false>(s, d_senscr, rows_total, d_row0, d_n_rows, n_frames, d_best);
+    else if (candidate == 6) rc = sweep_launch<3, 4, 512, 2, true, false>(s, d_senscr, rows_total, d_row0, d_n_rows, n_frames, d_best);
+    else if (candidate == 7) rc = sweep_launch<3, 4, 512, 2>(s, d_senscr, rows_total, d_row0, d_n_rows, n_frames, d_best);
+    else if (candidate == 8) rc = sweep_launch<3, 4, 256, 4>(s, d_senscr, rows_total, d_row0, d_n_rows, n_frames, d_best);
+#endif
+    else rc = sweep_launch<3, 4, 512, SWEEP_FR>(s, d_senscr, rows_total, d_row0, d_n_rows, n_frames, d_best);
+    (void)candidate;
+    if (rc) return rc;
     if (ms) {                                               // ms == NULL: asynchronous on the set's stream
         PSB_CUDA(cudaStreamSynchronize(s->stream));
         PSB_CUDA(cudaEventElapsedTime(ms, s->ev[0], s->ev[1]));
     }
     return PSB_OK;
 }
+
+extern "C" int psb_hmmset_sweep_device(psb_hmmset_t *s, const int16_t *d_senscr, int64_t rows_total, const int64_t *d_row0,
+                                       const int32_t *d_n_rows, int32_t n_frames, int32_t *d_best, float *ms)
+{
+    return sweep_device(s, d_senscr, rows_total, d_row0, d_n_rows, n_frames, d_best, 0, ms);
+}
+
+#ifdef PSB_SWEEP_CANDIDATES
+extern "C" int psb_hmmset_sweep_candidate_device(psb_hmmset_t *s, const int16_t *d_senscr, int64_t rows_total, const int64_t *d_row0,
+                                                 const int32_t *d_n_rows, int32_t n_frames, int32_t *d_best, int32_t candidate,
+                                                 float *ms)
+{
+    return sweep_device(s, d_senscr, rows_total, d_row0, d_n_rows, n_frames, d_best, candidate, ms);
+}
+#endif
 
 // The fused sweep with beam pruning between frames: one thread-block cluster per segment (hmmset_sweep_kernel<.., BEAM>).
 extern "C" int psb_hmmset_sweep_beam_device(psb_hmmset_t *s, const int16_t *d_senscr, int64_t rows_total, const int64_t *d_row0,

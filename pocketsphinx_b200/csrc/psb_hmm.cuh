@@ -105,16 +105,30 @@ __device__ __forceinline__ HmmTp3 hmm_tp3_decode(const uint8_t *tp)
     return k;
 }
 
+// Transitions for a padding slot (scores at WORST_SCORE, any senone): every candidate falls below the floor whatever
+// int16 score the slot gathers (WORST - (-32768) + PAD stays under WORST), so the slot's best score is WORST_SCORE in
+// every frame and never shows in a maximum -- no per-frame "is this slot an instance" test.
+__device__ __forceinline__ HmmTp3 hmm_tp3_padding()
+{
+    constexpr int PAD = -0x100000;
+    HmmTp3 k;
+    k.p00 = k.p01 = k.p02 = k.p11 = k.p12 = k.p13 = k.p22 = k.p23 = PAD;
+    k.m02 = k.m13 = -1;
+    return k;
+}
+
 // (m ? a : b) for an all-ones / zero mask m: one LOP3
 __device__ __forceinline__ int hmm_msel(int m, int a, int b) { return (a & m) | (b & ~m); }
 
-// x_i = senscore of state i's senone (not negated); returns the instance's best score
+// x_i = senscore of state i's senone (not negated); returns the instance's best score.  S1_LIVE: the caller has
+// established sc[1] - x1 > WORST_SCORE (the exit state is evaluated), so the four selects on that test fold away.
+template <bool S1_LIVE = false>
 __device__ __forceinline__ int hmm_step_3st_dec(int (&sc)[3], int (&hi)[3], int &osc, int &ohi, const HmmTp3 &k,
                                                 int x0, int x1, int x2)
 {
     const int s2 = sc[2] - x2, s1 = sc[1] - x1, s0 = sc[0] - x0;
     // exit state, only when s1 > WORST (hmm.c:545-556)
-    const bool a = s1 > PSB_WORST_SCORE;
+    const bool a = S1_LIVE || s1 > PSB_WORST_SCORE;
     const int e1 = s2 + k.p23;
     const int e2 = hmm_msel(k.m13, s1 + k.p13, INT_MIN);
     const int s3 = max(max(e1, e2), PSB_WORST_SCORE);
