@@ -643,8 +643,8 @@ int psb_decode_batch_pcm_host(psb_batch_t *b, psb_fe_t *fe, psb_phoneloop_t *p, 
  * ps_endpointer_init(window, ratio, mode, sample_rate, frame_length) produces when
  * ps_endpointer_process is called on every full frame and ps_endpointer_end_stream once with the
  * remaining samples (0 <= r < frame size) -- also when r is 0, which the reference's Python
- * Segmenter skips.  Timestamp callbacks and state carried across calls are not implemented: every
- * call takes whole streams.
+ * Segmenter skips.  psb_vad_feed_* below carries the state of live streams from one call to the
+ * next.  Timestamp callbacks are not implemented.
  * Refused like ps_vad_set_input_params (ps_vad.c:91-127) and ps_endpointer_init
  * (ps_endpointer.c:63-116): a rate with no supported rate within 50 % (8/16/32/48 kHz), frames other
  * than 10/20/30 ms at that rate, mode outside 0..3, ratios whose start_frames or end_frames fall
@@ -686,6 +686,50 @@ int psb_vad_process_host(psb_vad_t *v, const int16_t *pcm, const int64_t *samp_o
 int psb_vad_process_device(psb_vad_t *v, const int16_t *d_pcm, const int64_t *samp_off, int32_t n_streams,
                            int8_t *d_flags, int32_t *frame_off, int32_t *d_seg_n, int64_t *d_segs, double *d_times,
                            float *ms);
+
+/* Live endpointing: the handle keeps n_slots streams on the device, each one ps_endpointer_t (with
+ * its VAD) fed one frame at a time as audio arrives.  A call feeds the next samples of any subset of
+ * slots, in any lengths; a slot's results are bit for bit the reference's when the same samples
+ * are given to ps_endpointer_process frame by frame across the same calls (the samples after the
+ * last full frame wait for the next call).  Whole-stream calls (psb_vad_process_*) on the same
+ * handle never read or change the slots.
+ * psb_vad_live_open: creates the slot table, or grows it; every slot starts fresh (ps_endpointer_init).
+ * psb_vad_live_reset: the listed slots start fresh.
+ * psb_vad_feed_*: fed slot i = slots[i] (host, each slot at most once per call) gets the samples
+ * pcm[samp_off[i] .. samp_off[i + 1] - 1] (host samp_off int64[n + 1], samp_off[0] = 0; zero
+ * samples is allowed).  final (host int8[n], may be NULL): where non-zero, ps_endpointer_end_stream
+ * runs after the slot's frames with the samples left after its last full frame, which are then
+ * dropped.  As in the reference, ending a stream resets neither the VAD nor the endpointer: a slot
+ * fed after a final call goes on like the same ps_endpointer_t fed on (reset it for a new stream).
+ * Outputs:
+ *   frame_off int32[n + 1] (host): fed slot i's new frames are frame_off[i] .. frame_off[i + 1] - 1;
+ *     at most sum over i of (samp_off[i + 1] - samp_off[i] + frame_size - 1) / frame_size frames;
+ *   flags int8[frames]: their decisions;
+ *   seg_n int32[n]: segments that ended in this call, rows frame_off[i] + i .. + seg_n[i] - 1 of
+ *     segs int64[frames + n][2] (first sample, one past the last) and times double[frames + n][2]
+ *     (ps_endpointer_speech_start / _speech_end).  Sample positions count the samples of the full
+ *     frames fed since the slot was made fresh, frame f starting at f * frame_size (a final call's
+ *     dropped samples are counted only by the segment it closes, as the reference returns them);
+ *   status[n]: the slot's state at the end of the call.
+ * Refused: feeding or resetting before psb_vad_live_open, a slot outside 0 .. n_slots - 1, a slot
+ * fed twice in one call, a slot taken past 2^31 - 1 frames.  _device: pcm, flags, seg_n, segs,
+ * times and status on the device, *ms (may be NULL) = device time of the call's kernels. */
+typedef struct psb_vad_live_status_s {
+    int32_t in_speech;            /* ps_endpointer_in_speech */
+    int32_t reserved;
+    int64_t start_sample;         /* first sample of the open segment, -1 when not in speech */
+    int64_t frames;               /* frames fed since the slot was made fresh */
+    double speech_start;          /* ps_endpointer_speech_start */
+    double speech_end;            /* ps_endpointer_speech_end */
+} psb_vad_live_status_t;
+int psb_vad_live_open(psb_vad_t *v, int32_t n_slots);
+int psb_vad_live_reset(psb_vad_t *v, const int32_t *slots, int32_t n);
+int psb_vad_feed_host(psb_vad_t *v, const int32_t *slots, int32_t n, const int16_t *pcm, const int64_t *samp_off,
+                      const int8_t *final, int8_t *flags, int32_t *frame_off, int32_t *seg_n, int64_t *segs,
+                      double *times, psb_vad_live_status_t *status);
+int psb_vad_feed_device(psb_vad_t *v, const int32_t *slots, int32_t n, const int16_t *d_pcm, const int64_t *samp_off,
+                        const int8_t *final, int8_t *d_flags, int32_t *frame_off, int32_t *d_seg_n, int64_t *d_segs,
+                        double *d_times, psb_vad_live_status_t *d_status, float *ms);
 
 /* number of kernels launched by this library in the calling process so far */
 int64_t psb_kernel_launch_count(void);

@@ -160,6 +160,10 @@ SYMBOLS = [
     ("psb_vad_last_passes", _I32, [_VP]),
     ("psb_vad_process_host", C.c_int, [_VP, _VP, _VP, _I32, _VP, _VP, _VP, _VP, _VP]),
     ("psb_vad_process_device", C.c_int, [_VP, _VP, _VP, _I32, _VP, _VP, _VP, _VP, _VP, C.POINTER(C.c_float)]),
+    ("psb_vad_live_open", C.c_int, [_VP, _I32]),
+    ("psb_vad_live_reset", C.c_int, [_VP, _VP, _I32]),
+    ("psb_vad_feed_host", C.c_int, [_VP, _VP, _I32, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP]),
+    ("psb_vad_feed_device", C.c_int, [_VP, _VP, _I32, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, C.POINTER(C.c_float)]),
     ("psb_kernel_launch_count", _I64, []),
     ("psb_device_bytes_live", _I64, []),
 ]

@@ -880,6 +880,72 @@ class Endpointer:
             self.h = None
 
 
+LIVE_STATUS = np.dtype([("in_speech", np.int32), ("reserved", np.int32), ("start_sample", np.int64), ("frames", np.int64),
+                        ("speech_start", np.float64), ("speech_end", np.float64)])     # psb_vad_live_status_t
+
+
+class LiveEndpointer(Endpointer):
+    """ps_endpointer_t for n_slots live streams on the device: feed() hands each listed slot its next samples, in any
+    lengths; the results are bit for bit the reference's when the same samples reach ps_endpointer_process one frame
+    at a time across the same calls.  Options as Endpointer's; the whole-stream calls of Endpointer on this handle
+    leave the slots alone."""
+
+    def __init__(self, n_slots, window=0.3, ratio=0.9, vad_mode=0, sample_rate=16000, frame_length=0.03, device=0,
+                 warmup=None):
+        super().__init__(window, ratio, vad_mode, sample_rate, frame_length, device, warmup)
+        try:
+            check(lib().psb_vad_live_open(self.h, int(n_slots)), "psb_vad_live_open")
+        except PsbError:
+            self.close()
+            raise
+        self.n_slots = int(n_slots)
+
+    def feed(self, chunks, slots=None, final=None):
+        """chunks: int16 arrays, one per slot in `slots` (default: slots 0 .. len(chunks) - 1).  final: per slot, true
+        to end the stream after these samples (ps_endpointer_end_stream; the samples after the last full frame are
+        dropped, and a slot fed afterwards goes on like the reference's endpointer does).  Returns one dict per fed slot:
+        flags (int8 per new frame), segments ended in this call [(start_time, end_time, start_sample, end_sample)],
+        in_speech, speech_start, speech_end, start_sample (of the open segment, -1 when not in speech), frames (fed
+        since the slot was made fresh)."""
+        chunks = [np.ascontiguousarray(c, np.int16) for c in chunks]
+        n = len(chunks)
+        slots = np.arange(n, dtype=np.int32) if slots is None else np.ascontiguousarray(slots, np.int32)
+        if len(slots) != n:
+            raise ValueError("feed: %d chunks for %d slots" % (n, len(slots)))
+        fin = None if final is None else np.ascontiguousarray([bool(f) for f in final], np.int8)
+        if fin is not None and len(fin) != n:
+            raise ValueError("feed: %d final flags for %d slots" % (len(fin), n))
+        samp_off = np.zeros(n + 1, np.int64)
+        samp_off[1:] = np.cumsum([len(c) for c in chunks])
+        pcm = np.concatenate(chunks) if n else np.zeros(0, np.int16)
+        cap = int(sum((len(c) + self.frame_size - 1) // self.frame_size for c in chunks))
+        flags = np.zeros(max(cap, 1), np.int8)
+        frame_off = np.zeros(n + 1, np.int32)
+        seg_n = np.zeros(max(n, 1), np.int32)
+        segs = np.zeros((cap + n + 1, 2), np.int64)
+        times = np.zeros((cap + n + 1, 2), np.float64)
+        status = np.zeros(max(n, 1), LIVE_STATUS)
+        check(lib().psb_vad_feed_host(self.h, _p(slots) if n else None, n, _p(pcm) if pcm.size else None, _p(samp_off),
+                                      _p(fin) if fin is not None else None, _p(flags), _p(frame_off), _p(seg_n), _p(segs),
+                                      _p(times), _p(status)), "psb_vad_feed_host")
+        out = []
+        for i in range(n):
+            r0 = int(frame_off[i]) + i
+            st = status[i]
+            out.append(dict(flags=flags[frame_off[i]:frame_off[i + 1]].copy(),
+                            segments=[(float(times[j, 0]), float(times[j, 1]), int(segs[j, 0]), int(segs[j, 1]))
+                                      for j in range(r0, r0 + int(seg_n[i]))],
+                            in_speech=bool(st["in_speech"]), speech_start=float(st["speech_start"]),
+                            speech_end=float(st["speech_end"]), start_sample=int(st["start_sample"]),
+                            frames=int(st["frames"])))
+        return out
+
+    def reset(self, slots):
+        """The listed slots start fresh streams (a new ps_endpointer_init)."""
+        slots = np.ascontiguousarray(slots, np.int32)
+        check(lib().psb_vad_live_reset(self.h, _p(slots) if len(slots) else None, len(slots)), "psb_vad_live_reset")
+
+
 class Vad(Endpointer):
     """ps_vad_t for whole batches (arguments as the reference's Python Vad: mode, sample_rate, frame_length):
     classify_batch(streams) gives ps_vad_classify's decision for every full frame of each stream."""

@@ -1,7 +1,7 @@
 // psb_vad_core.h -- the per-frame fixed-point arithmetic of the reference's voice activity
 // detector (PocketSphinx 5's WebRTC-derived VAD) and of its endpointer, as __host__ __device__
-// functions.  psb_vad.cu's kernels and tests/emul/vad_emul.cpp (the CPU restatement the tests pin
-// against the compiled reference) are built from this one file.
+// functions.  psb_vad.cu's kernels and tests/emul/vad_emul.cpp / vad_live_emul.cpp (the CPU
+// restatements the tests pin against the compiled reference) are built from this one file.
 //
 // Restated, in the reference's int16 / int32 types, truncations and wrap-arounds:
 //   WebRtcVad_Downsampling                                 (common_audio/vad/vad_sp.c:25-53)
@@ -582,13 +582,61 @@ PSB_VAD_HD int psb_ep_end_stream(psb_ep_t *e, const Flags &flags, int nsamp, psb
         e->speech_end = e->last_audio_timestamp;
         end += nsamp;
     }
+    // ep_clear: the rest of the queue is dropped without advancing qstart_time (the times of a stream that goes on
+    // lag by the dropped frames, as the reference's do), while frame numbers stay the stream's own
     e->n = 0;
     e->speech_count = 0;
+    e->head = e->pushed;
     seg->start = e->seg_start;
     seg->end = end;
     seg->start_time = e->speech_start;
     seg->end_time = e->speech_end;
     return 1;
+}
+
+// ---- live streams -----------------------------------------------------------------------------
+
+// Everything a ps_endpointer_t (and the ps_vad_t inside it) carries from one frame to the next,
+// except the decisions of its queue (a ring of maxlen + 1 int8 indexed by frame number, kept beside
+// the record) and the samples after the last full frame (fewer than frame_size, also kept beside
+// it).  A stream saved here after any frame and restored goes on exactly as if it had not stopped.
+struct psb_vad_slot_t {
+    psb_vad_filt_t filt;
+    int16_t nm[PSB_VAD_NCH][2], sm[PSB_VAD_NCH][2], ns[PSB_VAD_NCH][2], ss[PSB_VAD_NCH][2];
+    int16_t mean_value[PSB_VAD_NCH];
+    int16_t age[PSB_VAD_NCH][16], low[PSB_VAD_NCH][16];
+    int32_t frame_counter;
+    int16_t over_hang, num_of_speech;
+    psb_ep_t ep;
+};
+
+// the state of a fresh ps_endpointer_init
+PSB_VAD_HD void psb_vad_slot_init(psb_vad_slot_t *s, int maxlen, int start_frames, int end_frames, int frame_size,
+                                  int sample_rate)
+{
+    psb_vad_filt_init(&s->filt);
+    for (int ch = 0; ch < PSB_VAD_NCH; ++ch) {
+        psb_vad_chan_t c;
+        psb_vad_chan_init(&c, ch, s->age[ch], s->low[ch]);
+        for (int k = 0; k < 2; ++k) s->nm[ch][k] = c.nm[k], s->sm[ch][k] = c.sm[k], s->ns[ch][k] = c.ns[k], s->ss[ch][k] = c.ss[k];
+        s->mean_value[ch] = c.mean_value;
+    }
+    s->frame_counter = 0;
+    s->over_hang = s->num_of_speech = 0;
+    psb_ep_init(&s->ep, maxlen, start_frames, end_frames, frame_size, sample_rate);
+}
+
+// channel ch's adapted GMM into *c, whose constants psb_vad_chan_init has set
+PSB_VAD_HD void psb_vad_slot_load_chan(const psb_vad_slot_t *s, int ch, psb_vad_chan_t *c)
+{
+    for (int k = 0; k < 2; ++k) c->nm[k] = s->nm[ch][k], c->sm[k] = s->sm[ch][k], c->ns[k] = s->ns[ch][k], c->ss[k] = s->ss[ch][k];
+    c->mean_value = s->mean_value[ch];
+}
+
+PSB_VAD_HD void psb_vad_slot_store_chan(psb_vad_slot_t *s, int ch, const psb_vad_chan_t *c)
+{
+    for (int k = 0; k < 2; ++k) s->nm[ch][k] = c->nm[k], s->sm[ch][k] = c->sm[k], s->ns[ch][k] = c->ns[k], s->ss[ch][k] = c->ss[k];
+    s->mean_value[ch] = c->mean_value;
 }
 
 #endif  // PSB_VAD_CORE_H
