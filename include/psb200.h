@@ -610,7 +610,8 @@ typedef struct psb_fe_opts_s {
 int psb_fe_create_ex(const psb_fe_desc_t *d, const psb_fe_opts_t *o, int device, psb_fe_t **out);
 
 /* What a ps_decoder_t carries from one utterance to the next: the live-CMN state (cmn_t), the
- * dither generator (genrand.c) and the emax AGC estimate (agc_t).  ps_start_stream resets none. */
+ * dither generator (genrand.c) and the emax AGC estimate (agc_t).  ps_start_stream resets none of
+ * these; the one piece of per-stream state it does reset, the noise tracker, is psb_fe_noise_t. */
 typedef struct psb_fe_state_s {
     float cmn_mean[PSB_FE_MAX_CEP], cmn_sum[PSB_FE_MAX_CEP];
     int32_t cmn_nframe;
@@ -629,6 +630,27 @@ int psb_fe_state_init(const psb_fe_t *fe, psb_fe_state_t *s);
 int psb_fe_set_sessions(psb_fe_t *fe, const int32_t *sess_off, int32_t n_sess, const psb_fe_state_t *states_in);
 /* the sessions' states after the last process call (n_sess of them, in session order) */
 int psb_fe_get_states(const psb_fe_t *fe, psb_fe_state_t *states_out, int32_t n_sess);
+
+/* The noise tracker of -remove_noise (fe_noise.c noise_stats_t, float build) for filters 0 .. n_filt - 1;
+ * later entries are 0.  fe_init and ps_start_stream make it undefined (fe_reset_noisestats), and the
+ * next frame initialises it; fe_start_utt, ps_start_utt and ps_decode_raw leave it alone.  An undefined
+ * tracker's arrays are never read and are reported as 0. */
+#define PSB_FE_MAX_FILT 64
+typedef struct psb_fe_noise_s {
+    int32_t undefined;                     /* 1: the next frame initialises the tracker */
+    int32_t reserved;                      /* 0 */
+    double power[PSB_FE_MAX_FILT], noise[PSB_FE_MAX_FILT], floor[PSB_FE_MAX_FILT], peak[PSB_FE_MAX_FILT];
+} psb_fe_noise_t;
+/* Names the stream starts of the next psb_fe_process_* / psb_decode_batch_pcm_host call: start[u] = 1
+ * runs ps_start_stream before utterance u (in decode order), 0 continues the stream of the utterance
+ * before it in its session (psb_fe_set_sessions), or, for a session's first utterance, the session's
+ * incoming tracker noise_in[s] (NULL: undefined for every session, as after fe_init).  n_utt must be that
+ * call's utterance count and n_sess (read only with noise_in) its session count.  Without this call
+ * every utterance starts a stream.  With remove_noise off the flags change nothing. */
+int psb_fe_set_stream_starts(psb_fe_t *fe, const uint8_t *start, int32_t n_utt, const psb_fe_noise_t *noise_in,
+                             int32_t n_sess);
+/* the sessions' trackers after the last process call, which must have set stream starts */
+int psb_fe_get_noise_states(const psb_fe_t *fe, psb_fe_noise_t *noise_out, int32_t n_sess);
 /* From audio to phone-loop results in one call: front end, senone scores and Viterbi on the
  * device, features never leave it.  frame_off int32[n_utt + 1] (out) indexes best / pen / senscr
  * like utt_off of psb_decode_batch_host. */

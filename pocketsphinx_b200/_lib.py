@@ -49,6 +49,11 @@ class FeState(C.Structure):
                 ("agc_obs_frame", C.c_int32), ("agc_obs_utt", C.c_int32)]
 
 
+class FeNoise(C.Structure):
+    _fields_ = [("undefined", C.c_int32), ("reserved", C.c_int32), ("power", C.c_double * 64), ("noise", C.c_double * 64),
+                ("floor", C.c_double * 64), ("peak", C.c_double * 64)]
+
+
 class FsgDesc(C.Structure):
     _fields_ = [("n_pnode", C.c_int32), ("pnodes", C.c_void_p), ("n_state", C.c_int32), ("roots", C.c_void_p),
                 ("n_link", C.c_int32), ("links", C.c_void_p), ("nulloff", C.c_void_p), ("nullarc", C.c_void_p),
@@ -138,6 +143,8 @@ SYMBOLS = [
     ("psb_fe_state_init", C.c_int, [_VP, C.POINTER(FeState)]),
     ("psb_fe_set_sessions", C.c_int, [_VP, _VP, _I32, _VP]),
     ("psb_fe_get_states", C.c_int, [_VP, _VP, _I32]),
+    ("psb_fe_set_stream_starts", C.c_int, [_VP, _VP, _I32, _VP, _I32]),
+    ("psb_fe_get_noise_states", C.c_int, [_VP, _VP, _I32]),
     ("psb_phoneloop_create", C.c_int, [_VP, _I32, _VP, _VP, _I32, _I32, _I32, _I32, C.c_double, C.POINTER(_VP)]),
     ("psb_phoneloop_free", None, [_VP]),
     ("psb_phoneloop_run_device", C.c_int, [_VP, _VP, _VP, _I32, _VP, _VP, _VP, _VP]),

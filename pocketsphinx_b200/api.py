@@ -766,11 +766,36 @@ class FrontEnd:
         check(lib().psb_fe_get_states(self.h, arr, n_sess), "psb_fe_get_states")
         return [arr[i] for i in range(n_sess)]
 
-    def process_sessions(self, pcm, samp_off, sess_off, states=None, want_mfcc=False):
-        """process_host over named sessions; returns (feats, frame_off, outgoing states[, mfcc])."""
+    def set_stream_starts(self, starts, noise=None):
+        """Names the stream starts of the next process_* / Batch.decode_pcm_host call: starts[u] true runs
+        ps_start_stream before utterance u, false carries the noise tracker on from the utterance before it in its
+        session, or for a session's first utterance from noise[s] (FeNoise objects, one per session of that call;
+        None: a fresh tracker for every session).  Without this call every utterance starts a stream."""
+        from ._lib import FeNoise
+        starts = np.ascontiguousarray(np.asarray(starts, bool), np.uint8)
+        arr, n = None, 0
+        if noise is not None:
+            n = len(noise)
+            arr = (FeNoise * max(n, 1))(*noise)
+        check(lib().psb_fe_set_stream_starts(self.h, _p(starts) if starts.size else None, len(starts), arr, n),
+              "psb_fe_set_stream_starts")
+
+    def get_noise_states(self, n_sess):
+        """The sessions' noise trackers after the last call, which must have set stream starts, as a list of FeNoise."""
+        from ._lib import FeNoise
+        arr = (FeNoise * max(n_sess, 1))()
+        check(lib().psb_fe_get_noise_states(self.h, arr, n_sess), "psb_fe_get_noise_states")
+        return [arr[i] for i in range(n_sess)]
+
+    def process_sessions(self, pcm, samp_off, sess_off, states=None, want_mfcc=False, starts=None, noise=None):
+        """process_host over named sessions; returns (feats, frame_off, outgoing states[, mfcc]).  With starts (one
+        flag per utterance, set_stream_starts) the outgoing noise trackers follow as one more item at the end."""
         self.set_sessions(sess_off, states)
+        if starts is not None:
+            self.set_stream_starts(starts, noise)
         r = self.process_host(pcm, samp_off, want_mfcc)
-        return r[:2] + (self.get_states(len(sess_off) - 1),) + r[2:]
+        r = r[:2] + (self.get_states(len(sess_off) - 1),) + r[2:]
+        return r + (self.get_noise_states(len(sess_off) - 1),) if starts is not None else r
 
     def n_frames(self, n_samples):
         return lib().psb_fe_n_frames(self.h, int(n_samples))

@@ -1,6 +1,7 @@
 // psb_fe.cu -- batched front end on the device (SURVEY 8 row f-2): int16 PCM -> MFCC -> CMN ->
 // dynamic features, for whole batches of utterances, each treated as a fresh stream
-// (ps_start_stream + ps_process_raw(full_utt), pocketsphinx.c:1073, acmod.c:528-560).
+// (ps_start_stream + ps_process_raw(full_utt), pocketsphinx.c:1073, acmod.c:528-560) unless
+// psb_fe_set_stream_starts carries the noise tracker from one utterance of a session to the next.
 //
 // Restates, operation for operation and in the reference's float32/float64 types and order:
 //   fe_pre_emphasis_int16 / fe_hamming_window / fe_spch_to_frame     (fe_sigproc.c:726-853)
@@ -60,11 +61,18 @@ struct psb_fe_s {
     DevBuf<int64_t> d_draw;                   // per utterance: first tail sample, tail offset, main draws, tail draws
     DevBuf<int16_t> d_dpcm;                   // dithered samples of the full frames
     DevBuf<int16_t> d_tail;                   // freshly dithered samples of each utterance's last frame
+    // psb_fe_set_stream_starts, for the next call only
+    std::vector<uint8_t> starts;              // per utterance: 1 = ps_start_stream before it
+    std::vector<psb_fe_noise_t> noise;        // in: the next call's trackers (empty: undefined); out: after it
+    bool starts_pending, noise_out;           // noise_out: the last call set stream starts, noise holds its trackers
+    DevBuf<psb_fe_noise_t> d_noise;           // [2][n_sess]: in, then out
+    DevBuf<int4> d_chain;
 };
 
 namespace {
 
 constexpr int FE_MAX_FILT = 64;
+static_assert(FE_MAX_FILT == PSB_FE_MAX_FILT, "psb_fe_noise_t holds one entry per filter");
 constexpr int FE_MAX_CEP = 32;
 
 struct FeDev {
@@ -206,6 +214,55 @@ fe_frame_kernel(FeDev p, const int16_t *__restrict__ pcm, const int64_t *__restr
     }
 }
 
+// fe_remove_noise (fe_noise.c:270-364, float build) for one filter of one frame: the tracker's
+// smoothers (power, noise, floor_, peak), and the gain (fe_noise_gain) and its +-4-filter smoothing
+// (fe_noise_smooth) in two steps, since the smoothing reads the neighbours' gains.
+// INIT: noise_stats->undefined (:290-305).
+__device__ __forceinline__ double fe_noise_gain(double &power, double &noise, double &floor_, double &peak, double mval,
+                                                bool init)
+{
+    // fe_noise.c constants (:64-75, :214-227)
+    const double lambda_power = 0.7, comp_lambda_power = 1 - 0.7, lambda_a = 0.995, comp_lambda_a = 1 - 0.995,
+                 lambda_b = 0.5, comp_lambda_b = 1 - 0.5, lambda_t = 0.85, mu_t = 0.2, max_gain = 20,
+                 inv_max_gain = 1.0 / 20;
+    if (init) {
+        power = mval;
+        noise = mval / max_gain;
+        floor_ = mval / max_gain;
+        peak = 0.0;
+    }
+    power = lambda_power * power + comp_lambda_power * mval;
+    // fe_lower_envelope(power -> noise)
+    if (power >= noise) noise = lambda_a * noise + comp_lambda_a * power;
+    else noise = lambda_b * noise + comp_lambda_b * power;
+    double signal = power - noise;
+    if (signal < 1.0) signal = 1.0;
+    // fe_lower_envelope(signal -> floor)
+    if (signal >= floor_) floor_ = lambda_a * floor_ + comp_lambda_a * signal;
+    else floor_ = lambda_b * floor_ + comp_lambda_b * signal;
+    // fe_temp_masking
+    const double cur_in = signal;
+    peak *= lambda_t;
+    if (signal < lambda_t * peak) signal = peak * mu_t;
+    if (cur_in > peak) peak = cur_in;
+    if (signal < floor_) signal = floor_;
+    double g;
+    if (signal < max_gain * power) g = signal / power;
+    else g = max_gain;
+    if (g < inv_max_gain) g = inv_max_gain;
+    return g;
+}
+
+// fe_weight_smooth, window of +-4 filters: filter tid's value after noise removal
+__device__ __forceinline__ double fe_noise_smooth(const double *gain, int tid, int nf, double mval)
+{
+    const int l1 = (tid - 4) > 0 ? (tid - 4) : 0;
+    const int l2 = (tid + 4) < (nf - 1) ? (tid + 4) : (nf - 1);
+    double coef = 0;
+    for (int j = l1; j <= l2; ++j) coef += gain[j];
+    return mval * (coef / (l2 - l1 + 1));
+}
+
 // One CTA (64 threads) per utterance: noise removal (sequential over frames), log, cepstral
 // transform, lifter; then batch CMN (VARNORM: with variance normalisation); then the dynamic features.
 template <bool VARNORM>
@@ -219,52 +276,14 @@ fe_utt_kernel(FeDev p, const int32_t *__restrict__ frame_off, double *__restrict
     const int f0 = frame_off[u], T = frame_off[u + 1] - f0;
     if (T <= 0) return;
     const int nf = p.n_filt, nc = p.n_cep;
-    // fe_noise.c constants (:64-75, :214-227)
-    const double lambda_power = 0.7, comp_lambda_power = 1 - 0.7, lambda_a = 0.995, comp_lambda_a = 1 - 0.995,
-                 lambda_b = 0.5, comp_lambda_b = 1 - 0.5, lambda_t = 0.85, mu_t = 0.2, max_gain = 20,
-                 inv_max_gain = 1.0 / 20;
     double power = 0, noise = 0, floor_ = 0, peak = 0;
     for (int t = 0; t < T; ++t) {
         const size_t fr = (size_t)(f0 + t);
         double mval = tid < nf ? mfspec[fr * nf + tid] : 0.0;
         if (p.remove_noise) {
-            if (tid < nf) {
-                if (t == 0) {                                            // noise_stats->undefined (:290-305)
-                    power = mval;
-                    noise = mval / max_gain;
-                    floor_ = mval / max_gain;
-                    peak = 0.0;
-                }
-                power = lambda_power * power + comp_lambda_power * mval;
-                // fe_lower_envelope(power -> noise)
-                if (power >= noise) noise = lambda_a * noise + comp_lambda_a * power;
-                else noise = lambda_b * noise + comp_lambda_b * power;
-                double signal = power - noise;
-                if (signal < 1.0) signal = 1.0;
-                // fe_lower_envelope(signal -> floor)
-                if (signal >= floor_) floor_ = lambda_a * floor_ + comp_lambda_a * signal;
-                else floor_ = lambda_b * floor_ + comp_lambda_b * signal;
-                // fe_temp_masking
-                const double cur_in = signal;
-                peak *= lambda_t;
-                if (signal < lambda_t * peak) signal = peak * mu_t;
-                if (cur_in > peak) peak = cur_in;
-                if (signal < floor_) signal = floor_;
-                double g;
-                if (signal < max_gain * power) g = signal / power;
-                else g = max_gain;
-                if (g < inv_max_gain) g = inv_max_gain;
-                gain[tid] = g;
-            }
+            if (tid < nf) gain[tid] = fe_noise_gain(power, noise, floor_, peak, mval, t == 0);
             __syncthreads();
-            if (tid < nf) {
-                // fe_weight_smooth, window of +-4 filters
-                const int l1 = (tid - 4) > 0 ? (tid - 4) : 0;
-                const int l2 = (tid + 4) < (nf - 1) ? (tid + 4) : (nf - 1);
-                double coef = 0;
-                for (int j = l1; j <= l2; ++j) coef += gain[j];
-                mval = mval * (coef / (l2 - l1 + 1));
-            }
+            if (tid < nf) mval = fe_noise_smooth(gain, tid, nf, mval);
         }
         if (tid < nf) lm[tid] = log(mval + 1e-4);                        // fe_mel_cep, LOG_FLOOR
         __syncthreads();
@@ -362,6 +381,66 @@ fe_utt_kernel(FeDev p, const int32_t *__restrict__ frame_off, double *__restrict
             o[2 * nc + c] = __fsub_rn(d1, d2);
 #undef CEP
         }
+    }
+}
+
+// The noise tracker carried across utterances (ps_start_stream only where a stream starts), in place
+// on the mel spectra before fe_utt_kernel, which then runs without its own noise removal.  One CTA per
+// chain: a chain is utterances chain.x .. chain.y - 1 of one session, whose frames are consecutive, with
+// no stream start after its first utterance.  It starts from in[chain.z] (chain.z < 0: a stream start,
+// noise_stats->undefined) and stores its tracker in out[chain.w] (chain.w < 0: a later chain of the
+// session has the session's last state).  A stored tracker that is still undefined has zero arrays, so
+// the bytes do not depend on how a session is cut into calls.
+// Only the four smoothers are a recurrence over frames.  The chain is walked in runs of FE_NOISE_RUN
+// frames: the run's spectra are staged in shared memory by all threads, one thread per filter runs the
+// recurrence and each frame's gain through the run, then all threads smooth the gains and write the run.
+constexpr int FE_NOISE_RUN = 32, FE_NOISE_THREADS = 128;
+
+__global__ void __launch_bounds__(FE_NOISE_THREADS)
+fe_noise_kernel(int nf, const int32_t *__restrict__ frame_off, const int4 *__restrict__ chain,
+                const psb_fe_noise_t *__restrict__ in, psb_fe_noise_t *__restrict__ out, double *__restrict__ mfspec)
+{
+    __shared__ double ms[FE_NOISE_RUN * FE_MAX_FILT], gain[FE_NOISE_RUN][FE_MAX_FILT];
+    const int4 c = chain[blockIdx.x];
+    const int tid = threadIdx.x;
+    const bool on = tid < nf;
+    double power = 0, noise = 0, floor_ = 0, peak = 0;
+    bool undef = true;
+    if (c.z >= 0) {
+        const psb_fe_noise_t *i = in + c.z;
+        undef = i->undefined != 0;
+        if (on && !undef) { power = i->power[tid]; noise = i->noise[tid]; floor_ = i->floor[tid]; peak = i->peak[tid]; }
+    }
+    const int f0 = frame_off[c.x], f1 = frame_off[c.y];
+    for (int r0 = f0; r0 < f1; r0 += FE_NOISE_RUN) {
+        const int n = min(FE_NOISE_RUN, f1 - r0);
+        double *run = mfspec + (size_t)r0 * nf;
+        for (int i = tid; i < n * nf; i += blockDim.x) ms[i] = run[i];
+        __syncthreads();
+        if (on)
+            for (int k = 0; k < n; ++k) {
+                gain[k][tid] = fe_noise_gain(power, noise, floor_, peak, ms[k * nf + tid], undef);
+                undef = false;
+            }
+        undef = false;
+        __syncthreads();
+        for (int i = tid; i < n * nf; i += blockDim.x) {
+            const int k = i / nf;
+            run[i] = fe_noise_smooth(gain[k], i - k * nf, nf, ms[i]);
+        }
+        __syncthreads();
+    }
+    if (c.w >= 0) {
+        psb_fe_noise_t *o = out + c.w;
+        if (tid == 0) { o->undefined = undef; o->reserved = 0; }
+        if (on) {
+            o->power[tid] = undef ? 0.0 : power;
+            o->noise[tid] = undef ? 0.0 : noise;
+            o->floor[tid] = undef ? 0.0 : floor_;
+            o->peak[tid] = undef ? 0.0 : peak;
+        }
+        for (int i = nf + tid; i < FE_MAX_FILT; i += blockDim.x)
+            o->power[i] = o->noise[i] = o->floor[i] = o->peak[i] = 0.0;
     }
 }
 
@@ -773,12 +852,21 @@ static void state_init(const psb_fe_t *fe, psb_fe_state_t *s)
     s->agc_max = fe->cmn != PSB_CMN_NONE ? 5.f : 10.f;                 // feat_init's agc_emax_set (feat.c:879)
 }
 
+// what fe_init and ps_start_stream leave (fe_reset_noisestats): the next frame initialises the tracker
+static psb_fe_noise_t noise_undefined()
+{
+    psb_fe_noise_t z;
+    memset(&z, 0, sizeof(z));
+    z.undefined = 1;
+    return z;
+}
+
 static int fe_run(psb_fe_t *fe, const int16_t *d_pcm, const int64_t *samp_off, int32_t n_utt, float *d_feats,
                   float *d_mfcc_out, int32_t *frame_off, float *ms)
 {
     // sessions: the ones psb_fe_set_sessions named for this call, else one per utterance
-    const bool pending = fe->sess_pending;
-    fe->sess_pending = false;
+    const bool pending = fe->sess_pending, carry = fe->starts_pending;
+    fe->sess_pending = fe->starts_pending = fe->noise_out = false;
     if (pending) {
         PSB_REQUIRE(fe->sess_off.back() == n_utt, "psb_fe: the sessions cover %d utterances, the call has %d", fe->sess_off.back(), n_utt);
     }
@@ -793,6 +881,29 @@ static int fe_run(psb_fe_t *fe, const int16_t *d_pcm, const int64_t *samp_off, i
         fe->states.resize((size_t)n_sess);
         for (auto &st : fe->states) state_init(fe, &st);
     }
+    // stream starts: the ones psb_fe_set_stream_starts named for this call, else one before every utterance.
+    // noise_next: each session's tracker where none of its frames changes it -- the incoming one, undefined
+    // after a stream start; fe_noise_kernel overwrites the sessions whose frames it walks.
+    std::vector<int4> chains;
+    std::vector<psb_fe_noise_t> noise_next;
+    if (carry) {
+        PSB_REQUIRE(fe->starts.size() == (size_t)n_utt, "psb_fe: the stream starts cover %d utterances, the call has %d",
+                    (int)fe->starts.size(), n_utt);
+        PSB_REQUIRE(fe->noise.empty() || fe->noise.size() == (size_t)n_sess, "psb_fe: %d noise trackers for %d sessions",
+                    (int)fe->noise.size(), n_sess);
+        if (fe->noise.empty()) fe->noise.resize((size_t)n_sess, noise_undefined());
+        noise_next = fe->noise;
+        for (int s = 0; s < n_sess; ++s) {
+            const int u0 = fe->sess_off[(size_t)s], u1 = fe->sess_off[(size_t)s + 1];
+            for (int u = u0; u < u1; ++u) {
+                if (fe->starts[(size_t)u]) noise_next[(size_t)s] = noise_undefined();
+                if (u == u0 || fe->starts[(size_t)u]) chains.push_back(make_int4(u, u + 1, u == u0 && !fe->starts[(size_t)u] ? s : -1, -1));
+                else chains.back().y = u + 1;
+            }
+            if (u1 > u0) chains.back().w = s;
+        }
+        if (!fe->remove_noise) chains.clear();
+    }
     std::vector<int32_t> foff((size_t)n_utt + 1);
     foff[0] = 0;
     for (int u = 0; u < n_utt; ++u) {
@@ -804,6 +915,9 @@ static int fe_run(psb_fe_t *fe, const int16_t *d_pcm, const int64_t *samp_off, i
     const int32_t total = foff[(size_t)n_utt];
     if (frame_off) memcpy(frame_off, foff.data(), foff.size() * sizeof(int32_t));
     if (ms) *ms = 0.f;
+    if (total == 0) chains.clear();
+    if (chains.empty()) fe->noise.swap(noise_next);
+    fe->noise_out = carry && chains.empty();
     // live CMN and emax AGC update their state even after an utterance without frames (cmn_live_update,
     // agc_emax_update)
     if (total == 0 && !((live || emax) && n_sess > 0)) return PSB_OK;
@@ -841,6 +955,10 @@ static int fe_run(psb_fe_t *fe, const int16_t *d_pcm, const int64_t *samp_off, i
         if (!rc) rc = grow(fe->d_state, (size_t)n_sess);
         if (!rc) rc = grow(fe->d_sess_off, (size_t)n_sess + 1);
     }
+    if (!chains.empty()) {
+        if (!rc) rc = grow(fe->d_noise, 2 * (size_t)n_sess);
+        if (!rc) rc = grow(fe->d_chain, chains.size());
+    }
     if (rc) return rc;
     PSB_CUDA(cudaMemcpyAsync(fe->d_samp_off, samp_off, ((size_t)n_utt + 1) * 8, cudaMemcpyHostToDevice, fe->stream));
     PSB_CUDA(cudaMemcpyAsync(fe->d_frame_off, foff.data(), foff.size() * 4, cudaMemcpyHostToDevice, fe->stream));
@@ -850,7 +968,16 @@ static int fe_run(psb_fe_t *fe, const int16_t *d_pcm, const int64_t *samp_off, i
         PSB_CUDA(cudaMemcpyAsync(fe->d_state, fe->states.data(), (size_t)n_sess * sizeof(psb_fe_state_t), cudaMemcpyHostToDevice, fe->stream));
         PSB_CUDA(cudaMemcpyAsync(fe->d_sess_off, fe->sess_off.data(), ((size_t)n_sess + 1) * 4, cudaMemcpyHostToDevice, fe->stream));
     }
+    const size_t noise_bytes = (size_t)n_sess * sizeof(psb_fe_noise_t);
+    if (!chains.empty()) {
+        PSB_CUDA(cudaMemcpyAsync(fe->d_noise, fe->noise.data(), noise_bytes, cudaMemcpyHostToDevice, fe->stream));
+        PSB_CUDA(cudaMemcpyAsync(fe->d_noise.get() + n_sess, noise_next.data(), noise_bytes, cudaMemcpyHostToDevice, fe->stream));
+        PSB_CUDA(cudaMemcpyAsync(fe->d_chain, chains.data(), chains.size() * sizeof(int4), cudaMemcpyHostToDevice, fe->stream));
+    }
     const FeDev p = dev_fe(fe);
+    // with the noise tracker carried, fe_noise_kernel removes the noise and fe_utt_kernel does not
+    FeDev pu = p;
+    if (!chains.empty()) pu.remove_noise = 0;
     const size_t smem = ((size_t)fe->fft_size + fe->fft_size / 2 + 1) * sizeof(double);
     // the features of 1s_c_d_dd without live CMN, AGC or LDA come out of fe_utt_kernel; every other
     // configuration normalises and builds them in the kernels behind it
@@ -869,11 +996,16 @@ static int fe_run(psb_fe_t *fe, const int16_t *d_pcm, const int64_t *samp_off, i
             fe_frame_kernel<false><<<(unsigned)total, 128, smem, fe->stream>>>(p, d_pcm, fe->d_samp_off, fe->d_frame_off,
                                                                              fe->d_frame_utt, fe->d_mfspec, nullptr, nullptr);
         PSB_LAUNCH_CHECK();
+        if (!chains.empty()) {
+            fe_noise_kernel<<<(unsigned)chains.size(), FE_NOISE_THREADS, 0, fe->stream>>>(
+                fe->n_filt, fe->d_frame_off, fe->d_chain, fe->d_noise, fe->d_noise.get() + n_sess, fe->d_mfspec);
+            PSB_LAUNCH_CHECK();
+        }
         if (fe->varnorm)
-            fe_utt_kernel<true><<<(unsigned)n_utt, 64, 0, fe->stream>>>(p, fe->d_frame_off, fe->d_mfspec, fe->d_mfcc,
+            fe_utt_kernel<true><<<(unsigned)n_utt, 64, 0, fe->stream>>>(pu, fe->d_frame_off, fe->d_mfspec, fe->d_mfcc,
                                                                        utt_feats ? d_feats : nullptr, fe->cmn, fe->window);
         else
-            fe_utt_kernel<false><<<(unsigned)n_utt, 64, 0, fe->stream>>>(p, fe->d_frame_off, fe->d_mfspec, fe->d_mfcc,
+            fe_utt_kernel<false><<<(unsigned)n_utt, 64, 0, fe->stream>>>(pu, fe->d_frame_off, fe->d_mfspec, fe->d_mfcc,
                                                                         utt_feats ? d_feats : nullptr, live ? 0 : fe->cmn, fe->window);
         PSB_LAUNCH_CHECK();
     }
@@ -913,7 +1045,10 @@ static int fe_run(psb_fe_t *fe, const int16_t *d_pcm, const int64_t *samp_off, i
         PSB_CUDA(cudaMemcpyAsync(d_mfcc_out, fe->d_mfcc, (size_t)total * fe->n_cep * 4, cudaMemcpyDeviceToDevice, fe->stream));
     if (stateful)
         PSB_CUDA(cudaMemcpyAsync(fe->states.data(), fe->d_state, (size_t)n_sess * sizeof(psb_fe_state_t), cudaMemcpyDeviceToHost, fe->stream));
+    if (!chains.empty())
+        PSB_CUDA(cudaMemcpyAsync(fe->noise.data(), fe->d_noise.get() + n_sess, noise_bytes, cudaMemcpyDeviceToHost, fe->stream));
     PSB_CUDA(cudaStreamSynchronize(fe->stream));
+    fe->noise_out = carry;
     if (ms) PSB_CUDA(cudaEventElapsedTime(ms, fe->ev[0], fe->ev[1]));
     return PSB_OK;
 }
@@ -991,5 +1126,35 @@ extern "C" int psb_fe_get_states(const psb_fe_t *fe, psb_fe_state_t *states_out,
         if (fe->states.empty()) state_init(fe, &states_out[s]);     // nothing carried: the state is the initial one
         else states_out[s] = fe->states[(size_t)s];
     }
+    return PSB_OK;
+}
+
+extern "C" int psb_fe_set_stream_starts(psb_fe_t *fe, const uint8_t *start, int32_t n_utt, const psb_fe_noise_t *noise_in,
+                                        int32_t n_sess)
+{
+    PSB_REQUIRE(fe && n_utt >= 0 && (start || n_utt == 0) && (!noise_in || n_sess >= 0), "psb_fe_set_stream_starts: bad argument");
+    for (int u = 0; u < n_utt; ++u)
+        PSB_REQUIRE(start[u] <= 1, "psb_fe_set_stream_starts: start[%d] is %d, not 0 or 1", u, start[u]);
+    if (noise_in)
+        for (int s = 0; s < n_sess; ++s)
+            PSB_REQUIRE(noise_in[s].undefined == 0 || noise_in[s].undefined == 1,
+                        "psb_fe_set_stream_starts: tracker %d is not a noise tracker (undefined = %d)", s, noise_in[s].undefined);
+    fe->starts.assign(start, start + n_utt);
+    fe->noise.clear();
+    if (noise_in) {
+        fe->noise.assign(noise_in, noise_in + n_sess);
+        for (auto &z : fe->noise)                       // an undefined tracker's arrays are never read
+            if (z.undefined) z = noise_undefined();
+    }
+    fe->starts_pending = true;
+    return PSB_OK;
+}
+
+extern "C" int psb_fe_get_noise_states(const psb_fe_t *fe, psb_fe_noise_t *noise_out, int32_t n_sess)
+{
+    PSB_REQUIRE(fe && noise_out && n_sess >= 0, "psb_fe_get_noise_states: bad argument");
+    PSB_REQUIRE(fe->noise_out, "psb_fe_get_noise_states: the last process call set no stream starts");
+    PSB_REQUIRE(n_sess == (int32_t)fe->noise.size(), "psb_fe_get_noise_states: the last call had %d sessions", (int)fe->noise.size());
+    memcpy(noise_out, fe->noise.data(), (size_t)n_sess * sizeof(psb_fe_noise_t));
     return PSB_OK;
 }

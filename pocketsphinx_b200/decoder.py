@@ -94,11 +94,18 @@ class Decoder:
         self.sample_rate = int(float(fp["samprate"]))
         self.max_utts = max_utts
 
-    def decode_raw_batch(self, utterances, sessions=None):
+    def decode_raw_batch(self, utterances, sessions=None, start_stream="utterance"):
         """utterances: int16 arrays, each a whole utterance.  sessions: None (every utterance a fresh decoder) or one
         session id per utterance; the utterances of one id are one decoder's, in list order, from a fresh decoder
-        (the front end's live CMN and dither state carry over).  Returns one dict per utterance: hyp (the words,
-        fillers and <s> / </s> left out), score, seg [n][7] = entry, wid, sf, ef, path score, ascr, lscr, and words()."""
+        (the front end's live CMN and dither state carry over).  start_stream says where that decoder calls
+        ps_start_stream, which resets the -remove_noise tracker: "utterance" reproduces a reference program that calls
+        ps_start_stream, ps_start_utt, ps_process_raw(full_utt), ps_end_utt for every utterance; "session" one that
+        calls ps_start_stream once before a session's first utterance and then only ps_start_utt, ps_process_raw,
+        ps_end_utt, so the tracker carries from one utterance to the next.  Returns one dict per utterance: hyp (the
+        words, fillers and <s> / </s> left out), score, seg [n][7] = entry, wid, sf, ef, path score, ascr, lscr, and
+        words()."""
+        if start_stream not in ("utterance", "session"):
+            raise ValueError("start_stream must be 'utterance' or 'session', not %r" % (start_stream,))
         if sessions is None:
             return self._decode(utterances, None)
         assert len(sessions) == len(utterances)
@@ -108,17 +115,20 @@ class Decoder:
         # the front end wants each session's utterances consecutive, in decode order
         order = sorted(range(len(utterances)), key=lambda i: (first[sessions[i]], i))
         sizes = [sessions.count(sid) for sid in sorted(first, key=first.get)]
-        res = self._decode([utterances[i] for i in order], np.cumsum([0] + sizes))
+        res = self._decode([utterances[i] for i in order], np.cumsum([0] + sizes), start_stream == "session")
         out = [None] * len(utterances)
         for j, i in enumerate(order):
             out[i] = res[j]
         return out
 
-    def decode_stream_batch(self, streams, vad_mode=0, vad_window=0.3, vad_ratio=0.9, vad_frame_length=0.03):
+    def decode_stream_batch(self, streams, vad_mode=0, vad_window=0.3, vad_ratio=0.9, vad_frame_length=0.03,
+                            start_stream="utterance"):
         """Whole recordings in, words out: every stream is cut into speech segments by the device endpointer (at the
         model's sample rate; api.Endpointer), and all segments of all streams are decoded in one decode_raw_batch call
         with one session per stream, so a stream's segments are one decoder's utterances in order (live CMN and dither
-        carry over, as for a reference decoder fed the segments one after another).  Returns, per stream, a list of
+        carry over, as for a reference decoder fed the segments one after another).  start_stream is decode_raw_batch's:
+        "utterance" for a reference program that calls ps_start_stream before every segment, "session" for one that
+        calls it once per recording, so the -remove_noise tracker carries across its segments.  Returns, per stream, a list of
         dicts: start_time, end_time (the endpointer's float64 seconds), start_sample, end_sample, and decode_raw_batch's
         hyp, score, seg, words, n_frames.  The segments count against max_utts / max_frames of this Decoder."""
         ep = api.Endpointer(vad_window, vad_ratio, vad_mode, self.sample_rate, vad_frame_length, self.device)
@@ -134,7 +144,7 @@ class Decoder:
         if len(utts) > self.max_utts:
             raise ValueError("%d speech segments, more than this Decoder's max_utts (%d): create it with a larger max_utts"
                              % (len(utts), self.max_utts))
-        res = self.decode_raw_batch(utts, sessions) if utts else []
+        res = self.decode_raw_batch(utts, sessions, start_stream) if utts else []
         out, k = [], 0
         for ss in segs:
             row = []
@@ -146,7 +156,7 @@ class Decoder:
             out.append(row)
         return out
 
-    def _decode(self, utterances, sess_off):
+    def _decode(self, utterances, sess_off, carry_noise=False):
         import torch
         g = self.search
         info = g["info"]
@@ -154,6 +164,10 @@ class Decoder:
         pcm = np.concatenate([np.ascontiguousarray(u, np.int16) for u in utterances]) if utterances else np.zeros(0, np.int16)
         if sess_off is not None:
             self.fe.set_sessions(sess_off)
+            if carry_noise:
+                starts = np.zeros(len(utterances), bool)
+                starts[np.asarray(sess_off[:-1])[np.diff(sess_off) > 0]] = True
+                self.fe.set_stream_starts(starts)
         frame_off, best, pen = self.batch.decode_pcm_host(self.fe, self.phoneloop, pcm, off)
         d_scr = self.batch.senscr_device_ptr()
         d_pen = (torch.from_numpy(np.ascontiguousarray(pen, np.int32)).to(torch.device("cuda", self.device))
