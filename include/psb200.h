@@ -135,8 +135,8 @@ int psb_batch_last_kernel_ms(psb_batch_t *b, float *out3);
  * launched on): record slot 0/1, then elapsed ms between them (synchronises). */
 int psb_batch_event_record(psb_batch_t *b, int slot);
 int psb_batch_event_elapsed_ms(psb_batch_t *b, float *ms);
-/* debugging: with PSB_TC_CHECK=1 in the environment the tensor-core filter kernels (the default top-N path
- * for 13-dimensional PTM streams; PSB_TOPN_VARIANT=5 selects the scan over time instead) measure, over
+/* debugging: with PSB_TC_CHECK=1 in the environment the tensor-core filter kernels (the top-N path of PTM
+ * models whose streams are all 13-dimensional, at -ds 1) measure, over
  * everything this batch has scored, the largest |filter value - exact distance| / error bound (must stay
  * below 1) and the largest candidate count per (frame, codebook-stream pair); stats4 (may be NULL) = rows seen,
  * rows whose record came from the filter values alone, exact distances computed, rows handed to the tie fix-up. */

@@ -295,11 +295,11 @@ extern "C" int psb_model_device(const psb_model_t *m) { return m ? m->device : -
 extern "C" int psb_batch_create(psb_model_t *m, int32_t max_utts, int64_t max_frames, psb_batch_t **out)
 {
     PSB_REQUIRE(m && out && max_utts > 0 && max_frames > 0, "psb_batch_create: bad argument");
-    // top-N path (see psb_internal.cuh): a value that selects no kernel is an error rather than the default, so that a
-    // run never times the default under another kernel's name
+    // The top-N kernel follows from the model (psb_launch_ptm_batch).  A selector naming another kernel is an error
+    // rather than ignored, so that a run never times the model's kernel under another kernel's name.
     const char *v = getenv("PSB_TOPN_VARIANT"), *impl = getenv("PSB_TC_IMPL");
-    PSB_REQUIRE(!v || (strlen(v) == 1 && strchr("023456", v[0])),
-                "psb_batch_create: PSB_TOPN_VARIANT=%s; accepted values are 0, 2, 3, 4, 5 and 6 (default)", v);
+    PSB_REQUIRE(!v || !strcmp(v, "6"),
+                "psb_batch_create: PSB_TOPN_VARIANT=%s; the top-N kernel now follows from the model (the only accepted value is 6)", v);
     PSB_REQUIRE(!impl || !strcmp(impl, "wgmma"), "psb_batch_create: PSB_TC_IMPL=%s; the only accepted value is wgmma", impl);
     PSB_CUDA(cudaSetDevice(m->device));
     std::unique_ptr<psb_batch_t> b(new psb_batch_t());
@@ -307,9 +307,6 @@ extern "C" int psb_batch_create(psb_model_t *m, int32_t max_utts, int64_t max_fr
     b->max_utts = max_utts;
     b->max_frames = max_frames;
     {
-        // default 6 = tensor-core filter + exact rescoring (psb_ptm_tc.cu) where the model allows it,
-        // else codeword pairs with deferred insertion (ptm_topnq_kernel, variant 5)
-        b->topn_variant = v ? atoi(v) : 6;
         const char *p = getenv("PSB_PIPELINE");         // sub-batches in flight for psb_decode_batch_*
         b->n_pipe = p ? atoi(p) : 0;                   // 0 = auto (see decode_common)
         if (b->n_pipe < 0) b->n_pipe = 0;
@@ -446,7 +443,7 @@ static int get_kid(psb_batch_t *b, int i, psb_batch_t **out)
 {
     while ((int)b->kids.size() <= i) {
         std::unique_ptr<psb_batch_t> k(new psb_batch_t());
-        k->m = b->m; k->max_utts = b->max_utts; k->max_frames = b->max_frames; k->topn_variant = b->topn_variant;
+        k->m = b->m; k->max_utts = b->max_utts; k->max_frames = b->max_frames;
         k->n_pipe = 1;
         cudaError_t e = k->stream.create();
         for (int j = 0; j < 4 && e == cudaSuccess; ++j) e = k->ev[j].create();

@@ -494,7 +494,7 @@ extern "C" int psb_phoneloop_run_host(psb_phoneloop_t *p, const int16_t *senscr,
 constexpr int HS_V = 4;                     // instances per thread
 constexpr int HS_TS = 512;                  // storage tile: [tile][field][HS_TS], so a CTA's fields are one contiguous block
 constexpr int SWEEP_FR = 4;                 // hmmset_sweep_kernel: frames per block barrier (2 * SWEEP_FR score rows in flight)
-// threads per CTA: 128 (default) or 256 (PSB_HMMSET_THREADS)
+constexpr int HS_THREADS = 128;             // hmmset_eval_kernel: threads per CTA
 
 struct psb_hmmset_s {
     psb_hmmctx_t *c;
@@ -621,8 +621,8 @@ __device__ __forceinline__ void tma_bulk_g2s(void *dst, const void *src, unsigne
 // segment.  row0[seg] + t is the segment's senone-score row of this frame (staged in shared
 // memory: the gathers of a tile hit ~3 x HS_TILE random int16 of it); segments with
 // n_rows[seg] <= t are finished.  NS = 3 or 5 (0: any topology, runtime count).
-template <int NS, int HS_THREADS>
-__global__ void __launch_bounds__(HS_THREADS, (NS == 3 ? 3 : 2) * (256 / HS_THREADS))
+template <int NS>
+__global__ void __launch_bounds__(HS_THREADS, NS == 3 ? 6 : 4)
 hmmset_eval_kernel(HmmSetDev s, HmmCtxDev c, const int16_t *__restrict__ senscr, const int64_t *__restrict__ row0,
                    const int32_t *__restrict__ n_rows, int t, int32_t *__restrict__ best_out)
 {
@@ -1095,6 +1095,9 @@ extern "C" void psb_hmmset_free(psb_hmmset_t *s)
 extern "C" int psb_hmmset_create(psb_hmmctx_t *c, int64_t n_max, int32_t n_seg_max, psb_hmmset_t **out)
 {
     PSB_REQUIRE(c && out && n_max > 0 && n_seg_max > 0 && n_seg_max <= 65535, "psb_hmmset_create: bad argument");
+    // hmmset_eval_kernel has one CTA shape; a selector asking for another is an error rather than ignored
+    const char *v = getenv("PSB_HMMSET_THREADS");
+    PSB_REQUIRE(!v || !strcmp(v, "128"), "psb_hmmset_create: PSB_HMMSET_THREADS=%s; the only accepted value is 128", v);
     PSB_CUDA(cudaSetDevice(c->device));
     std::unique_ptr<psb_hmmset_t> s(new psb_hmmset_t());
     s->c = c; s->n_max = n_max; s->n_seg_max = n_seg_max;
@@ -1237,37 +1240,26 @@ extern "C" int psb_hmmset_eval_frames_device(psb_hmmset_t *s, const int16_t *d_s
         PSB_CUDA(cudaStreamSynchronize(s->stream));
         return PSB_OK;
     }
-    static const int threads = [] {
-        const char *v = getenv("PSB_HMMSET_THREADS");
-        return v && atoi(v) == 256 ? 256 : 128;
-    }();
-    const int tile = threads * HS_V;
+    const int tile = HS_THREADS * HS_V;
     const dim3 grid((unsigned)((s->max_seg_len + tile - 1) / tile), (unsigned)s->n_seg);
     const HmmSetDev sd = dev_set(s);
     const HmmCtxDev cd = dev_ctx(s->c);
     const size_t smem = (((size_t)cd.n_sen * 2 + 15) & ~(size_t)15) + 16;      // the row keeps its alignment within 16 bytes
     PSB_REQUIRE(smem <= 200 * 1024, "psb_hmmset: %d senones do not fit the shared-memory score row", cd.n_sen);
     auto launch = [&](auto kern, int t, int32_t *best) {
-        kern<<<grid, threads, smem, s->stream>>>(sd, cd, d_senscr, d_row0, d_n_rows, t, best);
+        kern<<<grid, HS_THREADS, smem, s->stream>>>(sd, cd, d_senscr, d_row0, d_n_rows, t, best);
     };
-#define PSB_HS_ATTR(NS, NT) PSB_CUDA(cudaFuncSetAttribute(hmmset_eval_kernel<NS, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem))
+#define PSB_HS_ATTR(NS) PSB_CUDA(cudaFuncSetAttribute(hmmset_eval_kernel<NS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem))
     if (smem > 48 * 1024) {
-        PSB_HS_ATTR(3, 256); PSB_HS_ATTR(5, 256); PSB_HS_ATTR(0, 256); PSB_HS_ATTR(3, 128); PSB_HS_ATTR(5, 128); PSB_HS_ATTR(0, 128);
+        PSB_HS_ATTR(3); PSB_HS_ATTR(5); PSB_HS_ATTR(0);
     }
 #undef PSB_HS_ATTR
     PSB_CUDA(cudaEventRecord(s->ev[0], s->stream));
     for (int t = 0; t < n_frames; ++t) {
         int32_t *best = d_best + (size_t)t * s->n_seg;
-        if (threads == 256) {
-            if (cd.n_emit == 3) launch(hmmset_eval_kernel<3, 256>, t, best);
-            else if (cd.n_emit == 5) launch(hmmset_eval_kernel<5, 256>, t, best);
-            else launch(hmmset_eval_kernel<0, 256>, t, best);
-        }
-        else {
-            if (cd.n_emit == 3) launch(hmmset_eval_kernel<3, 128>, t, best);
-            else if (cd.n_emit == 5) launch(hmmset_eval_kernel<5, 128>, t, best);
-            else launch(hmmset_eval_kernel<0, 128>, t, best);
-        }
+        if (cd.n_emit == 3) launch(hmmset_eval_kernel<3>, t, best);
+        else if (cd.n_emit == 5) launch(hmmset_eval_kernel<5>, t, best);
+        else launch(hmmset_eval_kernel<0>, t, best);
         PSB_LAUNCH_CHECK();
     }
     PSB_CUDA(cudaEventRecord(s->ev[1], s->stream));

@@ -137,9 +137,6 @@ struct psb_batch_s {
     long long last_frames;
     DevBuf<float2> d_semi_dist;   // semi-continuous split path: {d, partial} per (stream, frame, codeword)
     DevBuf<int32_t> d_uttoff;
-    int topn_variant;             // PSB_TOPN_VARIANT: 0 scalar, 2 codeword pairs, 3 two utterances per lane,
-                                  // 4/5 pairs + deferred insertion (2 / 1 utterances per lane),
-                                  // 6 (default) tensor-core filter + exact rescoring where the model allows, else 5
     DevBuf<unsigned> d_tc_flags; size_t tc_flag_words;   // [K][words]: frames the tie fix-up redoes
     DevBuf<float> d_tc_check;     // debug (PSB_TC_CHECK=1): max |a - d| / eps, max candidates, decision-path counters
     int tc_last_tpc;              // the last filter launch: tiles per CTA and CTAs per pair
@@ -167,7 +164,7 @@ int psb_phoneloop_n_phones(const psb_phoneloop_t *p);
 int psb_launch_ptm_batch(psb_batch_t *b, const float *d_feats, const int32_t *utt_off,
                          int32_t n_utt, int16_t *d_senscr);
 int psb_tc_prepare(psb_model_t *m, const float *hm, const float *hv, const float *hd);
-bool psb_tc_usable(const psb_batch_t *b);
+bool psb_tc_usable(const psb_model_t *m);
 int psb_launch_ptm_tc(psb_batch_t *b, const float *d_feats, const int32_t *utt_off, int32_t n_utt, const int32_t *d_klist,
                       const int32_t *d_featoff);
 int psb_ms_score_one(psb_model_t *m, cudaStream_t st, const float *d_feat, void *d_dist, int32_t *d_best,

@@ -826,10 +826,9 @@ int psb_tc_prepare(psb_model_t *m, const float *hm, const float *hv, const float
     return PSB_OK;
 }
 
-bool psb_tc_usable(const psb_batch_t *b)
+bool psb_tc_usable(const psb_model_t *m)
 {
-    const psb_model_t *m = b->m;
-    return m->tc_ok && m->ds_ratio == 1 && b->topn_variant >= 6;
+    return m->tc_ok && m->ds_ratio == 1;
 }
 
 // Top-N records of a whole batch into b->d_topn (same format as the scan kernels write).

@@ -237,8 +237,8 @@ def score_vs_oracle(api, oracle, pm, chunks, batch=None):
 
 
 def child(script, timeout=900):
-    """Run `script` in a fresh interpreter with PSB_TC_CHECK=1 (read once per process) and the filter path selected;
-    `script` prints one JSON line last, which is returned parsed."""
+    """Run `script` in a fresh interpreter with PSB_TC_CHECK=1 (read once per process); `script` prints one JSON line
+    last, which is returned parsed."""
     import json
     import os
     import subprocess
@@ -246,6 +246,6 @@ def child(script, timeout=900):
     here = os.path.dirname(os.path.abspath(__file__))
     prelude = "import sys\nsys.path.insert(0, %r)\nsys.path.insert(0, %r)\n" % (os.path.dirname(here), here)
     r = subprocess.run([sys.executable, "-c", prelude + script], capture_output=True, text=True, timeout=timeout,
-                       env=dict(os.environ, PSB_TC_CHECK="1", PSB_TOPN_VARIANT="6"))
+                       env=dict(os.environ, PSB_TC_CHECK="1"))
     assert r.returncode == 0, r.stderr[-3000:]
     return json.loads(r.stdout.strip().splitlines()[-1])

@@ -4,6 +4,7 @@ import numpy as np
 import pytest
 
 from conftest import assert_hmm_equal, golden, hmm_view
+from pocketsphinx_b200.model import make_logadd8, quantize_for_ties, synth_feats, synth_ptm, synth_semi
 
 pytestmark = pytest.mark.gpu
 
@@ -364,44 +365,95 @@ def test_phoneloop_large_and_5state_vs_oracle(api, n_emit, H, window, skip):
 
 
 # ---------------------------------------------------------------------------------------
-# every top-N kernel variant (PSB_TOPN_VARIANT, read at psb_batch_create) must give the same bits
+# the top-N path follows from the model (psb_launch_ptm_batch); every path must give the oracle's bits.
+# FIXED_POINT models (ptm_topn_kernel<FL, SEMI, true>) are checked in test_gpu_fixed_point.py.
 
-@pytest.mark.parametrize("variant", [0, 2, 3, 4, 5, 6])
-def test_topn_kernel_variants(api, en_us_dev, variant, monkeypatch):
-    from oracle import oracle
-    from pocketsphinx_b200.model import quantize_for_ties, synth_feats, synth_ptm
-    monkeypatch.setenv("PSB_TOPN_VARIANT", str(variant))
-    # (1) shipped model, real features
-    g = golden("en_us_goforward.npz")
-    b = api.Batch(en_us_dev, 4, 1024)
-    assert np.array_equal(b.score_host(g["feats"], np.array([0, 278], np.int32)), g["senscr"])
-    _, raw = oracle.OracleModel(en_us_dev.pm).score_utt(g["feats"], want_raw=True)
-    oracle.assert_records_equal(b.get_topn(278), oracle.ptm_records(raw), "en-us")
-    b.close()
-    # (2) BASELINE shape, ragged batch of 70 utterances (3 lane groups: an odd group count, padding
-    #     lanes, zero-length utterances)
-    pm = synth_ptm(seed=11, n_density=256, n_sen=600)
+def _ragged_70(pm):
+    """70 utterances: 3 lane groups (an odd group count), padding lanes, zero-length utterances."""
     rng = np.random.default_rng(4)
     lens = [0, 1, 40, 0, 17] + [int(x) for x in rng.integers(1, 40, 65)]
     feats = synth_feats(pm, len(lens), 40, seed=3)
-    _batch_vs_oracle(api, pm, [feats[u][:n].reshape(n, pm.sumlen) for u, n in enumerate(lens)])
+    return [feats[u][:n].reshape(n, pm.sumlen) for u, n in enumerate(lens)]
+
+
+# path -> model maker (seed, n_density, n_sen); the semi paths that need other densities ignore n_density
+TOPN_PATHS = {
+    "tc_filter": lambda seed, nd, n_sen: synth_ptm(seed=seed, n_density=nd, n_sen=n_sen),
+    "ptm_scan": lambda seed, nd, n_sen: synth_ptm(seed=seed, n_density=nd, n_sen=n_sen, featlen=12),
+    "ptm_scalar": lambda seed, nd, n_sen: synth_ptm(seed=seed, n_density=nd, n_sen=n_sen, featlen=39),
+    "semi_split": lambda seed, nd, n_sen: synth_semi(seed=seed, n_density=nd, n_sen=n_sen),
+    "semi_pairs": lambda seed, nd, n_sen: synth_semi(seed=seed, n_density=96, n_sen=n_sen),
+    "semi_scalar": lambda seed, nd, n_sen: synth_semi(seed=seed, n_density=96, n_sen=n_sen, featlens=(39,)),
+}
+
+
+@pytest.mark.parametrize("path", list(TOPN_PATHS))
+def test_topn_path_follows_the_model(api, en_us, en_us_dev, path):
+    """One case per top-N path, each selected by the model alone:
+    tc_filter   13-dimensional PTM, 64/128/256 densities, -ds 1: tensor-core filter, exact rows, fix-up
+    ptm_scan    other PTM with streams of up to 16 dimensions: ptm_topnq_kernel
+    ptm_scalar  streams longer than 16 dimensions: ptm_topn_kernel<FL, false, false>
+    semi_split  semi-continuous, one codebook of 64/128/256 densities: semi_dist_kernel + semi_scan_kernel
+    semi_pairs  other semi-continuous models, streams of up to 16 dimensions: ptm_topn2_kernel
+    semi_scalar semi-continuous, streams longer than 16 dimensions: ptm_topn_kernel<FL, true, false>"""
+    import copy
+    from oracle import oracle
+    make = TOPN_PATHS[path]
+    g = golden("en_us_goforward.npz")
+    if path == "tc_filter":
+        # (1) shipped model, real features
+        b = api.Batch(en_us_dev, 4, 1024)
+        assert np.array_equal(b.score_host(g["feats"], np.array([0, 278], np.int32)), g["senscr"])
+        _, raw = oracle.OracleModel(en_us).score_utt(g["feats"], want_raw=True)
+        oracle.assert_records_equal(b.get_topn(278), oracle.ptm_records(raw), "en-us")
+        b.close()
+    if path == "ptm_scan":
+        # (1) shipped model, real features, -ds 2 (the filter takes -ds 1 only)
+        en2 = copy.copy(en_us)
+        en2.ds_ratio = 2
+        _batch_vs_oracle(api, en2, [g["feats"]])
+    # (2) ragged batch of 70 utterances
+    pm = make(11, 256, 600)
+    _batch_vs_oracle(api, pm, _ragged_70(pm))
     # (3) exact ties everywhere
-    pmq, gen = quantize_for_ties(synth_ptm(seed=2, n_density=64, n_sen=400), seed=6)
+    pmq, gen = quantize_for_ties(make(2, 64, 400), seed=6)
     _batch_vs_oracle(api, pmq, list(gen(40, 25, s=9)))
-    # (4) frame down-sampling (-ds 2): odd frames only re-score the listed codewords
-    pm2 = synth_ptm(seed=12, n_density=128, n_sen=300)
-    pm2.ds_ratio = 2
-    f2 = synth_feats(pm2, 33, 20, seed=5)
-    _batch_vs_oracle(api, pm2, [f2[u].reshape(-1, pm2.sumlen) for u in range(33)])
+    # (4) frame down-sampling (-ds 2): odd frames only re-score the listed codewords.  The filter takes -ds 1
+    #     only: the 13-dimensional model at -ds 2 is a case of the scan.
+    ds2 = [] if path == "tc_filter" else [make(12, 128, 300)]
+    if path == "ptm_scan":
+        ds2.append(synth_ptm(seed=12, n_density=128, n_sen=300))
+    for pm2 in ds2:
+        pm2.ds_ratio = 2
+        f2 = synth_feats(pm2, 33, 20, seed=5)
+        _batch_vs_oracle(api, pm2, [f2[u].reshape(-1, pm2.sumlen) for u in range(33)])
 
 
-@pytest.mark.parametrize("var,value", [("PSB_TOPN_VARIANT", "1"), ("PSB_TOPN_VARIANT", "7"), ("PSB_TC_IMPL", "mma")])
-def test_batch_refuses_a_selector_without_a_kernel(api, en_us_dev, var, value, monkeypatch):
-    """A top-N selector value that names no kernel is an error at psb_batch_create, not a silent fall-back to the
-    default, and the error names the accepted values."""
+@pytest.mark.parametrize("kind", ["ptm", "semi"])
+def test_senone_kernels_for_a_wide_add_table(api, kind):
+    """An add table whose largest entry e has 3 e >= SEN_BIAS (64) is outside the 16x2 senone kernels' bias bound:
+    the model then selects ptm_senone_kernel / semi_senone_kernel (8-bit weights)."""
+    pm = synth_ptm(seed=7, n_density=64, n_sen=400) if kind == "ptm" else synth_semi(seed=7, n_density=64, n_sen=200)
+    pm.logadd8 = make_logadd8(shift=8)
+    assert 3 * int(pm.logadd8.max()) >= 64
+    feats = synth_feats(pm, 20, 30, seed=8)
+    _batch_vs_oracle(api, pm, list(feats))
+
+
+@pytest.mark.parametrize("var,value", [("PSB_TOPN_VARIANT", "0"), ("PSB_TOPN_VARIANT", "1"), ("PSB_TOPN_VARIANT", "5"),
+                                       ("PSB_TOPN_VARIANT", "7"), ("PSB_TC_IMPL", "mma"), ("PSB_HMMSET_THREADS", "256")])
+def test_batch_refuses_a_selector_without_a_kernel(api, en_us, en_us_dev, var, value, monkeypatch):
+    """A kernel selector naming anything but the one kernel the model selects is an error at psb_batch_create
+    (psb_hmmset_create for PSB_HMMSET_THREADS), not a silent fall-back, and the error names the accepted value."""
     from pocketsphinx_b200._lib import PsbError
     monkeypatch.setenv(var, value)
-    with pytest.raises(PsbError, match=r"accepted value.*(0, 2, 3, 4, 5 and 6|wgmma)"):
+    if var == "PSB_HMMSET_THREADS":
+        ctx = api.HmmContext(en_us.tp, en_us.sseq, en_us.n_sen)
+        with pytest.raises(PsbError, match=r"PSB_HMMSET_THREADS=256; the only accepted value is 128"):
+            api.HmmSet(ctx, 64, 1)
+        ctx.close()
+        return
+    with pytest.raises(PsbError, match=r"(follows from the model \(the only accepted value is 6\)|accepted value is wgmma)"):
         api.Batch(en_us_dev, 4, 1024)
 
 
@@ -628,24 +680,24 @@ def test_hmmset_sweep_beam_matches_oracle(api, n_emit, big, maxhmmpf):
 # BASELINE.json config 2 at FULL size (1000 utterances x 998 frames, 5138 senones): properties
 # that do not need the oracle on every frame, plus the oracle on a sample of utterances.
 
-def test_full_size_properties(api, monkeypatch):
+def test_full_size_properties_filter_and_scan(api):
     import torch
     import zlib
     from oracle import oracle
-    from pocketsphinx_b200.model import synth_feats, synth_ptm
-    pm = synth_ptm(seed=0)
     U, T = 1000, 998
-    feats = synth_feats(pm, U, T, seed=77)
-    flat = np.ascontiguousarray(feats.reshape(U * T, pm.sumlen))
     off = api.Batch.offsets([T] * U)
-    m = api.Model(pm)
-    ctx = api.HmmContext(pm.tp, pm.sseq, pm.n_sen)
-    H = pm.n_ciphone
-    pl = api.PhoneLoop(ctx, pm.phone_ssid[:H], pm.phone_tmat[:H], 5, -1080, -1080, 0, 3.0)
-    d_feats = torch.from_numpy(flat).cuda()
 
-    def run(variant, pipe):
-        monkeypatch.setenv("PSB_TOPN_VARIANT", str(variant))
+    def shape(pm):
+        feats = synth_feats(pm, U, T, seed=77)
+        m = api.Model(pm)
+        ctx = api.HmmContext(pm.tp, pm.sseq, pm.n_sen)
+        H = pm.n_ciphone
+        pl = api.PhoneLoop(ctx, pm.phone_ssid[:H], pm.phone_tmat[:H], 5, -1080, -1080, 0, 3.0)
+        return feats, m, ctx, pl
+
+    def run(pm, feats, m, pl, pipe):
+        flat = np.ascontiguousarray(feats.reshape(U * T, pm.sumlen))
+        d_feats = torch.from_numpy(flat).cuda()
         b = api.Batch(m, U, U * T)
         b.set_pipeline(pipe)
         best, pen = b.decode_host(pl, flat, off)
@@ -660,35 +712,45 @@ def test_full_size_properties(api, monkeypatch):
         sample = {u: scr[off[u]:off[u + 1]].cpu().numpy() for u in (0, 499, 999)}
         mins = scr.view(U * T, pm.n_sen).min(1).values.cpu().numpy()
         b.close()
+        del scr, d_feats
         return best, pen, rows.cpu().numpy(), sample, mins
 
-    best5, pen5, rows5, sample5, mins5 = run(5, 1)
-    # every frame's best senone scores 0 (ptm_mgau.c:398-400) and the phone loop saw every frame
-    assert (mins5 == 0).all()
-    assert best5.shape == (U * T,) and pen5.shape == (U * T, H)
-    # oracle on three whole utterances
-    om = oracle.OracleModel(pm)
-    for u, got in sample5.items():
-        assert np.array_equal(got, om.score_utt(feats[u])), "utterance %d" % u
-    # same bits from the packed kernel without deferred insertion, and from two ranges in flight
-    best2, pen2, rows2, _, _ = run(2, 2)
-    assert np.array_equal(rows5, rows2)
-    assert np.array_equal(best5, best2) and np.array_equal(pen5, pen2)
-    # and from the path without the recurrence over time (tensor-core filter + exact rescoring + tie fix-up)
-    best6, pen6, rows6, _, _ = run(6, 1)
-    assert np.array_equal(rows5, rows6)
-    assert np.array_equal(best5, best6) and np.array_equal(pen5, pen6)
-    best6p, pen6p, rows6p, _, _ = run(6, 3)                 # ... and with three sub-batches of it in flight on their own streams
-    assert np.array_equal(rows5, rows6p)
-    assert np.array_equal(best5, best6p) and np.array_equal(pen5, pen6p)
+    def check_one(pm, feats, got):
+        best, pen, _, sample, mins = got
+        # every frame's best senone scores 0 (ptm_mgau.c:398-400) and the phone loop saw every frame
+        assert (mins == 0).all()
+        assert best.shape == (U * T,) and pen.shape == (U * T, pm.n_ciphone)
+        # oracle on three whole utterances
+        om = oracle.OracleModel(pm)
+        for u, scr in sample.items():
+            assert np.array_equal(scr, om.score_utt(feats[u])), "utterance %d" % u
+
+    def same(a, b):
+        assert np.array_equal(a[2], b[2])
+        assert np.array_equal(a[0], b[0]) and np.array_equal(a[1], b[1])
+
+    # BASELINE shape: the tensor-core filter, with one, two and three sub-batches in flight on their own streams
+    pm = synth_ptm(seed=0)
+    feats, m, ctx, pl = shape(pm)
+    r1 = run(pm, feats, m, pl, 1)
+    check_one(pm, feats, r1)
+    same(r1, run(pm, feats, m, pl, 2))
+    same(r1, run(pm, feats, m, pl, 3))
+    pl.close(); ctx.close(); m.close()
+    # 12-dimensional streams: the scan, whose lanes take the utterances longest first
+    pm = synth_ptm(seed=0, featlen=12)
+    feats, m, ctx, pl = shape(pm)
+    s1 = run(pm, feats, m, pl, 1)
+    check_one(pm, feats, s1)
+    s2 = run(pm, feats, m, pl, 2)
+    same(s1, s2)
     # utterance order does not matter: reversed batch gives the reversed result
-    monkeypatch.setenv("PSB_TOPN_VARIANT", "5")
     b = api.Batch(m, U, U * T)
     rbest, rpen = b.decode_host(pl, np.ascontiguousarray(feats[::-1].reshape(U * T, pm.sumlen)), off)
-    assert np.array_equal(rbest.reshape(U, T)[::-1], best5.reshape(U, T))
-    assert np.array_equal(rpen.reshape(U, T, H)[::-1], pen5.reshape(U, T, H))
+    assert np.array_equal(rbest.reshape(U, T)[::-1], s1[0].reshape(U, T))
+    assert np.array_equal(rpen.reshape(U, T, pm.n_ciphone)[::-1], s1[1].reshape(U, T, pm.n_ciphone))
     b.close(); pl.close(); ctx.close(); m.close()
-    assert zlib.crc32(rows5.tobytes()) == zlib.crc32(rows2.tobytes())
+    assert zlib.crc32(s1[2].tobytes()) == zlib.crc32(s2[2].tobytes())
 
 
 # ---------------------------------------------------------------------------------------

@@ -17,17 +17,15 @@ def api():
 
 
 @pytest.mark.parametrize("name", tc.CASES)
-def test_crafted_case_records_match_oracle(api, name, monkeypatch):
+def test_crafted_case_records_match_oracle(api, name):
     from oracle import oracle
-    monkeypatch.setenv("PSB_TOPN_VARIANT", "6")
     pm, utts, _ = tc.case(name)
     tc.score_vs_oracle(api, oracle, pm, utts)
 
 
-def test_work_list_overflow_is_deterministic(api, monkeypatch):
+def test_work_list_overflow_is_deterministic(api):
     """Which rows fall back to the filter kernel depends on the order of atomics; the records must not."""
     from oracle import oracle
-    monkeypatch.setenv("PSB_TOPN_VARIANT", "6")
     pm, utts, _ = tc.case("positive_256")
     r1, _ = tc.score_vs_oracle(api, oracle, pm, utts)
     r2, _ = tc.score_vs_oracle(api, oracle, pm, utts)
@@ -72,10 +70,9 @@ def _tpc_rule(tiles, K, P):
     return t
 
 
-def test_geometry_ragged_totals_and_tiles_per_cta(api, monkeypatch):
+def test_geometry_ragged_totals_and_tiles_per_cta_vs_oracle(api):
     """Ragged batches of 1 .. 191 frames (partial tiles, an empty second warpgroup) and batches sized so that a CTA walks
-    1, 2, 8 and 32 tiles with a partial last CTA: every record equals the scan kernel's (variant 5, itself checked
-    against the oracle), and the oracle scores every utterance that crosses a CTA boundary or lies in the last CTA."""
+    1, 2, 8 and 32 tiles with a partial last CTA: every record of every utterance equals the oracle's."""
     import torch
     from oracle import oracle
     lays = [tc.layout_split(64, a, b, -6000.3) for a, b in tc.SPLITS]
@@ -98,27 +95,19 @@ def test_geometry_ragged_totals_and_tiles_per_cta(api, monkeypatch):
         utts = tc.utterances(pm, fr, lens, target, p_crafted=0.3)
         feats, off = np.concatenate(utts), api.Batch.offsets(lens)
         m = api.Model(pm)
-        recs = []
-        for variant in ("5", "6"):
-            monkeypatch.setenv("PSB_TOPN_VARIANT", variant)
-            b = api.Batch(m, len(lens) + 1, total + 1)
-            b.score_host(feats, off)
-            recs.append(b.get_topn(total))
-            if variant == "6":
-                b.tc_check()
-                st = b.tc_stats
-            b.close()
-        m.close()
+        b = api.Batch(m, len(lens) + 1, total + 1)
+        b.score_host(feats, off)
+        rec = b.get_topn(total)
+        b.tc_check()
+        st = b.tc_stats
+        b.close(); m.close()
         assert st["tiles_per_cta"] == target and st["ctas_per_pair"] == -(-tiles // target), (target, tiles, st)
         seen.add(st["tiles_per_cta"])
-        oracle.assert_records_equal(recs[1], recs[0], "%d tiles per CTA: filter vs scan" % target)
-        span = target * 128                                  # frames per CTA
-        last0 = (total - 1) // span * span
-        pick = [u for u in range(len(lens)) if off[u] // span != (off[u + 1] - 1) // span or off[u + 1] > last0]
         om = oracle.OracleModel(pm)
-        for u in pick[:8] + pick[-4:]:
+        for u in range(len(lens)):
             _, raw = om.score_utt(utts[u], want_raw=True)
-            oracle.assert_records_equal(recs[1][off[u]:off[u + 1]], oracle.ptm_records(raw), "utterance %d" % u)
+            oracle.assert_records_equal(rec[off[u]:off[u + 1]], oracle.ptm_records(raw),
+                                        "%d tiles per CTA, utterance %d" % (target, u))
     assert seen == {1, 2, 8, 32}
 
 
@@ -147,13 +136,14 @@ def _mllr(pm, raw, seed):
     return q
 
 
-@pytest.mark.parametrize("kind,variant", [("ptm", "6"), ("ptm", "5"), ("semi", "6"), ("ms", "6")])
-def test_batch_after_gaussian_update_matches_oracle(api, kind, variant, monkeypatch):
+@pytest.mark.parametrize("kind", ["ptm", "ptm_scan", "semi", "ms"])
+def test_batch_after_gaussian_update_matches_oracle(api, kind):
+    """ptm: 13-dimensional streams, the tensor-core filter; ptm_scan: 12-dimensional streams, the scan."""
     from oracle import oracle
     from pocketsphinx_b200.model import synth_feats, synth_ms, synth_ptm, synth_semi
-    monkeypatch.setenv("PSB_TOPN_VARIANT", variant)
-    if kind == "ptm":
-        pm, raw = synth_ptm(seed=17, n_mgau=6, n_density=128, n_sen=120, return_raw=True)
+    if kind.startswith("ptm"):
+        pm, raw = synth_ptm(seed=17, n_mgau=6, n_density=128, n_sen=120, featlen=12 if kind == "ptm_scan" else 13,
+                            return_raw=True)
     elif kind == "semi":
         pm, raw = synth_semi(seed=17, n_sen=300, return_raw=True)
     else:
@@ -169,7 +159,7 @@ def test_batch_after_gaussian_update_matches_oracle(api, kind, variant, monkeypa
     scr = b.score_host(feats.reshape(-1, pm.sumlen), off)
     om = oracle.OracleModel(pm2)
     for u in range(6):
-        if kind == "ptm":
+        if kind.startswith("ptm"):
             want, rawl = om.score_utt(utts[u], want_raw=True)
             oracle.assert_records_equal(b.get_topn(180)[off[u]:off[u + 1]], oracle.ptm_records(rawl), "utt %d" % u)
         else:

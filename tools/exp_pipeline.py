@@ -1,5 +1,5 @@
 """Scratch experiment (GPU): device-resident and host-buffer step times of the BASELINE shape for
-the PSB_PIPELINE / PSB_TOPN_VARIANT combination given in the environment."""
+the sub-batch counts listed in the environment (PIPES)."""
 import os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
@@ -35,4 +35,4 @@ batch.sync()
 for pipe in [int(x) for x in os.environ.get("PIPES", "1,2,3,4").split(",")]:
     batch.set_pipeline(pipe)
     run(1); runh(1)
-    print("variant", os.environ.get("PSB_TOPN_VARIANT", "default"), "pipeline", pipe, "device %.2f %.2f" % (run(4), run(4)), "host %.2f %.2f" % (runh(4), runh(4)), flush=True)
+    print("pipeline", pipe, "device %.2f %.2f" % (run(4), run(4)), "host %.2f %.2f" % (runh(4), runh(4)), flush=True)
