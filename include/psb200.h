@@ -651,6 +651,21 @@ int psb_fe_set_stream_starts(psb_fe_t *fe, const uint8_t *start, int32_t n_utt, 
                              int32_t n_sess);
 /* the sessions' trackers after the last process call, which must have set stream starts */
 int psb_fe_get_noise_states(const psb_fe_t *fe, psb_fe_noise_t *noise_out, int32_t n_sess);
+/* Per-utterance mel filter banks for the next psb_fe_process_* / psb_decode_batch_pcm_host call, as -warp_type /
+ * -warp_params make them (VTLN: fe_warp.c, fe_build_melfilters): n_bank banks of the handle's n_filt filters each,
+ * in fe_build_melfilters' layout -- spec_start / filt_start / filt_width [n_bank][n_filt], filt_start relative to
+ * the bank's first coefficient coeff_off[b] (coeff_off[n_bank + 1], coeff_off[0] = 0) in coeffs.  Utterance u
+ * (in decode order; n_utt must be that call's utterance count) reads bank bank[u] in [0, n_bank).  An empty filter
+ * (no DFT point) is spec_start -1, filt_start 0, filt_width 0, or width 0 at the running coefficient count; its
+ * mel energy is 0.  Every other filter is checked as psb_fe_create checks its bank.  Without this call every
+ * utterance reads the bank of psb_fe_create.  A refused call changes nothing. */
+int psb_fe_set_filterbanks(psb_fe_t *fe, int32_t n_bank, const int16_t *spec_start, const int16_t *filt_start,
+                           const int16_t *filt_width, const int32_t *coeff_off, const float *coeffs,
+                           const int32_t *bank, int32_t n_utt);
+/* Drops what psb_fe_set_sessions, psb_fe_set_stream_starts and psb_fe_set_filterbanks named for the next call, so
+ * a host that is refused one of them does not leave the others behind; the next call runs with none of them.
+ * psb_fe_get_states / psb_fe_get_noise_states refuse until a call names sessions / stream starts again. */
+int psb_fe_cancel_settings(psb_fe_t *fe);
 /* From audio to phone-loop results in one call: front end, senone scores and Viterbi on the
  * device, features never leave it.  frame_off int32[n_utt + 1] (out) indexes best / pen / senscr
  * like utt_off of psb_decode_batch_host. */

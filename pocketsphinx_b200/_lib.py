@@ -145,6 +145,8 @@ SYMBOLS = [
     ("psb_fe_get_states", C.c_int, [_VP, _VP, _I32]),
     ("psb_fe_set_stream_starts", C.c_int, [_VP, _VP, _I32, _VP, _I32]),
     ("psb_fe_get_noise_states", C.c_int, [_VP, _VP, _I32]),
+    ("psb_fe_set_filterbanks", C.c_int, [_VP, _I32, _VP, _VP, _VP, _VP, _VP, _VP, _I32]),
+    ("psb_fe_cancel_settings", C.c_int, [_VP]),
     ("psb_phoneloop_create", C.c_int, [_VP, _I32, _VP, _VP, _I32, _I32, _I32, _I32, C.c_double, C.POINTER(_VP)]),
     ("psb_phoneloop_free", None, [_VP]),
     ("psb_phoneloop_run_device", C.c_int, [_VP, _VP, _VP, _I32, _VP, _VP, _VP, _VP]),

@@ -787,12 +787,85 @@ class FrontEnd:
         check(lib().psb_fe_get_noise_states(self.h, arr, n_sess), "psb_fe_get_noise_states")
         return [arr[i] for i in range(n_sess)]
 
-    def process_sessions(self, pcm, samp_off, sess_off, states=None, want_mfcc=False, starts=None, noise=None):
+    def filterbanks(self, banks, bank_of_utt):
+        """The arrays psb_fe_set_filterbanks takes, built and checked on the host (ValueError) without naming
+        anything for the next call: utterance u reads banks[bank_of_utt[u]].  Each bank is a dict with make_fe_desc's
+        spec_start / filt_start / filt_width / filt_coeffs, or a (warp_type, warp_params) pair built with this front
+        end's own settings (fe_tables.make_filterbank over desc["bank_args"])."""
+        from .fe_tables import make_filterbank
+        nf = int(self.desc["n_filt"])
+        ss, fs, fw, co, coeff_off = [], [], [], [], [0]
+        for b in banks:
+            if not isinstance(b, dict):
+                if "bank_args" not in self.desc:
+                    raise ValueError("(warp_type, warp_params) banks need a desc from make_fe_desc (its bank_args)")
+                b = make_filterbank(warp_type=b[0], warp_params=b[1], **self.desc["bank_args"])
+            for lst, k, dt in ((ss, "spec_start", np.int16), (fs, "filt_start", np.int16), (fw, "filt_width", np.int16)):
+                a = np.ascontiguousarray(b[k], dt).ravel()
+                if a.size != nf:
+                    raise ValueError("a filter bank has %d filters, this front end %d" % (a.size, nf))
+                lst.append(a)
+            co.append(np.ascontiguousarray(b["filt_coeffs"], np.float32).ravel())
+            coeff_off.append(coeff_off[-1] + co[-1].size)
+        cat = lambda parts, dt: np.ascontiguousarray(np.concatenate(parts) if parts else np.zeros(0, dt), dt)
+        return (len(banks), cat(ss, np.int16), cat(fs, np.int16), cat(fw, np.int16), np.asarray(coeff_off, np.int32),
+                cat(co, np.float32), np.ascontiguousarray(bank_of_utt, np.int32))
+
+    def warp_filterbanks(self, warps, sess_off=None):
+        """filterbanks() for one warp per utterance, or with sess_off one per session: a -warp_params string (under
+        desc's warp_type), a (warp_type, warp_params) pair, a filter-bank dict, or None for desc's own bank."""
+        if sess_off is not None:
+            if len(warps) != len(sess_off) - 1:
+                raise ValueError("%d warps for %d sessions" % (len(warps), len(sess_off) - 1))
+            warps = [w for s, w in enumerate(warps) for _ in range(int(sess_off[s + 1]) - int(sess_off[s]))]
+        banks, index, bank_of_utt = [], {}, []
+        for w in warps:
+            if isinstance(w, str):
+                w = (self.desc.get("warp_type", "inverse_linear"), w)
+            k = id(w) if isinstance(w, dict) else w
+            if k not in index:
+                index[k] = len(banks)
+                banks.append(self.desc if w is None else w)
+            bank_of_utt.append(index[k])
+        return self.filterbanks(banks or [self.desc], bank_of_utt)
+
+    def name_filterbanks(self, arrays):
+        """Names the banks filterbanks() / warp_filterbanks() built for the next process_* / Batch.decode_pcm_host
+        call (psb_fe_set_filterbanks).  Without it every utterance reads desc's bank."""
+        n, ss, fs, fw, coeff_off, co, bank_of_utt = arrays
+        check(lib().psb_fe_set_filterbanks(self.h, n, _p(ss) if ss.size else None, _p(fs) if fs.size else None,
+                                           _p(fw) if fw.size else None, _p(coeff_off), _p(co) if co.size else None,
+                                           _p(bank_of_utt) if bank_of_utt.size else None, len(bank_of_utt)),
+              "psb_fe_set_filterbanks")
+
+    def set_filterbanks(self, banks, bank_of_utt):
+        """Per-utterance mel filter banks (VTLN) for the next call: name_filterbanks(filterbanks(...))."""
+        self.name_filterbanks(self.filterbanks(banks, bank_of_utt))
+
+    def set_warps(self, warps, sess_off=None):
+        """Per-utterance (or with sess_off per-session) warps for the next call: name_filterbanks(warp_filterbanks(...))."""
+        self.name_filterbanks(self.warp_filterbanks(warps, sess_off))
+
+    def cancel_settings(self):
+        """Drops what set_sessions, set_stream_starts and set_filterbanks named for the next call
+        (psb_fe_cancel_settings): the next call runs with none of them."""
+        check(lib().psb_fe_cancel_settings(self.h), "psb_fe_cancel_settings")
+
+    def process_sessions(self, pcm, samp_off, sess_off, states=None, want_mfcc=False, starts=None, noise=None, warp=None):
         """process_host over named sessions; returns (feats, frame_off, outgoing states[, mfcc]).  With starts (one
-        flag per utterance, set_stream_starts) the outgoing noise trackers follow as one more item at the end."""
-        self.set_sessions(sess_off, states)
-        if starts is not None:
-            self.set_stream_starts(starts, noise)
+        flag per utterance, set_stream_starts) the outgoing noise trackers follow as one more item at the end.  warp:
+        one -warp_params string, (warp_type, warp_params) pair or filter-bank dict per session (None: desc's bank).
+        A refused setting leaves nothing named for the next call."""
+        banks = None if warp is None else self.warp_filterbanks(warp, sess_off=sess_off)
+        try:
+            self.set_sessions(sess_off, states)
+            if starts is not None:
+                self.set_stream_starts(starts, noise)
+            if banks is not None:
+                self.name_filterbanks(banks)
+        except BaseException:
+            self.cancel_settings()
+            raise
         r = self.process_host(pcm, samp_off, want_mfcc)
         r = r[:2] + (self.get_states(len(sess_off) - 1),) + r[2:]
         return r + (self.get_noise_states(len(sess_off) - 1),) if starts is not None else r

@@ -67,6 +67,14 @@ struct psb_fe_s {
     bool starts_pending, noise_out;           // noise_out: the last call set stream starts, noise holds its trackers
     DevBuf<psb_fe_noise_t> d_noise;           // [2][n_sess]: in, then out
     DevBuf<int4> d_chain;
+    // psb_fe_set_filterbanks, for the next call only: n_bank banks of n_filt filters, bank[u] per utterance
+    std::vector<int16_t> bank_spec_start, bank_filt_start, bank_filt_width;   // [n_bank][n_filt]
+    std::vector<int32_t> bank_coeff_off, bank_of_utt;                          // [n_bank + 1], [n_utt]
+    std::vector<float> bank_coeffs;
+    bool banks_pending;
+    DevBuf<int16_t> d_bank_spec_start, d_bank_filt_start, d_bank_filt_width;
+    DevBuf<int32_t> d_bank_coeff_off, d_bank_of_utt;
+    DevBuf<float> d_bank_coeffs;
 };
 
 namespace {
@@ -90,11 +98,14 @@ struct FeDev {
 // DITHER: pcm holds the dithered samples of the full frames, and the last frame of utterance u
 // reads its own freshly dithered copy at tail + draw[4u + 1] (fe_end_utt re-reads the overflow
 // samples); its pre-emphasis prior is still the full frames' sample before it.
-template <bool DITHER>
+// BANKS: p's filter tables hold several banks ([bank][n_filt], filt_start relative to the bank's first
+// coefficient coeff_off[bank]), and utterance u reads bank bank_of_utt[u] (psb_fe_set_filterbanks).
+template <bool DITHER, bool BANKS>
 __global__ void __launch_bounds__(128)
 fe_frame_kernel(FeDev p, const int16_t *__restrict__ pcm, const int64_t *__restrict__ samp_off,
                 const int32_t *__restrict__ frame_off, const int32_t *__restrict__ frame_utt,
-                double *__restrict__ mfspec, const int16_t *__restrict__ tail, const int64_t *__restrict__ draw)
+                double *__restrict__ mfspec, const int16_t *__restrict__ tail, const int64_t *__restrict__ draw,
+                const int32_t *__restrict__ bank_of_utt, const int32_t *__restrict__ coeff_off)
 {
     extern __shared__ double x[];             // [fft_size] frame, then [fft_size/2 + 1] power spectrum
     double *spec = x + p.fft_size;
@@ -205,11 +216,18 @@ fe_frame_kernel(FeDev p, const int16_t *__restrict__ pcm, const int64_t *__restr
     for (int j = tid; j <= N / 2; j += nt)
         spec[j] = j == 0 ? x[0] * x[0] : x[j] * x[j] + x[N - j] * x[N - j];
     __syncthreads();
-    // fe_mel_spec: one thread per filter, bins in ascending order
+    // fe_mel_spec: one thread per filter, bins in ascending order; an empty filter (width 0) gives 0
     if (tid < p.n_filt) {
-        const int ss = p.spec_start[tid], fs = p.filt_start[tid], fw = p.filt_width[tid];
+        int row = tid;
+        const float *coeffs = p.filt_coeffs;
+        if constexpr (BANKS) {
+            const int b = bank_of_utt[u];
+            row += b * p.n_filt;
+            coeffs += coeff_off[b];
+        }
+        const int ss = p.spec_start[row], fs = p.filt_start[row], fw = p.filt_width[row];
         double acc = 0;
-        for (int i = 0; i < fw; ++i) acc += spec[ss + i] * (double)p.filt_coeffs[fs + i];
+        for (int i = 0; i < fw; ++i) acc += spec[ss + i] * (double)coeffs[fs + i];
         mfspec[(size_t)f * p.n_filt + tid] = acc;
     }
 }
@@ -865,8 +883,11 @@ static int fe_run(psb_fe_t *fe, const int16_t *d_pcm, const int64_t *samp_off, i
                   float *d_mfcc_out, int32_t *frame_off, float *ms)
 {
     // sessions: the ones psb_fe_set_sessions named for this call, else one per utterance
-    const bool pending = fe->sess_pending, carry = fe->starts_pending;
-    fe->sess_pending = fe->starts_pending = fe->noise_out = false;
+    const bool pending = fe->sess_pending, carry = fe->starts_pending, banks = fe->banks_pending;
+    fe->sess_pending = fe->starts_pending = fe->noise_out = fe->banks_pending = false;
+    if (banks)
+        PSB_REQUIRE(fe->bank_of_utt.size() == (size_t)n_utt, "psb_fe: the filter banks name %d utterances, the call has %d",
+                    (int)fe->bank_of_utt.size(), n_utt);
     if (pending) {
         PSB_REQUIRE(fe->sess_off.back() == n_utt, "psb_fe: the sessions cover %d utterances, the call has %d", fe->sess_off.back(), n_utt);
     }
@@ -959,6 +980,14 @@ static int fe_run(psb_fe_t *fe, const int16_t *d_pcm, const int64_t *samp_off, i
         if (!rc) rc = grow(fe->d_noise, 2 * (size_t)n_sess);
         if (!rc) rc = grow(fe->d_chain, chains.size());
     }
+    if (banks) {
+        if (!rc) rc = grow(fe->d_bank_spec_start, fe->bank_spec_start.size());
+        if (!rc) rc = grow(fe->d_bank_filt_start, fe->bank_filt_start.size());
+        if (!rc) rc = grow(fe->d_bank_filt_width, fe->bank_filt_width.size());
+        if (!rc) rc = grow(fe->d_bank_coeff_off, fe->bank_coeff_off.size());
+        if (!rc) rc = grow(fe->d_bank_coeffs, std::max<size_t>(fe->bank_coeffs.size(), 1));
+        if (!rc) rc = grow(fe->d_bank_of_utt, std::max<size_t>(fe->bank_of_utt.size(), 1));
+    }
     if (rc) return rc;
     PSB_CUDA(cudaMemcpyAsync(fe->d_samp_off, samp_off, ((size_t)n_utt + 1) * 8, cudaMemcpyHostToDevice, fe->stream));
     PSB_CUDA(cudaMemcpyAsync(fe->d_frame_off, foff.data(), foff.size() * 4, cudaMemcpyHostToDevice, fe->stream));
@@ -974,7 +1003,23 @@ static int fe_run(psb_fe_t *fe, const int16_t *d_pcm, const int64_t *samp_off, i
         PSB_CUDA(cudaMemcpyAsync(fe->d_noise.get() + n_sess, noise_next.data(), noise_bytes, cudaMemcpyHostToDevice, fe->stream));
         PSB_CUDA(cudaMemcpyAsync(fe->d_chain, chains.data(), chains.size() * sizeof(int4), cudaMemcpyHostToDevice, fe->stream));
     }
-    const FeDev p = dev_fe(fe);
+    FeDev p = dev_fe(fe);
+    if (banks) {
+        PSB_CUDA(cudaMemcpyAsync(fe->d_bank_spec_start, fe->bank_spec_start.data(), fe->bank_spec_start.size() * 2,
+                                 cudaMemcpyHostToDevice, fe->stream));
+        PSB_CUDA(cudaMemcpyAsync(fe->d_bank_filt_start, fe->bank_filt_start.data(), fe->bank_filt_start.size() * 2,
+                                 cudaMemcpyHostToDevice, fe->stream));
+        PSB_CUDA(cudaMemcpyAsync(fe->d_bank_filt_width, fe->bank_filt_width.data(), fe->bank_filt_width.size() * 2,
+                                 cudaMemcpyHostToDevice, fe->stream));
+        PSB_CUDA(cudaMemcpyAsync(fe->d_bank_coeff_off, fe->bank_coeff_off.data(), fe->bank_coeff_off.size() * 4,
+                                 cudaMemcpyHostToDevice, fe->stream));
+        if (!fe->bank_coeffs.empty())
+            PSB_CUDA(cudaMemcpyAsync(fe->d_bank_coeffs, fe->bank_coeffs.data(), fe->bank_coeffs.size() * 4,
+                                     cudaMemcpyHostToDevice, fe->stream));
+        if (n_utt) PSB_CUDA(cudaMemcpyAsync(fe->d_bank_of_utt, fe->bank_of_utt.data(), (size_t)n_utt * 4, cudaMemcpyHostToDevice, fe->stream));
+        p.spec_start = fe->d_bank_spec_start; p.filt_start = fe->d_bank_filt_start; p.filt_width = fe->d_bank_filt_width;
+        p.filt_coeffs = fe->d_bank_coeffs;
+    }
     // with the noise tracker carried, fe_noise_kernel removes the noise and fe_utt_kernel does not
     FeDev pu = p;
     if (!chains.empty()) pu.remove_noise = 0;
@@ -989,12 +1034,14 @@ static int fe_run(psb_fe_t *fe, const int16_t *d_pcm, const int64_t *samp_off, i
         PSB_LAUNCH_CHECK();
     }
     if (total) {
-        if (fe->dither)
-            fe_frame_kernel<true><<<(unsigned)total, 128, smem, fe->stream>>>(p, fe->d_dpcm, fe->d_samp_off, fe->d_frame_off,
-                                                                            fe->d_frame_utt, fe->d_mfspec, fe->d_tail, fe->d_draw);
-        else
-            fe_frame_kernel<false><<<(unsigned)total, 128, smem, fe->stream>>>(p, d_pcm, fe->d_samp_off, fe->d_frame_off,
-                                                                             fe->d_frame_utt, fe->d_mfspec, nullptr, nullptr);
+        const int16_t *src = fe->dither ? fe->d_dpcm.get() : d_pcm;
+        const int16_t *tail = fe->dither ? fe->d_tail.get() : nullptr;
+        const int64_t *draw_d = fe->dither ? fe->d_draw.get() : nullptr;
+        const int32_t *bank_of_utt = banks ? fe->d_bank_of_utt.get() : nullptr, *coeff_off = banks ? fe->d_bank_coeff_off.get() : nullptr;
+        auto kern = fe->dither ? (banks ? fe_frame_kernel<true, true> : fe_frame_kernel<true, false>)
+                               : (banks ? fe_frame_kernel<false, true> : fe_frame_kernel<false, false>);
+        kern<<<(unsigned)total, 128, smem, fe->stream>>>(p, src, fe->d_samp_off, fe->d_frame_off, fe->d_frame_utt, fe->d_mfspec,
+                                                          tail, draw_d, bank_of_utt, coeff_off);
         PSB_LAUNCH_CHECK();
         if (!chains.empty()) {
             fe_noise_kernel<<<(unsigned)chains.size(), FE_NOISE_THREADS, 0, fe->stream>>>(
@@ -1156,5 +1203,62 @@ extern "C" int psb_fe_get_noise_states(const psb_fe_t *fe, psb_fe_noise_t *noise
     PSB_REQUIRE(fe->noise_out, "psb_fe_get_noise_states: the last process call set no stream starts");
     PSB_REQUIRE(n_sess == (int32_t)fe->noise.size(), "psb_fe_get_noise_states: the last call had %d sessions", (int)fe->noise.size());
     memcpy(noise_out, fe->noise.data(), (size_t)n_sess * sizeof(psb_fe_noise_t));
+    return PSB_OK;
+}
+
+// One bank of n_filt filters in fe_build_melfilters' layout: every filter either covers DFT points inside the
+// spectrum with filt_start the running coefficient count, or is empty (width 0) -- at spec_start -1 with
+// filt_start 0, as a filter no DFT point falls in is left, or at any start with the running count.  Returns the
+// first filter that is neither, or -1; *n_coeffs = the sum of the widths.
+static int bank_bad_filter(int n_filt, int fft_size, const int16_t *ss, const int16_t *fs, const int16_t *fw, int32_t *n_coeffs)
+{
+    int32_t n = 0;
+    for (int i = 0; i < n_filt; ++i) {
+        const bool empty_calloc = ss[i] == -1 && fw[i] == 0 && fs[i] == 0;
+        if (!empty_calloc && !(fw[i] >= 0 && ss[i] >= 0 && ss[i] + fw[i] <= fft_size / 2 + 1 && fs[i] == n)) return i;
+        n += fw[i];
+    }
+    *n_coeffs = n;
+    return -1;
+}
+
+extern "C" int psb_fe_set_filterbanks(psb_fe_t *fe, int32_t n_bank, const int16_t *spec_start, const int16_t *filt_start,
+                                      const int16_t *filt_width, const int32_t *coeff_off, const float *coeffs,
+                                      const int32_t *bank, int32_t n_utt)
+{
+    PSB_REQUIRE(fe && n_bank > 0 && spec_start && filt_start && filt_width && coeff_off && n_utt >= 0 && (bank || n_utt == 0),
+                "psb_fe_set_filterbanks: bad argument");
+    PSB_REQUIRE(coeff_off[0] == 0, "psb_fe_set_filterbanks: coeff_off[0] must be 0 (got %d)", coeff_off[0]);
+    const int nf = fe->n_filt;
+    for (int b = 0; b < n_bank; ++b) {
+        const size_t o = (size_t)b * nf;
+        int32_t n = 0;
+        PSB_REQUIRE(coeff_off[b + 1] >= coeff_off[b], "psb_fe_set_filterbanks: coeff_off not monotone at bank %d", b);
+        const int bad = bank_bad_filter(nf, fe->fft_size, spec_start + o, filt_start + o, filt_width + o, &n);
+        PSB_REQUIRE(bad < 0, "psb_fe_set_filterbanks: bank %d, mel filter %d out of range", b, bad);
+        PSB_REQUIRE(n == coeff_off[b + 1] - coeff_off[b], "psb_fe_set_filterbanks: bank %d has %d coefficients, coeff_off says %d",
+                    b, n, coeff_off[b + 1] - coeff_off[b]);
+    }
+    PSB_REQUIRE(coeff_off[n_bank] == 0 || coeffs, "psb_fe_set_filterbanks: coeffs is null");
+    for (int u = 0; u < n_utt; ++u)
+        PSB_REQUIRE(bank[u] >= 0 && bank[u] < n_bank, "psb_fe_set_filterbanks: utterance %d names bank %d of %d", u, bank[u], n_bank);
+    const size_t n = (size_t)n_bank * nf;
+    fe->bank_spec_start.assign(spec_start, spec_start + n);
+    fe->bank_filt_start.assign(filt_start, filt_start + n);
+    fe->bank_filt_width.assign(filt_width, filt_width + n);
+    fe->bank_coeff_off.assign(coeff_off, coeff_off + n_bank + 1);
+    fe->bank_coeffs.assign(coeffs, coeffs + coeff_off[n_bank]);
+    fe->bank_of_utt.assign(bank, bank + n_utt);
+    fe->banks_pending = true;
+    return PSB_OK;
+}
+
+extern "C" int psb_fe_cancel_settings(psb_fe_t *fe)
+{
+    PSB_REQUIRE(fe, "psb_fe_cancel_settings: bad argument");
+    // the setters overwrote the last call's states / trackers with the next call's inputs: report neither
+    if (fe->sess_pending) { fe->sess_off.clear(); fe->states.clear(); }
+    if (fe->starts_pending) { fe->noise.clear(); fe->noise_out = false; }
+    fe->sess_pending = fe->starts_pending = fe->banks_pending = false;
     return PSB_OK;
 }

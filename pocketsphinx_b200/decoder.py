@@ -21,7 +21,8 @@ FE_REFERENCE_DEFAULTS = dict(feat="1s_c_d_dd", cmn="live", agc="none", agcthresh
                              svspec="", dither="no",
                              round_filters="yes", ncep="13", frate="100", nfft="0", cmninit="40,3,-1", seed="-1", samprate="16000",
                              wlen="0.025625", nfilt="40", lowerf="133.33334", upperf="6855.4976", alpha="0.97",
-                             transform="legacy", lifter="0", remove_noise="no", remove_dc="no", unit_area="yes", doublebw="no")
+                             transform="legacy", lifter="0", remove_noise="no", remove_dc="no", unit_area="yes", doublebw="no",
+                             warp_type="inverse_linear", warp_params="")
 PL_DEFAULTS = dict(pl_window="5", pl_beam="1e-10", pl_pbeam="1e-10", pl_pip="1.0", pl_weight="3.0")
 
 
@@ -65,7 +66,8 @@ class Decoder:
                             lowerf=float(fp["lowerf"]), upperf=float(fp["upperf"]), alpha=float(fp["alpha"]),
                             transform=fp["transform"], lifter=int(fp["lifter"]), remove_noise=fp["remove_noise"] in yes,
                             remove_dc=fp["remove_dc"] in yes, unit_area=fp["unit_area"] in yes,
-                            round_filters=fp["round_filters"] in yes, doublebw=fp["doublebw"] in yes)
+                            round_filters=fp["round_filters"] in yes, doublebw=fp["doublebw"] in yes,
+                            warp_type=fp["warp_type"], warp_params=fp["warp_params"] or None)
         # 1s_c_d_dd with batch CMN and nothing else is the front end desc alone describes
         plain = (opts["feat"], opts["cmn"], opts["dither"], opts["varnorm"], opts["agc"], lda is None) == (0, 1, 0, 0, 0, True)
         # the dimension psb_fe_feat_dim will report: feat_read_lda's out_dim, else the feature type's
@@ -92,9 +94,10 @@ class Decoder:
         self.second_pass = search_cfg.get("fwdflat", "yes") in ("yes", "1", "true", "True")
         self.bp_cap = int(cfg.get("latsize", 5000))
         self.sample_rate = int(float(fp["samprate"]))
+        self.warp_params = fp["warp_params"] or None
         self.max_utts = max_utts
 
-    def decode_raw_batch(self, utterances, sessions=None, start_stream="utterance"):
+    def decode_raw_batch(self, utterances, sessions=None, start_stream="utterance", warp=None):
         """utterances: int16 arrays, each a whole utterance.  sessions: None (every utterance a fresh decoder) or one
         session id per utterance; the utterances of one id are one decoder's, in list order, from a fresh decoder
         (the front end's live CMN and dither state carry over).  start_stream says where that decoder calls
@@ -103,26 +106,44 @@ class Decoder:
         calls ps_start_stream once before a session's first utterance and then only ps_start_utt, ps_process_raw,
         ps_end_utt, so the tracker carries from one utterance to the next.  Returns one dict per utterance: hyp (the
         words, fillers and <s> / </s> left out), score, seg [n][7] = entry, wid, sf, ef, path score, ascr, lscr, and
-        words()."""
+        words().  warp: None, or one -warp_params string per utterance (under this decoder's -warp_type; None: the
+        decoder's own -warp_params), so each utterance is decoded with its own VTLN warp; the utterances of one session
+        are one decoder's and must name the same warp."""
         if start_stream not in ("utterance", "session"):
             raise ValueError("start_stream must be 'utterance' or 'session', not %r" % (start_stream,))
+        if warp is not None:
+            warp = list(warp)
+            if len(warp) != len(utterances):
+                raise ValueError("%d warps for %d utterances" % (len(warp), len(utterances)))
+            # None is the decoder's own -warp_params, and "" is unset: both name the bank of the decoder's front end
+            # when they mean its warp (None below)
+            warp = [None if (self.warp_params if w is None else w or None) == self.warp_params else w for w in warp]
+            if all(w is None for w in warp):
+                warp = None
         if sessions is None:
-            return self._decode(utterances, None)
+            return self._decode(utterances, None, warp=warp)
         assert len(sessions) == len(utterances)
+        if warp is not None:
+            named = {}
+            for sid, w in zip(sessions, warp):
+                if named.setdefault(sid, w) != w:
+                    raise ValueError("session %r names two warps, %r and %r: a session is one decoder, with one warp"
+                                     % (sid, named[sid], w))
         first = {}
         for i, sid in enumerate(sessions):
             first.setdefault(sid, i)
         # the front end wants each session's utterances consecutive, in decode order
         order = sorted(range(len(utterances)), key=lambda i: (first[sessions[i]], i))
         sizes = [sessions.count(sid) for sid in sorted(first, key=first.get)]
-        res = self._decode([utterances[i] for i in order], np.cumsum([0] + sizes), start_stream == "session")
+        res = self._decode([utterances[i] for i in order], np.cumsum([0] + sizes), start_stream == "session",
+                           None if warp is None else [warp[i] for i in order])
         out = [None] * len(utterances)
         for j, i in enumerate(order):
             out[i] = res[j]
         return out
 
     def decode_stream_batch(self, streams, vad_mode=0, vad_window=0.3, vad_ratio=0.9, vad_frame_length=0.03,
-                            start_stream="utterance"):
+                            start_stream="utterance", warp=None):
         """Whole recordings in, words out: every stream is cut into speech segments by the device endpointer (at the
         model's sample rate; api.Endpointer), and all segments of all streams are decoded in one decode_raw_batch call
         with one session per stream, so a stream's segments are one decoder's utterances in order (live CMN and dither
@@ -130,7 +151,10 @@ class Decoder:
         "utterance" for a reference program that calls ps_start_stream before every segment, "session" for one that
         calls it once per recording, so the -remove_noise tracker carries across its segments.  Returns, per stream, a list of
         dicts: start_time, end_time (the endpointer's float64 seconds), start_sample, end_sample, and decode_raw_batch's
-        hyp, score, seg, words, n_frames.  The segments count against max_utts / max_frames of this Decoder."""
+        hyp, score, seg, words, n_frames.  The segments count against max_utts / max_frames of this Decoder.  warp:
+        None, or one -warp_params string per stream (decode_raw_batch's warp; None: the decoder's own)."""
+        if warp is not None and len(warp) != len(streams):
+            raise ValueError("%d warps for %d streams" % (len(warp), len(streams)))
         ep = api.Endpointer(vad_window, vad_ratio, vad_mode, self.sample_rate, vad_frame_length, self.device)
         try:
             segs = ep.segment_batch(streams)
@@ -144,7 +168,8 @@ class Decoder:
         if len(utts) > self.max_utts:
             raise ValueError("%d speech segments, more than this Decoder's max_utts (%d): create it with a larger max_utts"
                              % (len(utts), self.max_utts))
-        res = self.decode_raw_batch(utts, sessions, start_stream) if utts else []
+        res = self.decode_raw_batch(utts, sessions, start_stream, None if warp is None else [warp[i] for i in sessions]) \
+            if utts else []
         out, k = [], 0
         for ss in segs:
             row = []
@@ -156,19 +181,28 @@ class Decoder:
             out.append(row)
         return out
 
-    def _decode(self, utterances, sess_off, carry_noise=False):
+    def _decode(self, utterances, sess_off, carry_noise=False, warp=None):
         import torch
         g = self.search
         info = g["info"]
         off = api.FrontEnd.sample_offsets([len(u) for u in utterances])
         pcm = np.concatenate([np.ascontiguousarray(u, np.int16) for u in utterances]) if utterances else np.zeros(0, np.int16)
-        if sess_off is not None:
-            self.fe.set_sessions(sess_off)
-            if carry_noise:
-                starts = np.zeros(len(utterances), bool)
-                starts[np.asarray(sess_off[:-1])[np.diff(sess_off) > 0]] = True
-                self.fe.set_stream_starts(starts)
-        frame_off, best, pen = self.batch.decode_pcm_host(self.fe, self.phoneloop, pcm, off)
+        # the banks are built (and a refused warp raises) before anything is named for the front end's next call;
+        # whatever is refused after that drops every setting, so none is left for a later call
+        banks = None if warp is None else self.fe.warp_filterbanks(warp)
+        try:
+            if sess_off is not None:
+                self.fe.set_sessions(sess_off)
+                if carry_noise:
+                    starts = np.zeros(len(utterances), bool)
+                    starts[np.asarray(sess_off[:-1])[np.diff(sess_off) > 0]] = True
+                    self.fe.set_stream_starts(starts)
+            if banks is not None:
+                self.fe.name_filterbanks(banks)
+            frame_off, best, pen = self.batch.decode_pcm_host(self.fe, self.phoneloop, pcm, off)
+        except BaseException:
+            self.fe.cancel_settings()
+            raise
         d_scr = self.batch.senscr_device_ptr()
         d_pen = (torch.from_numpy(np.ascontiguousarray(pen, np.int32)).to(torch.device("cuda", self.device))
                  if self.pl_window > 0 and len(pen) else None)
