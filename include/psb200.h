@@ -339,7 +339,13 @@ int psb_align_batch_host(psb_hmmctx_t *c, const int16_t *senscr, const int32_t *
  * [frames][n_sen], all senones.  Every detection the reference would pass to kws_detections_add
  * (:286-294) is returned as a row {frame, keyphrase, start frame, prob, ascr} in hits
  * [n_utt][cap_per_utt][5] (host), in the reference's order; n_hits[u] (host) counts them (rows past
- * cap_per_utt are dropped).  The host applies kws_detections_add unchanged. */
+ * cap_per_utt are dropped).  The host applies kws_detections_add unchanged.
+ * One CTA per utterance keeps the whole search state in shared memory, (2 N + 6) ints per HMM for
+ * N emitting states, so H = n_pl + kp_off[n_kp] is limited to
+ * (max opt-in shared memory per block / 4 - 96) / (2 N + 6): PSB_KWS_MAX_HMMS_3ST / _5ST on an
+ * H100 (227 KB).  A larger H is refused (PSB_ERR_ARG) with H and the limit in the message. */
+#define PSB_KWS_MAX_HMMS_3ST 4834
+#define PSB_KWS_MAX_HMMS_5ST 3626
 int psb_kws_batch_device(psb_hmmctx_t *c, const int16_t *d_senscr, const int32_t *utt_off, int32_t n_utt,
                          int32_t n_pl, const int32_t *pl_ssid, const int32_t *pl_tmat, int32_t n_kp,
                          const int32_t *kp_off, const int32_t *kp_thresh, const int32_t *kp_ssid,

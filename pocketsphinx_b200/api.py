@@ -246,6 +246,20 @@ class Batch:
               "psb_decode_batch_pcm_host")
         return (frame_off, best, pen, senscr) if want_senscr else (frame_off, best, pen)
 
+    def score_pcm(self, fe, pcm, samp_off):
+        """Audio in, senone scores out, all on the device: the front end's features go straight to the scorer and the
+        scores stay at senscr_device_ptr() (ready when this returns).  Returns frame_off int32 [n_utt+1]."""
+        pcm = np.ascontiguousarray(pcm, np.int16)
+        samp_off = np.ascontiguousarray(samp_off, np.int64)
+        n_utt = len(samp_off) - 1
+        frame_off = np.zeros(n_utt + 1, np.int32)
+        check(lib().psb_fe_process_host(fe.h, _p(pcm) if pcm.size else None, _p(samp_off), n_utt, None, None,
+                                        _p(frame_off)), "psb_fe_process_host")
+        if frame_off[-1]:
+            self.score_device(lib().psb_fe_device_feats(fe.h), frame_off)
+            self.sync()
+        return frame_off
+
     def close(self):
         if self.h:
             lib().psb_batch_free(self.h)
@@ -464,17 +478,27 @@ class HmmContext:
 
     def kws(self, d_senscr_ptr, utt_off, pl_ssid, pl_tmat, kp_off, kp_thresh, kp_ssid, kp_tmat, beam, plp, cap=None):
         """kws_search over a batch (scores on the device).  Returns a list of raw hit arrays
-        [n][5] = (frame, keyphrase, start frame, prob, ascr), one per utterance."""
+        [n][5] = (frame, keyphrase, start frame, prob, ascr), one per utterance, and the hit counts.
+        cap: hit rows per utterance, rows past it dropped (counted all the same).  By default the rows
+        start at two per frame (a frame has at most one per keyphrase, which for long lists would reserve
+        far more than is ever written) and a batch that overflows them is searched again with as many as
+        its fullest utterance needs."""
         utt_off = np.ascontiguousarray(utt_off, np.int32)
         a = [np.ascontiguousarray(x, np.int32) for x in (pl_ssid, pl_tmat, kp_off, kp_thresh, kp_ssid, kp_tmat)]
         n_utt, n_kp = len(utt_off) - 1, len(a[2]) - 1
-        if cap is None:
-            cap = max(1, int(np.diff(utt_off).max(initial=1)) * max(1, n_kp))
-        hits = np.zeros((max(1, n_utt), cap, 5), np.int32)
-        n_hits = np.zeros(max(1, n_utt), np.int32)
-        check(lib().psb_kws_batch_device(self.h, C.c_void_p(d_senscr_ptr), _p(utt_off), n_utt, len(a[0]), _p(a[0]), _p(a[1]),
-                                         n_kp, _p(a[2]), _p(a[3]), _p(a[4]), _p(a[5]), int(beam), int(plp), _p(hits), cap,
-                                         _p(n_hits)), "psb_kws_batch_device")
+        grow = cap is None
+        if grow:
+            cap = max(1, int(np.diff(utt_off).max(initial=1)) * min(2, max(1, n_kp)))
+        while True:
+            hits = np.zeros((max(1, n_utt), cap, 5), np.int32)
+            n_hits = np.zeros(max(1, n_utt), np.int32)
+            check(lib().psb_kws_batch_device(self.h, C.c_void_p(d_senscr_ptr), _p(utt_off), n_utt, len(a[0]), _p(a[0]),
+                                             _p(a[1]), n_kp, _p(a[2]), _p(a[3]), _p(a[4]), _p(a[5]), int(beam), int(plp),
+                                             _p(hits), cap, _p(n_hits)), "psb_kws_batch_device")
+            need = int(n_hits[:n_utt].max(initial=0))
+            if not grow or need <= cap:
+                break
+            cap = need
         return [hits[u, :min(int(n_hits[u]), cap)].copy() for u in range(n_utt)], n_hits[:n_utt].copy()
 
     def align(self, senscr, utt_off, ph_off, ssid, tmatid, sf=None, ef=None, device_ptr=None):

@@ -1685,18 +1685,46 @@ extern "C" int psb_align_batch_host(psb_hmmctx_t *c, const int16_t *senscr, cons
 // ---------------------------------------------------------------------------------------
 // Keyword spotting: kws_search.c on the device for whole batches (SURVEY 8 row b5 lists its
 // kws_search_hmm_eval, kws_search.c:194).  One CTA per utterance; the phone loop (all CI phones)
-// and the keyphrases' HMM chains sit side by side in shared memory (SoA); per frame
+// and the keyphrases' HMM chains sit side by side in shared memory (SoA), each thread striding over
+// any number of them; the CTA is sized from H (kws_threads).  Per frame
 // kws_search_hmm_eval (:194-229), kws_search_hmm_prune (:234-251) and kws_search_trans (:256-348):
 // first-best exit score of the phone loop, detections, phone-loop re-entry, chain transitions
 // (decided from the state BEFORE any entry of this frame, which is what the reference's reverse
-// loop order achieves) and the chains' start from the phone loop.  Every detection the reference
-// would pass to kws_detections_add comes back as a row (frame, keyphrase, start frame, prob, ascr)
-// in the reference's order; the host applies the unchanged list logic (kws_detections.c:55-80).
+// loop order achieves: the decisions go to shared memory, a barrier, then they are applied) and the
+// chains' start from the phone loop.  Every detection the reference would pass to
+// kws_detections_add comes back as a row (frame, keyphrase, start frame, prob, ascr) in the
+// reference's order: each thread owns a contiguous run of keyphrases and a block scan of the
+// per-thread counts places its rows, so a frame's rows are in keyphrase order.  The host applies
+// the unchanged list logic (kws_detections.c:55-80).
 namespace {
 
 constexpr int KWS_MAX_SCORE = 1500;         // KWS_MAX, kws_search.c:59
+constexpr int KWS_NO_ENTRY = INT_MIN;       // pending-entry history of an HMM nothing enters this frame
 
-__global__ void __launch_bounds__(128)
+// exclusive prefix sum over the block (blockDim.x a multiple of 32); *total gets the sum.  wsum: [32]
+__device__ __forceinline__ int block_exclusive_scan(int v, int *wsum, int *total)
+{
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    int x = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int y = __shfl_up_sync(0xffffffffu, x, o);
+        if (lane >= o) x += y;
+    }
+    __syncthreads();
+    if (lane == 31) wsum[warp] = x;
+    __syncthreads();
+    int before = 0, all = 0;
+    for (int w = 0; w < nw; ++w) {
+        const int s = wsum[w];
+        if (w < warp) before += s;
+        all += s;
+    }
+    *total = all;
+    return before + x - v;
+}
+
+__global__ void __launch_bounds__(1024)
 kws_kernel(const int16_t *__restrict__ senscr, const int32_t *__restrict__ utt_off, HmmCtxDev c,
            int n_pl, int n_kp, const int32_t *__restrict__ kp_off, const int32_t *__restrict__ kp_thresh,
            const uint16_t *__restrict__ senid_g, const int32_t *__restrict__ tmatid_g, const int32_t *__restrict__ kp_of,
@@ -1713,11 +1741,17 @@ kws_kernel(const int16_t *__restrict__ senscr, const int32_t *__restrict__ utt_o
     int *out_hist = out_score + H;         // [H]
     int *bestsc = out_hist + H;            // [H]
     int *frame = bestsc + H;               // [H]
-    int *sval = frame + H;                 // [32]
+    int *ent_sc = frame + H;               // [H] this frame's pending hmm_enter: score
+    int *ent_hi = ent_sc + H;              // [H] ... and history (KWS_NO_ENTRY: none)
+    int *sval = ent_hi + H;                // [32]
     int *sidx = sval + 32;                 // [32]
+    int *wsum = sidx + 32;                 // [32]
     const HmmSoA<> V{score, hist, out_score, out_hist, bestsc, H};
     int32_t *my_hits = hits + (size_t)u * cap * 5;
     int nh = 0;
+    // this thread's keyphrases for the detections: a contiguous run, so the block scan keeps list order
+    const int kp_per = (n_kp + (int)blockDim.x - 1) / (int)blockDim.x;
+    const int k0 = min(n_kp, tid * kp_per), k1 = min(n_kp, k0 + kp_per);
 
     // kws_search_reinit: hmm_init (= hmm_clear); kws_search_start: phone loop hmm_clear + hmm_enter(0, -1, 0)
     for (int i = tid; i < H; i += blockDim.x) {
@@ -1758,49 +1792,56 @@ kws_kernel(const int16_t *__restrict__ senscr, const int32_t *__restrict__ utt_o
         __syncthreads();
         if (cand > PSB_WORST_SCORE) {                                     // else "out probs are not ready yet"
             const int plb_out = cand, plb_hist = out_hist[plb];
-            // detections, in keyphrase order
-            if (tid == 0)
-                for (int k = 0; k < n_kp; ++k) {
-                    if (kp_off[k + 1] - kp_off[k] < 1) continue;
+            // detections, in keyphrase order: count this thread's, place them by the block scan, write
+            int mine = 0;
+            for (int k = k0; k < k1; ++k) {
+                const int last = n_pl + kp_off[k + 1] - 1;
+                mine += kp_off[k + 1] > kp_off[k] && frame[last] > 0 && out_score[last] - plb_out >= kp_thresh[k];
+            }
+            int total;
+            int at = nh + block_exclusive_scan(mine, wsum, &total);
+            if (mine)
+                for (int k = k0; k < k1; ++k) {
                     const int last = n_pl + kp_off[k + 1] - 1;
-                    if (frame[last] > 0 && out_score[last] - plb_out >= kp_thresh[k]) {
-                        if (nh < cap) {
-                            int32_t *hrow = my_hits + (size_t)nh * 5;
+                    if (kp_off[k + 1] > kp_off[k] && frame[last] > 0 && out_score[last] - plb_out >= kp_thresh[k]) {
+                        if (at < cap) {
+                            int32_t *hrow = my_hits + (size_t)at * 5;
                             hrow[0] = t; hrow[1] = k; hrow[2] = out_hist[last];
                             hrow[3] = out_score[last] - plb_out - KWS_MAX_SCORE; hrow[4] = out_score[last];
                         }
-                        ++nh;
+                        ++at;
                     }
                 }
+            nh += total;
             // transitions: decide from the pre-entry state, then apply
-            int e_sc[4], e_hi[4];
-            bool e_on[4];
-            int q = 0;
-            for (int i = tid; i < H; i += blockDim.x, ++q) {
-                bool on = false; int sc = 0, hi = 0;
+            for (int i = tid; i < H; i += blockDim.x) {
+                int sc = 0, hi = KWS_NO_ENTRY;
                 if (i < n_pl) {                                            // phone-loop re-entry (:303-311)
-                    if (plb_out + plp > score[i]) { on = true; sc = plb_out + plp; hi = plb_hist; }
+                    if (plb_out + plp > score[i]) { sc = plb_out + plp; hi = plb_hist; }
                 }
                 else {
                     const int j = i - n_pl, k = kp_of[j];
                     if (j > kp_off[k]) {                                   // inside a chain (:320-332)
                         if (frame[i - 1] > 0 && (!(frame[i] > 0) || out_score[i - 1] > score[i])) {
-                            on = true; sc = out_score[i - 1]; hi = out_hist[i - 1];
+                            sc = out_score[i - 1]; hi = out_hist[i - 1];
                         }
                     }
-                    else if (plb_out > score[i]) { on = true; sc = plb_out; hi = t; }   // chain start (:335-340)
+                    else if (plb_out > score[i]) { sc = plb_out; hi = t; }  // chain start (:335-340)
                 }
-                if (q < 4) { e_on[q] = on; e_sc[q] = sc; e_hi[q] = hi; }
+                ent_sc[i] = sc; ent_hi[i] = hi;
             }
             __syncthreads();
-            q = 0;
-            for (int i = tid; i < H; i += blockDim.x, ++q)
-                if (q < 4 && e_on[q]) { score[i] = e_sc[q]; hist[i] = e_hi[q]; frame[i] = t + 1; }   // hmm_enter
+            for (int i = tid; i < H; i += blockDim.x)
+                if (ent_hi[i] != KWS_NO_ENTRY) { score[i] = ent_sc[i]; hist[i] = ent_hi[i]; frame[i] = t + 1; }   // hmm_enter
         }
         __syncthreads();
     }
     if (tid == 0) n_hits[u] = nh;
 }
+
+// the CTA: one thread per HMM up to 1024, at least four warps, whole warps (the reductions and scan want them)
+int kws_threads(int H) { return std::min(1024, std::max(128, (H + 31) / 32 * 32)); }
+size_t kws_smem(int N, int H) { return ((size_t)(2 * N + 6) * H + 96) * sizeof(int); }
 
 }  // namespace
 
@@ -1820,8 +1861,14 @@ extern "C" int psb_kws_batch_device(psb_hmmctx_t *c, const int16_t *d_senscr, co
         PSB_REQUIRE(kp_off[k + 1] >= kp_off[k], "psb_kws_batch_device: kp_off not monotone at %d", k);
     const int N = c->n_emit, n_k = kp_off[n_kp], H = n_pl + n_k;
     PSB_REQUIRE((n_kp == 0 || kp_thresh) && (n_k == 0 || (kp_ssid && kp_tmat)), "psb_kws_batch_device: keyphrase tables missing");
-    PSB_REQUIRE(H <= 4 * 128, "psb_kws_batch_device: %d HMMs exceed the 512 this kernel keeps per utterance", H);
     PSB_CUDA(cudaSetDevice(c->device));
+    int smem_max = 0;
+    PSB_CUDA(cudaDeviceGetAttribute(&smem_max, cudaDevAttrMaxSharedMemoryPerBlockOptin, c->device));
+    const size_t smem = kws_smem(N, H);
+    // the largest H whose state fits one CTA's shared memory (PSB_KWS_MAX_HMMS in psb200.h)
+    const int h_max = (int)(((size_t)smem_max / sizeof(int) - 96) / (2 * N + 6));
+    PSB_REQUIRE(H <= h_max, "psb_kws_batch_device: %d HMMs (%d phone-loop phones + %d keyphrase phones) exceed the %d "
+                "one CTA's shared memory holds at %d states per HMM", H, n_pl, n_k, h_max, N);
     std::vector<uint16_t> senid((size_t)H * N);      // the phone loop, then the keyphrases' chains
     rc = ctx_senids(c, "psb_kws_batch_device (phone loop)", n_pl, pl_ssid, pl_tmat, senid.data(), N, 1);
     if (rc) return rc;
@@ -1841,7 +1888,6 @@ extern "C" int psb_kws_batch_device(psb_hmmctx_t *c, const int16_t *d_senscr, co
         for (int j = kp_off[k]; j < kp_off[k + 1]; ++j) ibuf.push_back(k);
     const size_t o_nh = ibuf.size();
     ibuf.resize(o_nh + (size_t)n_utt, 0);
-    const size_t smem = ((size_t)(2 * N + 4) * H + 64) * sizeof(int);
     int32_t *d_i = nullptr, *d_hits = nullptr;
     uint16_t *d_senid = nullptr;
     const size_t hits_n = (size_t)n_utt * cap_per_utt * 5;
@@ -1854,8 +1900,9 @@ extern "C" int psb_kws_batch_device(psb_hmmctx_t *c, const int16_t *d_senscr, co
     if (e == cudaSuccess) e = cudaMemcpyAsync(d_senid, senid.data(), senid.size() * 2, cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(kws_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e == cudaSuccess)
-        kws_kernel<<<(unsigned)n_utt, 128, smem, st>>>(d_senscr, d_i, dev_ctx(c), n_pl, n_kp, d_i + o_kpoff, d_i + o_thr, d_senid,
-                                                      d_i + o_tm, d_i + o_of, beam, plp, d_hits, cap_per_utt, d_i + o_nh);
+        kws_kernel<<<(unsigned)n_utt, kws_threads(H), smem, st>>>(d_senscr, d_i, dev_ctx(c), n_pl, n_kp, d_i + o_kpoff,
+                                                                  d_i + o_thr, d_senid, d_i + o_tm, d_i + o_of, beam, plp,
+                                                                  d_hits, cap_per_utt, d_i + o_nh);
     return ctx_finish(c, "psb_kws_batch_device", e, 1, {{hits, d_hits, hits_n * 4}, {n_hits, d_i + o_nh, (size_t)n_utt * 4}});
 }
 

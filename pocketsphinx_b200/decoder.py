@@ -30,54 +30,63 @@ def _logs(p, logbase=1.0001):
     return (-(1 << 31) >> 2 if p <= 0 else int(math.log(p) * (1.0 / math.log(logbase)))) >> 10
 
 
+def acoustic_setup(hmm, cfg, device=0):
+    """The acoustic model and the device front end for -hmm `hmm` and the reference-named settings cfg (strings), as
+    ps_init configures them: the model's own settings (varfloor, tmatfloor, mixwfloor, topn, ds, aw); the front end
+    from the reference's defaults (config_macro.h), overlaid by the model's feat.params, then by cfg.  Returns
+    (PackedModel, api.FrontEnd, the front-end settings in force)."""
+    pm = PackedModel.from_dir(hmm, **{k: v for k, v in cfg.items() if k in ("varfloor", "tmatfloor", "mixwfloor", "topn", "ds", "aw")})
+    # front end: the reference's own defaults (config_macro.h), overlaid by the model's feat.params, then by the
+    # caller -- like ps_init; whatever the device front end does not implement is refused, not ignored
+    from .s3io import read_feat_params
+    fp = dict(FE_REFERENCE_DEFAULTS)
+    fp.update(read_feat_params(os.path.join(hmm, "feat.params")))
+    fp.update({k: v for k, v in cfg.items() if k in FE_REFERENCE_DEFAULTS})
+    yes = ("yes", "1", "true", "True")
+    unsupported = []
+    if fp["feat"] not in FEAT_TYPES: unsupported.append("-feat " + fp["feat"])
+    if fp["cmn"] not in CMN_TYPES: unsupported.append("-cmn " + fp["cmn"])
+    if fp["agc"] not in AGC_TYPES: unsupported.append("-agc " + fp["agc"])
+    if fp["varnorm"] in yes and CMN_TYPES.get(fp["cmn"]) != 1: unsupported.append("-varnorm yes with -cmn " + fp["cmn"])
+    if fp["svspec"] not in ("", "0-12/13-25/26-38"): unsupported.append("-svspec " + fp["svspec"])
+    if int(fp["ncep"]) != 13: unsupported.append("-ncep " + fp["ncep"])
+    if int(fp["frate"]) != 100: unsupported.append("-frate " + fp["frate"])
+    if int(fp["nfft"]) != 0: unsupported.append("-nfft " + fp["nfft"])
+    if unsupported:
+        raise NotImplementedError("front end settings the device front end does not implement: " + ", ".join(unsupported))
+    # -lda defaults to the model's feature_transform when there is one (ps_expand_model_config, pocketsphinx.c:119)
+    if not fp["lda"] and os.path.exists(os.path.join(hmm, "feature_transform")):
+        fp["lda"] = os.path.join(hmm, "feature_transform")
+    if fp["lda"] and fp["svspec"]:
+        # feat_dimension2 is the LDA output for every subvector, which no model's streams match (acmod_init fails)
+        raise ValueError("-lda %s with -svspec %s: the reference cannot load this model either" % (fp["lda"], fp["svspec"]))
+    lda = s3io.read_lda(fp["lda"])[0] if fp["lda"] else None
+    opts = make_fe_opts(feat=fp["feat"], cmn=fp["cmn"], cmninit=fp["cmninit"], dither=fp["dither"] in yes,
+                        seed=int(fp["seed"]), ncep=int(fp["ncep"]), varnorm=fp["varnorm"] in yes, agc=fp["agc"],
+                        agcthresh=float(fp["agcthresh"]), lda=lda, ldadim=int(fp["ldadim"]))
+    desc = make_fe_desc(samprate=float(fp["samprate"]), wlen=float(fp["wlen"]), nfilt=int(fp["nfilt"]),
+                        lowerf=float(fp["lowerf"]), upperf=float(fp["upperf"]), alpha=float(fp["alpha"]),
+                        transform=fp["transform"], lifter=int(fp["lifter"]), remove_noise=fp["remove_noise"] in yes,
+                        remove_dc=fp["remove_dc"] in yes, unit_area=fp["unit_area"] in yes,
+                        round_filters=fp["round_filters"] in yes, doublebw=fp["doublebw"] in yes,
+                        warp_type=fp["warp_type"], warp_params=fp["warp_params"] or None)
+    # 1s_c_d_dd with batch CMN and nothing else is the front end desc alone describes
+    plain = (opts["feat"], opts["cmn"], opts["dither"], opts["varnorm"], opts["agc"], lda is None) == (0, 1, 0, 0, 0, True)
+    # the dimension psb_fe_feat_dim will report: feat_read_lda's out_dim, else the feature type's
+    dim = 51 if opts["feat"] == 1 else 3 * int(fp["ncep"])
+    if lda is not None:
+        dim = opts["ldadim"] if 0 < opts["ldadim"] <= lda.shape[0] else lda.shape[0]
+    if dim != pm.sumlen:
+        raise ValueError("the front end makes %d-dimensional features (-feat %s%s), the model in %s wants %d"
+                         % (dim, fp["feat"], ", -lda %s" % fp["lda"] if fp["lda"] else "", hmm, pm.sumlen))
+    fe = api.FrontEnd(desc, device) if plain else api.FrontEnd(desc, device, opts)
+    return pm, fe, fp
+
+
 class Decoder:
     def __init__(self, hmm, dict_file, lm_file, max_utts=64, max_frames=1 << 16, device=0, **config):
         cfg = {k: str(v) for k, v in config.items()}
-        self.pm = PackedModel.from_dir(hmm, **{k: v for k, v in cfg.items() if k in ("varfloor", "tmatfloor", "mixwfloor", "topn", "ds", "aw")})
-        # front end: the reference's own defaults (config_macro.h), overlaid by the model's feat.params, then by the
-        # caller -- like ps_init; whatever the device front end does not implement is refused, not ignored
-        from .s3io import read_feat_params
-        fp = dict(FE_REFERENCE_DEFAULTS)
-        fp.update(read_feat_params(os.path.join(hmm, "feat.params")))
-        fp.update({k: v for k, v in cfg.items() if k in FE_REFERENCE_DEFAULTS})
-        yes = ("yes", "1", "true", "True")
-        unsupported = []
-        if fp["feat"] not in FEAT_TYPES: unsupported.append("-feat " + fp["feat"])
-        if fp["cmn"] not in CMN_TYPES: unsupported.append("-cmn " + fp["cmn"])
-        if fp["agc"] not in AGC_TYPES: unsupported.append("-agc " + fp["agc"])
-        if fp["varnorm"] in yes and CMN_TYPES.get(fp["cmn"]) != 1: unsupported.append("-varnorm yes with -cmn " + fp["cmn"])
-        if fp["svspec"] not in ("", "0-12/13-25/26-38"): unsupported.append("-svspec " + fp["svspec"])
-        if int(fp["ncep"]) != 13: unsupported.append("-ncep " + fp["ncep"])
-        if int(fp["frate"]) != 100: unsupported.append("-frate " + fp["frate"])
-        if int(fp["nfft"]) != 0: unsupported.append("-nfft " + fp["nfft"])
-        if unsupported:
-            raise NotImplementedError("front end settings the device front end does not implement: " + ", ".join(unsupported))
-        # -lda defaults to the model's feature_transform when there is one (ps_expand_model_config, pocketsphinx.c:119)
-        if not fp["lda"] and os.path.exists(os.path.join(hmm, "feature_transform")):
-            fp["lda"] = os.path.join(hmm, "feature_transform")
-        if fp["lda"] and fp["svspec"]:
-            # feat_dimension2 is the LDA output for every subvector, which no model's streams match (acmod_init fails)
-            raise ValueError("-lda %s with -svspec %s: the reference cannot load this model either" % (fp["lda"], fp["svspec"]))
-        lda = s3io.read_lda(fp["lda"])[0] if fp["lda"] else None
-        opts = make_fe_opts(feat=fp["feat"], cmn=fp["cmn"], cmninit=fp["cmninit"], dither=fp["dither"] in yes,
-                            seed=int(fp["seed"]), ncep=int(fp["ncep"]), varnorm=fp["varnorm"] in yes, agc=fp["agc"],
-                            agcthresh=float(fp["agcthresh"]), lda=lda, ldadim=int(fp["ldadim"]))
-        desc = make_fe_desc(samprate=float(fp["samprate"]), wlen=float(fp["wlen"]), nfilt=int(fp["nfilt"]),
-                            lowerf=float(fp["lowerf"]), upperf=float(fp["upperf"]), alpha=float(fp["alpha"]),
-                            transform=fp["transform"], lifter=int(fp["lifter"]), remove_noise=fp["remove_noise"] in yes,
-                            remove_dc=fp["remove_dc"] in yes, unit_area=fp["unit_area"] in yes,
-                            round_filters=fp["round_filters"] in yes, doublebw=fp["doublebw"] in yes,
-                            warp_type=fp["warp_type"], warp_params=fp["warp_params"] or None)
-        # 1s_c_d_dd with batch CMN and nothing else is the front end desc alone describes
-        plain = (opts["feat"], opts["cmn"], opts["dither"], opts["varnorm"], opts["agc"], lda is None) == (0, 1, 0, 0, 0, True)
-        # the dimension psb_fe_feat_dim will report: feat_read_lda's out_dim, else the feature type's
-        dim = 51 if opts["feat"] == 1 else 3 * int(fp["ncep"])
-        if lda is not None:
-            dim = opts["ldadim"] if 0 < opts["ldadim"] <= lda.shape[0] else lda.shape[0]
-        if dim != self.pm.sumlen:
-            raise ValueError("the front end makes %d-dimensional features (-feat %s%s), the model in %s wants %d"
-                             % (dim, fp["feat"], ", -lda %s" % fp["lda"] if fp["lda"] else "", hmm, self.pm.sumlen))
-        self.fe = api.FrontEnd(desc, device) if plain else api.FrontEnd(desc, device, opts)
+        self.pm, self.fe, fp = acoustic_setup(hmm, cfg, device)
         search_cfg = {k: v for k, v in cfg.items() if k in lextree.DEFAULTS}
         self.search = lextree.ngram_search_from_files(hmm, dict_file, lm_file, **search_cfg)
         self.model = api.Model(self.pm, device)
