@@ -181,12 +181,20 @@ class RefModel:
     def mfcc(self, pcm):
         """Cepstra before CMN from a fresh stream (noise tracker reset)."""
         pcm = np.ascontiguousarray(pcm, np.int16)
-        cap = len(pcm) // 160 + 16
         i = np.zeros(16, np.int32); f = np.zeros(4, np.float32)
         lib().refdrv_fe_info(self.h, _p(i), _p(f))
+        cap = len(pcm) // int(i[1]) + 16                    # more frames than the frame shift allows
         out = np.zeros((cap, int(i[5])), np.float32)
         T = lib().refdrv_mfcc(self.h, _p(pcm), len(pcm), _p(out), cap)
+        if T > cap:
+            raise RuntimeError("refdrv_mfcc made %d frames, more than the %d sized for" % (T, cap))
         return out[:T].copy()
+
+    def _frame_cap(self, n_samples):
+        """More frames than n_samples can make at this front end's own frame shift."""
+        i = np.zeros(16, np.int32); f = np.zeros(4, np.float32)
+        lib().refdrv_fe_info(self.h, _p(i), _p(f))
+        return n_samples // int(i[1]) + 16
 
     def featurize_fresh(self, pcm):
         """featurize() as the first utterance of a fresh stream (noise tracker reset first)."""
@@ -195,9 +203,11 @@ class RefModel:
 
     def featurize(self, pcm, max_frames=None):
         pcm = np.ascontiguousarray(pcm, np.int16)
-        cap = max_frames or (len(pcm) // 160 + 16)
+        cap = max_frames or self._frame_cap(len(pcm))
         out = np.zeros((cap, self.sumlen), np.float32)
         T = lib().refdrv_featurize(self.h, _p(pcm), len(pcm), _p(out), cap)
+        if T > cap and not max_frames:
+            raise RuntimeError("refdrv_featurize made %d frames, more than the %d sized for" % (T, cap))
         return out[:min(T, cap)].copy()
 
     def score(self, feats, reset=True, want_topn=False):
