@@ -318,13 +318,17 @@ int psb_batch_set_pipeline(psb_batch_t *b, int n);
  * per-phone alignment constraints of state_align_search_init (:462-469), NULL = always active.
  * Outputs per emitting state (index = phone * n_emit_state + j, ps_alignment_entry_t): start,
  * duration, score; -1 where the backtrace never visits the state.  status[u]: 0, -1 ("Failed to
- * reach final state"), -2 - frame ("Alignment failed in frame").  All arrays but d_senscr: host. */
+ * reach final state"), -2 - frame ("Alignment failed in frame").  All arrays but d_senscr: host.
+ * Tokens are kept only for the phones that can be active in each frame, a band that follows from sf / ef alone
+ * (DESIGN 4.7): with windows the arena grows with frames, without them it is frames x phones x states. */
 int psb_align_batch_device(psb_hmmctx_t *c, const int16_t *d_senscr, const int32_t *utt_off,
                            int32_t n_utt, const int32_t *ph_off, const int32_t *ssid,
                            const int32_t *tmatid, const int32_t *sf, const int32_t *ef,
                            int32_t *st_start, int32_t *st_dur, int32_t *st_score, int32_t *status);
 /* device time (CUDA events on the context's stream) of the last psb_align_batch_* kernel */
 float psb_align_last_kernel_ms(const psb_hmmctx_t *c);
+/* bytes of the token arena (ids and scores) the last psb_align_batch_* call used */
+int64_t psb_align_last_token_bytes(const psb_hmmctx_t *c);
 int psb_align_batch_host(psb_hmmctx_t *c, const int16_t *senscr, const int32_t *utt_off,
                          int32_t n_utt, const int32_t *ph_off, const int32_t *ssid,
                          const int32_t *tmatid, const int32_t *sf, const int32_t *ef,

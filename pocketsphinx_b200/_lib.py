@@ -130,6 +130,7 @@ SYMBOLS = [
                                                    _VP, _VP, _VP]),
     ("psb_align_batch_device", C.c_int, [_VP, _VP, _VP, _I32, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP]),
     ("psb_align_last_kernel_ms", C.c_float, [_VP]),
+    ("psb_align_last_token_bytes", C.c_int64, [_VP]),
     ("psb_align_batch_host", C.c_int, [_VP, _VP, _VP, _I32, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP]),
     ("psb_fe_create", C.c_int, [C.POINTER(FeDesc), C.c_int, C.POINTER(_VP)]),
     ("psb_fe_free", None, [_VP]),

@@ -1450,7 +1450,8 @@ __global__ void __launch_bounds__(128)
 align_kernel(const int16_t *__restrict__ senscr, const int32_t *__restrict__ utt_off, HmmCtxDev c,
              const int32_t *__restrict__ ph_off, const uint16_t *__restrict__ senid_g,
              const int32_t *__restrict__ tmatid_g, const int32_t *__restrict__ sf_g, const int32_t *__restrict__ ef_g,
-             int32_t *__restrict__ tok_id, int32_t *__restrict__ tok_sc, const int64_t *__restrict__ tok_off,
+             int32_t *__restrict__ tok_id, int32_t *__restrict__ tok_sc, const int64_t *__restrict__ tok_row,
+             const int32_t *__restrict__ band_lo, const int32_t *__restrict__ band_hi,
              int32_t *__restrict__ st_start, int32_t *__restrict__ st_dur, int32_t *__restrict__ st_score,
              int32_t *__restrict__ status)
 {
@@ -1468,7 +1469,8 @@ align_kernel(const int16_t *__restrict__ senscr, const int32_t *__restrict__ utt
     int *sval = frame + H;                 // [32]
     int *sidx = sval + 32;                 // [32]
     const HmmSoA<false> V{score, hist, out_score, out_hist, nullptr, H};
-    int32_t *tid_u = tok_id + tok_off[u], *tsc_u = tok_sc + tok_off[u];
+    const int64_t *row_u = tok_row + f0;
+    const int32_t *lo_u = band_lo + f0, *hi_u = band_hi + f0;
     int32_t *ss = st_start + (size_t)p0 * N, *sd = st_dur + (size_t)p0 * N, *sc = st_score + (size_t)p0 * N;
 
     for (int i = tid; i < n_st; i += blockDim.x) { ss[i] = -1; sd[i] = -1; sc[i] = -1; }
@@ -1536,9 +1538,11 @@ align_kernel(const int16_t *__restrict__ senscr, const int32_t *__restrict__ utt
             }
         }
         __syncthreads();
-        // record_transitions
-        int32_t *ti = tid_u + (size_t)t * n_st, *ts = tsc_u + (size_t)t * n_st;
-        for (int i = tid; i < H; i += blockDim.x) {
+        // record_transitions, into this frame's row of the arena: phones lo_t .. hi_t, the only ones that can be
+        // active now (psb_align_batch_device: align_band)
+        const int lo = lo_u[t], hi = hi_u[t];
+        int32_t *ti = tok_id + row_u[t] - (int64_t)lo * N, *ts = tok_sc + row_u[t] - (int64_t)lo * N;
+        for (int i = lo + tid; i <= hi; i += blockDim.x) {
             const bool on = frame[i] >= t;
             for (int s = 0; s < N; ++s) {
                 const int idx = i * N + s;
@@ -1557,9 +1561,12 @@ align_kernel(const int16_t *__restrict__ senscr, const int32_t *__restrict__ utt
         else {
             int last_frame = T;
             for (int cf = T - 2; cf >= 0; --cf) {
-                const int prev = cur_id;
-                cur_id = tid_u[(size_t)cf * n_st + prev];
-                cur_sc = tsc_u[(size_t)cf * n_st + prev];
+                // a token outside the frame's band is what the reference's 0xff memset leaves: id -1
+                const int prev = cur_id, i = prev / N;
+                if (i < lo_u[cf] || i > hi_u[cf]) { rc = -2 - cf; break; }
+                const int64_t k = row_u[cf] + (prev - lo_u[cf] * N);
+                cur_id = tok_id[k];
+                cur_sc = tok_sc[k];
                 if (cur_id == -1) { rc = -2 - cf; break; }
                 if (cur_id != last_id) {
                     ss[last_id] = cf + 1;
@@ -1577,6 +1584,30 @@ align_kernel(const int16_t *__restrict__ senscr, const int32_t *__restrict__ utt
 
 }  // namespace
 
+// The phones that can hold a token in each frame of one utterance (state_align_search has no beam: a phone leaves
+// only when nf > ef, :100, and is entered only when nf >= sf, :120).  lo_f is the first phone with ef >= f: a phone
+// whose window closes in frame f still records that frame's token (prune_hmms leaves its frame at f), and a phone
+// entered in frame f - 1 or f needs a predecessor that survived pruning there, whose ef is >= f.  Phone 0 holds the
+// start token in frame 0.  hi_f is the last phone i with sf[j] <= f + 1 for every 1 <= j <= i: a phone is entered
+// only from its predecessor, and the entry cascade within one frame stops at a window that is not open yet.  An empty
+// band has hi_f = lo_f - 1.  Returns the arena's size in tokens, rows of (hi_f - lo_f + 1) x n_emit.
+static int64_t align_band(int H, const int32_t *sf, const int32_t *ef, int T, int N, int32_t *lo_out, int32_t *hi_out,
+                          int64_t *row_out, int64_t row0)
+{
+    int lo = 0, hi = H > 0 ? 0 : -1;
+    int64_t n = 0;
+    for (int f = 0; f < T; ++f) {
+        if (f > 0)
+            while (lo < H && ef && ef[lo] < f) ++lo;
+        while (hi + 1 < H && (!sf || sf[hi + 1] <= f + 1)) ++hi;
+        const int h = std::max(hi, lo - 1);
+        lo_out[f] = lo; hi_out[f] = h;
+        row_out[f] = row0 + n;
+        n += (int64_t)(h - lo + 1) * N;
+    }
+    return n;
+}
+
 extern "C" int psb_align_batch_device(psb_hmmctx_t *c, const int16_t *d_senscr, const int32_t *utt_off, int32_t n_utt,
                                       const int32_t *ph_off, const int32_t *ssid, const int32_t *tmatid,
                                       const int32_t *sf, const int32_t *ef,
@@ -1590,38 +1621,44 @@ extern "C" int psb_align_batch_device(psb_hmmctx_t *c, const int16_t *d_senscr, 
     PSB_REQUIRE(ph_off[0] == 0, "psb_align_batch_device: offsets must start at 0");
     const int N = c->n_emit;
     const int total_ph = ph_off[n_utt];
+    const size_t n_frames = (size_t)utt_off[n_utt];
     PSB_REQUIRE(total_ph == 0 || (ssid && tmatid), "psb_align_batch_device: phones missing");
     PSB_CUDA(cudaSetDevice(c->device));
     std::vector<uint16_t> senid((size_t)std::max(total_ph, 1) * N);
-    std::vector<int64_t> tok_off((size_t)n_utt + 1);
     int max_h = 0;
-    tok_off[0] = 0;
     for (int u = 0; u < n_utt; ++u) {
-        const int H = ph_off[u + 1] - ph_off[u], T = utt_off[u + 1] - utt_off[u];
+        const int H = ph_off[u + 1] - ph_off[u];
         PSB_REQUIRE(H >= 0, "psb_align_batch_device: ph_off not monotone at %d", u);
         max_h = std::max(max_h, H);
-        tok_off[(size_t)u + 1] = tok_off[(size_t)u] + (int64_t)T * H * N;
     }
     rc = ctx_senids(c, "psb_align_batch_device", total_ph, ssid, tmatid, senid.data(), N, 1);
     if (rc) return rc;
     const size_t smem = ((size_t)(2 * N + 3) * max_h + 64) * sizeof(int);
     PSB_REQUIRE(smem <= 200 * 1024, "psb_align_batch_device: %d phones in one utterance do not fit shared memory", max_h);
     // workspace: one int32 block
-    //   utt_off | ph_off | tmatid | sf | ef | start | dur | score | status
-    // plus the token table (2 x frames x states), the senone ids and the token offsets
+    //   utt_off | ph_off | tmatid | sf | ef | start | dur | score | status | band lo | band hi   (the bands per frame)
+    // plus the token arena (ids, then scores), the senone ids and each frame's row offset in the arena
     const size_t n_state = (size_t)total_ph * N;
     const size_t o_utt = 0, o_ph = o_utt + n_utt + 1, o_tm = o_ph + n_utt + 1, o_sf = o_tm + total_ph, o_ef = o_sf + total_ph,
                  o_ss = o_ef + total_ph, o_sd = o_ss + n_state, o_sc = o_sd + n_state, o_st = o_sc + n_state,
-                 n_i32 = o_st + n_utt;
-    const size_t n_tok = (size_t)tok_off[(size_t)n_utt] * 2;
+                 o_lo = o_st + n_utt, o_hi = o_lo + n_frames, n_i32 = o_hi + n_frames;
+    std::vector<int32_t> band((size_t)2 * std::max<size_t>(n_frames, 1));
+    std::vector<int64_t> row(std::max<size_t>(n_frames, 1));
+    int64_t n_tok = 0;
+    for (int u = 0; u < n_utt; ++u) {
+        const int p0 = ph_off[u], f0 = utt_off[u];
+        n_tok += align_band(ph_off[u + 1] - p0, sf ? sf + p0 : nullptr, ef ? ef + p0 : nullptr, utt_off[u + 1] - f0, N,
+                            band.data() + f0, band.data() + n_frames + f0, row.data() + f0, n_tok);
+    }
     int32_t *d_i32 = nullptr, *d_tok = nullptr;
     uint16_t *d_senid = nullptr;
-    int64_t *d_tokoff = nullptr;
+    int64_t *d_row = nullptr;
     rc = srch_reserve(c, 0, n_i32, &d_i32);
-    if (!rc) rc = srch_reserve(c, 1, n_tok, &d_tok);
+    if (!rc) rc = srch_reserve(c, 1, (size_t)std::max<int64_t>(n_tok, 1) * 2, &d_tok);
     if (!rc) rc = srch_reserve(c, 2, senid.size(), &d_senid);
-    if (!rc) rc = srch_reserve(c, 3, tok_off.size(), &d_tokoff);
+    if (!rc) rc = srch_reserve(c, 3, row.size(), &d_row);
     if (rc) return rc;
+    c->last_align_tok_bytes = n_tok * 2 * (int64_t)sizeof(int32_t);
     cudaError_t e = cudaSuccess;
     if (!c->al_ev[0]) e = c->al_ev[0].create();
     if (e == cudaSuccess && !c->al_ev[1]) e = c->al_ev[1].create();
@@ -1631,15 +1668,18 @@ extern "C" int psb_align_batch_device(psb_hmmctx_t *c, const int16_t *d_senscr, 
     if (e == cudaSuccess && total_ph) e = cudaMemcpyAsync(d_i32 + o_tm, tmatid, (size_t)total_ph * 4, cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess && total_ph && sf) e = cudaMemcpyAsync(d_i32 + o_sf, sf, (size_t)total_ph * 4, cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess && total_ph && ef) e = cudaMemcpyAsync(d_i32 + o_ef, ef, (size_t)total_ph * 4, cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess && n_frames) e = cudaMemcpyAsync(d_i32 + o_lo, band.data(), n_frames * 4, cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess && n_frames)
+        e = cudaMemcpyAsync(d_i32 + o_hi, band.data() + n_frames, n_frames * 4, cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess) e = cudaMemcpyAsync(d_senid, senid.data(), senid.size() * 2, cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_tokoff, tok_off.data(), tok_off.size() * 8, cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_row, row.data(), row.size() * 8, cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(align_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e == cudaSuccess) e = cudaEventRecord(c->al_ev[0], st);
     if (e == cudaSuccess) {
         align_kernel<<<(unsigned)n_utt, 128, smem, st>>>(d_senscr, d_i32 + o_utt, dev_ctx(c), d_i32 + o_ph, d_senid, d_i32 + o_tm,
                                                         sf ? d_i32 + o_sf : nullptr, ef ? d_i32 + o_ef : nullptr, d_tok,
-                                                        d_tok + tok_off[(size_t)n_utt], d_tokoff, d_i32 + o_ss, d_i32 + o_sd,
-                                                        d_i32 + o_sc, d_i32 + o_st);
+                                                        d_tok + std::max<int64_t>(n_tok, 1), d_row, d_i32 + o_lo,
+                                                        d_i32 + o_hi, d_i32 + o_ss, d_i32 + o_sd, d_i32 + o_sc, d_i32 + o_st);
         e = cudaEventRecord(c->al_ev[1], st);
     }
     rc = ctx_finish(c, "psb_align_batch_device", e, 1,
@@ -1652,6 +1692,11 @@ extern "C" int psb_align_batch_device(psb_hmmctx_t *c, const int16_t *d_senscr, 
         return PSB_ERR_CUDA;
     }
     return PSB_OK;
+}
+
+extern "C" int64_t psb_align_last_token_bytes(const psb_hmmctx_t *c)
+{
+    return c ? c->last_align_tok_bytes : 0;
 }
 
 extern "C" float psb_align_last_kernel_ms(const psb_hmmctx_t *c)

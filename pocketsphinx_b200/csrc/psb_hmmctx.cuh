@@ -24,6 +24,7 @@ struct psb_hmmctx_s {
     HostBuf<int32_t> h_best;
     Event al_ev[2];               // around the last psb_align_batch_* kernel
     float last_align_ms;
+    int64_t last_align_tok_bytes; // the token arena of the last psb_align_batch_* call (ids and scores)
     // grow-only device workspace of the whole-utterance entry points (srch_reserve)
     DevBuf<unsigned char> srch[10];
 };

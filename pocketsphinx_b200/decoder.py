@@ -89,8 +89,18 @@ class Decoder:
         self.pm, self.fe, fp = acoustic_setup(hmm, cfg, device)
         search_cfg = {k: v for k, v in cfg.items() if k in lextree.DEFAULTS}
         self.search = lextree.ngram_search_from_files(hmm, dict_file, lm_file, **search_cfg)
+        # -phone_align / -state_align (pocketsphinx_main.c; -state_align implies -phone_align): a second pass aligns
+        # each utterance to its own word segments.  The alignment always has all three levels.
+        yes = ("yes", "1", "true", "True")
+        self.phone_align = cfg.get("phone_align", "no") in yes or cfg.get("state_align", "no") in yes
+        self.align_tables = None
+        if self.phone_align:
+            from .align import AlignTables
+            self.align_tables = AlignTables(hmm, dict_file)
         self.model = api.Model(self.pm, device)
-        self.batch = api.Batch(self.model, max_utts, max_frames)
+        # the second pass scores every utterance after a copy of itself (_align_pass): twice the frames
+        k = 2 if self.phone_align else 1
+        self.batch = api.Batch(self.model, max_utts * k, max_frames * k)
         self.ctx = api.HmmContext(self.pm.tp, self.pm.sseq, self.pm.n_sen, device=device)
         self.device = device
         pl = dict(PL_DEFAULTS)
@@ -115,7 +125,9 @@ class Decoder:
         calls ps_start_stream once before a session's first utterance and then only ps_start_utt, ps_process_raw,
         ps_end_utt, so the tracker carries from one utterance to the next.  Returns one dict per utterance: hyp (the
         words, fillers and <s> / </s> left out), score, seg [n][7] = entry, wid, sf, ef, path score, ascr, lscr, and
-        words().  warp: None, or one -warp_params string per utterance (under this decoder's -warp_type; None: the
+        words().  With phone_align / state_align each dict also has alignment (align.Alignment: the words, phones and
+        states of the second pass over seg; None where the reference's ps_set_alignment or search fails) and
+        alignment_error (that failure's reason, else None).  warp: None, or one -warp_params string per utterance (under this decoder's -warp_type; None: the
         decoder's own -warp_params), so each utterance is decoded with its own VTLN warp; the utterances of one session
         are one decoder's and must name the same warp."""
         if start_stream not in ("utterance", "session"):
@@ -246,7 +258,50 @@ class Decoder:
             seg = api.ngram_segments(info, g["model"], bp, bss, entry, lm_arrays=g["lm_arrays"], second_pass=self.second_pass)
             real = [words[base[w]] for w in seg[:, 1] if not (fs <= int(base[w]) <= fe_)]        # dict_real_word + dict_basestr
             out.append(dict(hyp=" ".join(real), score=score, seg=seg, words=[words[w] for w in seg[:, 1]], n_frames=T))
+        if self.phone_align:
+            self._align_pass(utterances, sess_off, carry_noise, warp, out)
         return out
+
+    def _align_pass(self, utterances, sess_off, carry_noise, warp, out):
+        """The second pass of `pocketsphinx single -phone_align yes` (decode_single, pocketsphinx_main.c:462-476):
+        ps_set_alignment(ps, NULL) turns the segments into timed words (ps_alignment_add_word(wid, sf, ef - sf + 1)),
+        and the same decoder decodes the same audio again, without ps_start_stream.  Its front end carries its state
+        (live CMN, the -remove_noise tracker, dither) from the first decode into the second, so the second pass is
+        scored as the utterance's own repeat in its session: every utterance is followed by a copy of itself, the
+        copies are aligned, the originals get no phones."""
+        from .align import align_batch
+        n = len(utterances)
+        lens = np.repeat([len(u) for u in utterances], 2)
+        pcm2 = (np.concatenate([np.ascontiguousarray(u, np.int16) for u in utterances for _ in (0, 1)]) if n
+                else np.zeros(0, np.int16))
+        sess2 = np.arange(0, 2 * n + 1, 2, dtype=np.int32) if sess_off is None else 2 * np.asarray(sess_off, np.int32)
+        starts = np.zeros(2 * n, bool)
+        if carry_noise:
+            starts[sess2[:-1][np.diff(sess2) > 0]] = True
+        else:
+            starts[0::2] = True
+        banks = None if warp is None else self.fe.warp_filterbanks([w for w in warp for _ in (0, 1)])
+        try:
+            self.fe.set_sessions(sess2)
+            self.fe.set_stream_starts(starts)
+            if banks is not None:
+                self.fe.name_filterbanks(banks)
+            frame_off = self.batch.score_pcm(self.fe, pcm2, api.FrontEnd.sample_offsets(lens))
+        except BaseException:
+            self.fe.cancel_settings()
+            raise
+        chains = []
+        for d in out:
+            seg = d["seg"]
+            # ps_seg_iter returns NULL for no segments, and ps_set_alignment fails
+            chains += [None, (seg[:, 1].tolist(), seg[:, 2].astype(np.int64), (seg[:, 3] - seg[:, 2] + 1).astype(np.int64))
+                       if len(seg) else None]
+        res, self.last_align_token_bytes = align_batch(self.ctx, self.align_tables, self.batch.senscr_device_ptr(),
+                                                       frame_off, chains, windows=True)
+        for u, d in enumerate(out):
+            a, why = res[2 * u + 1]
+            d["alignment"] = a
+            d["alignment_error"] = why if chains[2 * u + 1] is not None else "no word segments to align"
 
     def close(self):
         for o in (self.phoneloop, self.batch, self.ctx, self.model, self.fe):
