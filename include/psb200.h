@@ -151,6 +151,16 @@ int psb_batch_tc_check(psb_batch_t *b, float *ratio, int32_t *max_candidates, in
  * CTA and its CTAs per codebook-stream pair. */
 #define PSB_TC_N_COUNTERS 15
 int psb_batch_tc_counters(psb_batch_t *b, int64_t *out, int32_t n);
+/* debugging/tests: how a batch of total_frames frames on an ms model is scored -- the plan the batch launcher runs.
+ * out[0..n-1] receives the first n of, in order: tiled distances (1) or streamed (0); senones evaluated inside
+ * the tile kernel; the tile kernel's register prefetch of the next block's features (0: staged in place); list
+ * width (the next power of two >= topn); list entries a senone reads (topn clamped to the Gaussians); every
+ * Gaussian listed in order (1) or a sorted top-N (0); frames per CTA of the tile kernel in the first chunk;
+ * codebook tiles of 32; frames per chunk; chunks; list-buffer bytes (0 for fused plans); SMs of the device;
+ * weights transposed (one shared codebook); the tile kernel's dynamic shared memory in bytes.  A -topn the
+ * batch kernels refuse is refused here too. */
+#define PSB_MS_PLAN_N 14
+int psb_batch_ms_plan(psb_batch_t *b, int64_t total_frames, int64_t *out, int32_t n);
 /* debugging/parity: copy the per-frame top-N records of the last call to the host:
  * rec int32 [total_frames][n_mgau*n_feat][4] = {top>>10, cw[4] bytes, e[4] bytes, 0} */
 int psb_batch_get_topn(psb_batch_t *b, int32_t *rec, int64_t n_frames);

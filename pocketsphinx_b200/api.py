@@ -214,6 +214,15 @@ class Batch:
         self.tc_stats = {k: int(v) for k, v in zip(self.TC_COUNTERS, st)}
         return r.value, n.value
 
+    MS_PLAN = ("tile", "fuse", "prefetch", "nt", "n_used", "all", "frames_per_cta", "tiles_x", "chunk", "n_chunks",
+               "dist_bytes", "n_sm", "transposed", "tile_smem")
+
+    def ms_plan(self, total_frames):
+        """How a batch of total_frames frames on an ms model is scored (psb_batch_ms_plan), by name."""
+        v = np.zeros(len(self.MS_PLAN), np.int64)
+        check(lib().psb_batch_ms_plan(self.h, int(total_frames), _p(v), len(v)), "psb_batch_ms_plan")
+        return {k: int(x) for k, x in zip(self.MS_PLAN, v)}
+
     def decode_host(self, phoneloop, feats, utt_off, want_senscr=False, best=None, pen=None, senscr=None):
         """End to end: host features -> senone scores -> phone-loop Viterbi -> host results."""
         pm = self.model.pm

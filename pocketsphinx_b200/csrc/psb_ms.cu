@@ -11,6 +11,7 @@
 #include "psb_internal.cuh"
 
 #include <stdlib.h>
+#include <string.h>
 
 #include <algorithm>
 
@@ -119,6 +120,11 @@ __device__ __forceinline__ int logadd_wide(const uint32_t *__restrict__ tab, int
 // sums stay scalar).  On sm_90 each float2 operation is two scalar instructions; a pair shares the loads of
 // the mean and variance term.
 constexpr int MS_TCB = 32, MS_TFB = 64, MS_TFT = 4;      // codebooks per CTA, frames per block, frames per thread
+constexpr int MS_PRE = 6, MS_NTHR = MS_TFB / MS_TFT * 32;  // prefetch registers per thread, threads per CTA
+
+// the next block's features travel in registers (MS_PRE per thread) while a block is computed; longer vectors are
+// staged in place
+__host__ __device__ constexpr bool ms_prefetch(int sumlen) { return sumlen * MS_TFB <= MS_PRE * MS_NTHR; }
 
 // FUSE (continuous models: senone s owns codebook s): the lane that holds a codebook's list evaluates the senone on the spot --
 // senone_eval (ms_senone.c:358-407) exactly as ms_senone_kernel does, first clamp, raw int16 score, per-frame minimum -- so
@@ -128,7 +134,7 @@ struct MsSenArgs {
 };
 
 template <int NT, bool FUSE>
-__global__ void __launch_bounds__(MS_TFB / MS_TFT * 32, 2)
+__global__ void __launch_bounds__(MS_NTHR, 2)
 ms_dist_tile_kernel(const float *__restrict__ gT, const float *__restrict__ detT, const float *__restrict__ feats,
                     int2 *__restrict__ out, long long frame0, long long n_frames, int n_mgau, int n_feat, int nd,
                     int sumlen, const int32_t *__restrict__ featlen, const int32_t *__restrict__ featoff, int frames_per_cta,
@@ -151,8 +157,8 @@ ms_dist_tile_kernel(const float *__restrict__ gT, const float *__restrict__ detT
     const long long f_begin = (long long)blockIdx.y * frames_per_cta;
     const long long f_end = f_begin + frames_per_cta < n_frames ? f_begin + frames_per_cta : n_frames;
     // the next block's features travel while this block is computed: each thread keeps its share in registers
-    constexpr int PRE = 6, NTHR = MS_TFB / MS_TFT * 32;
-    const bool prefetch = sumlen * MS_TFB <= PRE * NTHR;            // uniform; longer vectors are staged in place
+    constexpr int PRE = MS_PRE, NTHR = MS_NTHR;
+    const bool prefetch = ms_prefetch(sumlen);                      // uniform; longer vectors are staged in place
     float pre[PRE];
     auto fetch = [&](long long fb) {
 #pragma unroll
@@ -345,7 +351,80 @@ __global__ void fill_i32(int32_t *p, long long n, int32_t v)
 }
 
 
+// How one batch of `total` frames is scored: which kernels, at which list width, in how many chunks.  The launcher runs
+// exactly this plan; psb_batch_ms_plan reports it.
+struct MsPlan {
+    int nt;               // list width: the next power of two >= topn
+    int n_used;           // list entries a senone reads: topn clamped to the Gaussians (ms_mgau.c:137-143)
+    bool all;             // every Gaussian listed in order (compute_dist_all, ms_gauden.c:378-419) rather than sorted
+    bool tile;            // ms_dist_tile_kernel (a codebook tile's Gaussians in shared memory) rather than ms_dist_kernel
+    bool fuse;            // the tile kernel evaluates the senones itself (continuous models: senone s owns codebook s)
+    bool prefetch;        // the tile kernel keeps the next block's features in registers
+    bool transposed;      // one shared codebook: weights stored [feat][cw][sen]
+    size_t tile_smem;     // the tile kernel's dynamic shared memory
+    int tiles_x;          // codebook tiles of MS_TCB
+    int n_sm;
+    long long chunk;      // frames per launch sequence
+    long long n_chunks;
+    size_t dist_bytes;    // list buffer (d_msdist) of one chunk; 0 when the lists never leave the tile kernel
+};
+
+constexpr size_t MS_LIST_BUDGET = (size_t)2 << 30;   // list bytes of one chunk
+constexpr long long MS_MAX_CHUNK = 65535;            // gridDim.y of ms_dist_kernel / ms_senone_kernel / ms_norm_kernel
+
+int ms_plan(const psb_model_t *m, long long total, MsPlan *p)
+{
+    PSB_REQUIRE(m->kind == PSB_KIND_MS, "ms batch plan: model is not ms");
+    PSB_REQUIRE(total >= 0, "ms batch plan: negative frame count");
+    int nt = 1;
+    while (nt < m->topn) nt <<= 1;
+    PSB_REQUIRE(nt <= MAXNT, "ms batch kernels support -topn up to %d (got %d)", MAXNT, m->topn);
+    PSB_REQUIRE(m->topn >= m->n_density || nt == m->topn, "ms batch kernels need a power-of-two -topn (got %d)", m->topn);
+    p->nt = nt;
+    p->n_used = std::min(m->topn, m->n_density);
+    p->all = nt >= m->n_density;
+    p->tile_smem = ((size_t)m->n_density * m->sumlen * 2 + (size_t)m->n_feat * m->n_density) * MS_TCB * sizeof(float)
+                   + (size_t)m->sumlen * MS_TFB * sizeof(float);
+    p->tile = p->tile_smem <= 100 * 1024;               // else the untiled kernel (parameters streamed from L2)
+    // continuous models: mixtures evaluated by the lane that holds the list (the kernel writes raw scores and minima)
+    p->fuse = p->tile && m->sen_is_cb && m->n_mgau > 1;
+    p->prefetch = ms_prefetch(m->sumlen);
+    p->transposed = m->n_mgau == 1;
+    p->tiles_x = (m->n_mgau + MS_TCB - 1) / MS_TCB;
+    p->n_sm = psb_sm_count(m->device);
+    // a fused chunk writes no lists, so only the grid limit bounds it
+    const size_t per_frame = (size_t)m->n_mgau * m->n_feat * nt * sizeof(int2);
+    long long chunk = p->fuse ? total
+                              : std::max<long long>(FT, std::min<long long>(total, (long long)(MS_LIST_BUDGET / per_frame) / FT * FT));
+    p->chunk = std::min<long long>(chunk, MS_MAX_CHUNK);
+    p->n_chunks = p->chunk ? (total + p->chunk - 1) / p->chunk : 0;
+    p->dist_bytes = p->fuse ? 0 : (size_t)p->chunk * per_frame;
+    return PSB_OK;
+}
+
+// frames per CTA of the tile kernel for a chunk of n frames: enough CTAs for ~4 waves of two resident CTAs per SM,
+// whole MS_TFB-frame blocks
+long long ms_frames_per_cta(const MsPlan &p, long long n)
+{
+    const long long waves = p.n_sm * 2LL * 4;
+    const long long fpc = (n * p.tiles_x + waves - 1) / waves;
+    return std::max<long long>(MS_TFB, (fpc + MS_TFB - 1) / MS_TFB * MS_TFB);
+}
+
 }  // namespace
+
+extern "C" int psb_batch_ms_plan(psb_batch_t *b, int64_t total_frames, int64_t *out, int32_t n)
+{
+    PSB_REQUIRE(b && (out || n == 0) && n >= 0, "psb_batch_ms_plan: bad argument");
+    MsPlan p;
+    const int rc = ms_plan(b->m, total_frames, &p);
+    if (rc) return rc;
+    const int64_t v[PSB_MS_PLAN_N] = {p.tile, p.fuse, p.prefetch, p.nt, p.n_used, p.all,
+                                      p.chunk ? ms_frames_per_cta(p, p.chunk) : 0, p.tiles_x, p.chunk, p.n_chunks,
+                                      (int64_t)p.dist_bytes, p.n_sm, p.transposed, (int64_t)p.tile_smem};
+    memcpy(out, v, sizeof(int64_t) * (size_t)std::min<int32_t>(n, PSB_MS_PLAN_N));
+    return PSB_OK;
+}
 
 int psb_launch_ms_batch(psb_batch_t *b, const float *d_feats, const int32_t *utt_off, int32_t n_utt, int16_t *d_senscr)
 {
@@ -354,36 +433,23 @@ int psb_launch_ms_batch(psb_batch_t *b, const float *d_feats, const int32_t *utt
     const long long total = utt_off[n_utt];
     b->last_frames = total;
     if (total == 0) return PSB_OK;
-    int nt = 1;
-    while (nt < m->topn) nt <<= 1;
-    PSB_REQUIRE(nt <= MAXNT, "ms batch kernels support -topn up to %d (got %d)", MAXNT, m->topn);
-    const int n_used = std::min(m->topn, m->n_density);     // ms_mgau_init clamps topn (ms_mgau.c:137-143)
-    PSB_REQUIRE(m->topn >= m->n_density || nt == m->topn, "ms batch kernels need a power-of-two -topn (got %d)", m->topn);
-    const size_t per_frame = (size_t)m->n_mgau * m->n_feat * nt * sizeof(int2);
-    const size_t budget = (size_t)2 << 30;
-    long long chunk = std::max<long long>(FT, std::min<long long>(total, (long long)(budget / per_frame) / FT * FT));
-    chunk = std::min<long long>(chunk, 65535);              // gridDim.y
-    int rc = b->d_msdist.reserve((size_t)chunk * per_frame);
-    if (!rc) rc = b->d_msbest.reserve(65536);
+    MsPlan p;
+    int rc = ms_plan(m, total, &p);
+    if (!rc && p.dist_bytes) rc = b->d_msdist.reserve(p.dist_bytes);
+    if (!rc) rc = b->d_msbest.reserve(MS_MAX_CHUNK + 1);
     if (rc) return rc;
+    const int nt = p.nt, n_used = p.n_used;
+    const bool tile = p.tile, fuse = p.fuse;
+    const size_t tile_smem = p.tile_smem;
     PSB_CUDA(cudaEventRecord(b->ev[0], b->stream));
     PSB_CUDA(cudaEventRecord(b->ev[1], b->stream));
-    for (long long f0 = 0; f0 < total; f0 += chunk) {
-        const long long n = std::min(chunk, total - f0);
+    for (long long f0 = 0; f0 < total; f0 += p.chunk) {
+        const long long n = std::min(p.chunk, total - f0);
         dim3 g1((m->n_mgau + 127) / 128, (unsigned)((n + FT - 1) / FT));
         size_t smem = (size_t)FT * m->sumlen * sizeof(float);
-        int2 *dist = reinterpret_cast<int2 *>(b->d_msdist.get());
-        const size_t tile_smem = ((size_t)m->n_density * m->sumlen * 2 + (size_t)m->n_feat * m->n_density) * MS_TCB * sizeof(float)
-                                 + (size_t)m->sumlen * MS_TFB * sizeof(float);
-        const bool tile = tile_smem <= 100 * 1024;           // else the untiled kernel (parameters streamed from L2)
-        // frames per CTA: enough CTAs for ~4 waves of two resident CTAs per SM, whole 32-frame blocks
-        const int tiles_x = (m->n_mgau + MS_TCB - 1) / MS_TCB;
-        const long long waves = psb_sm_count(m->device) * 2LL * 4;
-        long long fpc = (n * tiles_x + waves - 1) / waves;
-        fpc = std::max<long long>(MS_TFB, (fpc + MS_TFB - 1) / MS_TFB * MS_TFB);
-        const dim3 gt((unsigned)tiles_x, (unsigned)((n + fpc - 1) / fpc));
-        // continuous models: mixtures evaluated by the lane that holds the list (the kernel writes raw scores and minima)
-        const bool fuse = tile && m->sen_is_cb && m->n_mgau > 1;
+        int2 *dist = fuse ? nullptr : reinterpret_cast<int2 *>(b->d_msdist.get());
+        const long long fpc = ms_frames_per_cta(p, n);
+        const dim3 gt((unsigned)p.tiles_x, (unsigned)((n + fpc - 1) / fpc));
         MsSenArgs sa = {m->d_mixw, m->d_logadd_ms, m->logadd_ms_size, m->logadd_ms_zero, d_senscr, b->d_msbest, n_used, m->aw};
         if (fuse) {
             fill_i32<<<(unsigned)((n + 255) / 256), 256, 0, b->stream>>>(b->d_msbest, n, 0x7fffffff);
@@ -392,7 +458,7 @@ int psb_launch_ms_batch(psb_batch_t *b, const float *d_feats, const int32_t *utt
 #define PSB_MS_TILE(NT, FUSEV) do {                                                                                       \
             auto kern = ms_dist_tile_kernel<NT, FUSEV>;                                                                   \
             PSB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tile_smem));            \
-            kern<<<gt, MS_TFB / MS_TFT * 32, tile_smem, b->stream>>>(m->d_msT, m->d_msdetT, d_feats, dist, f0, n,         \
+            kern<<<gt, MS_NTHR, tile_smem, b->stream>>>(m->d_msT, m->d_msdetT, d_feats, dist, f0, n,                       \
                 m->n_mgau, m->n_feat, m->n_density, m->sumlen, m->d_featlen, m->d_featoff, (int)fpc, sa); } while (0)
 #define LAUNCH(NT) do { if (tile) {                                                                                       \
             if (fuse) PSB_MS_TILE(NT, true);                                                                               \
@@ -409,12 +475,12 @@ int psb_launch_ms_batch(psb_batch_t *b, const float *d_feats, const int32_t *utt
 #undef PSB_MS_TILE
         PSB_LAUNCH_CHECK();
         dim3 g2((m->n_sen + 255) / 256, (unsigned)n);
-        if (!(tile && fuse)) {
+        if (!fuse) {
             fill_i32<<<(unsigned)((n + 255) / 256), 256, 0, b->stream>>>(b->d_msbest, n, 0x7fffffff);
             PSB_LAUNCH_CHECK();
             ms_senone_kernel<<<g2, 256, 0, b->stream>>>(dist, m->d_mixw, m->d_sen2cb32, m->d_logadd_ms, m->logadd_ms_size,
                                                         m->logadd_ms_zero, d_senscr, b->d_msbest, f0, m->n_sen, m->n_mgau,
-                                                        m->n_feat, m->n_density, nt, n_used, m->aw, m->n_mgau == 1, nullptr, m->n_sen);
+                                                        m->n_feat, m->n_density, nt, n_used, m->aw, p.transposed, nullptr, m->n_sen);
             PSB_LAUNCH_CHECK();
         }
         ms_norm_kernel<<<g2, 256, 0, b->stream>>>(d_senscr, b->d_msbest, f0, m->n_sen, nullptr, m->n_sen);
