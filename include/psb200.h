@@ -161,6 +161,16 @@ int psb_batch_tc_counters(psb_batch_t *b, int64_t *out, int32_t n);
  * batch kernels refuse is refused here too. */
 #define PSB_MS_PLAN_N 14
 int psb_batch_ms_plan(psb_batch_t *b, int64_t total_frames, int64_t *out, int32_t n);
+/* debugging/tests: how a batch of total_frames frames on a ptm or semi-continuous model is scored -- the plan the batch
+ * launcher runs.  out[0..n-1] receives the first n of, in order: the top-N paths its streams take, as bits
+ * (1 tensor-core filter, 2 PTM deferred-insertion scan, 4 PTM scalar scan, 8 semi-continuous split distances and scan,
+ * 16 semi-continuous paired scan, 32 semi-continuous scalar scan, 64 fixed-point scan); the senone kernel (0
+ * ptm_senone4, 1 ptm_senone 8-bit, 2 ptm_senone 4-bit, 3 semi_senone4, 4 semi_senone 8-bit, 5 semi_senone 4-bit); its
+ * threads per CTA; the senones ptm_senone4 evaluates one by one (quads that straddle a codebook boundary, and the
+ * tail); its dynamic shared memory in bytes.  What the batch kernels refuse (a -topn other than 4, more than 512
+ * codebook-stream pairs, senones beyond shared memory) is refused here too. */
+#define PSB_TM_PLAN_N 5
+int psb_batch_tm_plan(psb_batch_t *b, int64_t total_frames, int64_t *out, int32_t n);
 /* debugging/parity: copy the per-frame top-N records of the last call to the host:
  * rec int32 [total_frames][n_mgau*n_feat][4] = {top>>10, cw[4] bytes, e[4] bytes, 0} */
 int psb_batch_get_topn(psb_batch_t *b, int32_t *rec, int64_t n_frames);

@@ -108,6 +108,7 @@ SYMBOLS = [
     ("psb_batch_tc_check", C.c_int, [_VP, C.POINTER(C.c_float), C.POINTER(C.c_int32), _VP]),
     ("psb_batch_tc_counters", C.c_int, [_VP, _VP, _I32]),
     ("psb_batch_ms_plan", C.c_int, [_VP, _I64, _VP, _I32]),
+    ("psb_batch_tm_plan", C.c_int, [_VP, _I64, _VP, _I32]),
     ("psb_hmmset_use_batch_stream", C.c_int, [_VP, _VP]),
     ("psb_hmmset_snapshot", C.c_int, [_VP]),
     ("psb_hmmset_restore", C.c_int, [_VP]),

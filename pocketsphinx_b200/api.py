@@ -223,6 +223,18 @@ class Batch:
         check(lib().psb_batch_ms_plan(self.h, int(total_frames), _p(v), len(v)), "psb_batch_ms_plan")
         return {k: int(x) for k, x in zip(self.MS_PLAN, v)}
 
+    TM_TOPN = ("tc_filter", "ptm_scan", "ptm_scalar", "semi_split", "semi_pairs", "semi_scalar", "fixed")
+    TM_SENONE = ("ptm_senone4", "ptm_senone_8b", "ptm_senone_4b", "semi_senone4", "semi_senone_8b", "semi_senone_4b")
+
+    def tm_plan(self, total_frames):
+        """How a batch of total_frames frames on a ptm or semi-continuous model is scored (psb_batch_tm_plan): "topn",
+        the top-N paths of its streams joined by "+"; "senone", the senone kernel; "threads", "n_bsen" and "smem" of
+        the senone launch."""
+        v = np.zeros(5, np.int64)
+        check(lib().psb_batch_tm_plan(self.h, int(total_frames), _p(v), len(v)), "psb_batch_tm_plan")
+        return dict(topn="+".join(n for i, n in enumerate(self.TM_TOPN) if int(v[0]) >> i & 1),
+                    senone=self.TM_SENONE[int(v[1])], threads=int(v[2]), n_bsen=int(v[3]), smem=int(v[4]))
+
     def decode_host(self, phoneloop, feats, utt_off, want_senscr=False, best=None, pen=None, senscr=None):
         """End to end: host features -> senone scores -> phone-loop Viterbi -> host results."""
         pm = self.model.pm

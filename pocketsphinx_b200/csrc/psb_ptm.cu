@@ -24,6 +24,8 @@
 #include "psb_gau.cuh"
 #include "psb_internal.cuh"
 
+#include <string.h>
+
 #include <algorithm>
 #include <numeric>
 
@@ -1243,18 +1245,114 @@ semi_senone4_kernel(const int4 *__restrict__ topn, const uint8_t *__restrict__ m
     }
 }
 
+// Top-N paths (bits of TmPlan::topn_paths) and senone kernels of a tied-mixture batch, in psb_batch_tm_plan's numbering.
+enum TmTopn { TOPN_TC_FILTER, TOPN_PTM_SCAN, TOPN_PTM_SCALAR, TOPN_SEMI_SPLIT, TOPN_SEMI_PAIRS, TOPN_SEMI_SCALAR, TOPN_FIXED };
+enum TmSenone { SEN_PTM4, SEN_PTM_8B, SEN_PTM_4B, SEN_SEMI4, SEN_SEMI_8B, SEN_SEMI_4B };
+
+// Stream lengths with top-N kernel instantiations (the CASE lists of psb_launch_ptm_batch).
+bool topn_fl_instantiated(int fl)
+{
+    for (int v : {13, 12, 24, 3, 39, 1, 2, 4, 8, 16, 26, 32})
+        if (fl == v) return true;
+    return false;
+}
+
+constexpr size_t TM_SMEM_MAX = 227 * 1024;   // dynamic shared memory one CTA may opt in to on sm_90
+
+// How a tied-mixture batch is scored: the top-N kernel of each stream length and the senone kernel with its launch
+// shape.  The launcher runs exactly this plan; psb_batch_tm_plan reports it.
+struct TmPlan {
+    unsigned topn_paths;  // bit p set: some stream takes top-N path p (TmTopn)
+    bool semi_split;      // semi-continuous distances out of the time loop (semi_dist_kernel + semi_scan_kernel)
+    int senone;           // TmSenone
+    int threads;          // senone kernel block size
+    size_t smem;          // senone kernel dynamic shared memory
+};
+
+int tm_plan(const psb_model_t *m, TmPlan *p)
+{
+    PSB_REQUIRE(m->kind == PSB_KIND_PTM || m->kind == PSB_KIND_SEMI, "psb_launch_ptm_batch: model is neither PTM nor semi-continuous");
+    const bool semi = m->kind == PSB_KIND_SEMI;
+    PSB_REQUIRE(m->topn == TOPN, "tied-mixture batch kernels are built for -topn 4 (got %d)", m->topn);
+    PSB_REQUIRE(m->n_density % 32 == 0 && m->n_density <= 32 * MAX_NDW,
+                "PTM batch kernels need n_density in {32..256, multiple of 32} (got %d)", m->n_density);
+    const int K = m->K;
+    const bool use_tc = !semi && psb_tc_usable(m);
+    p->semi_split = semi && !m->fixed_point && m->n_mgau == 1 && m->n_density <= 256 &&
+                    (m->n_density == 64 || m->n_density == 128 || m->n_density == 256);
+    p->topn_paths = 0;
+    for (int f = 0; f < m->n_feat; ++f) {
+        const int fl = m->featlen[f];
+        if (use_tc) { p->topn_paths |= 1u << TOPN_TC_FILTER; continue; }
+        if (!topn_fl_instantiated(fl)) {
+            psb_set_error("no %s instantiation for stream length %d", p->semi_split ? "semi_dist_kernel" : "ptm_topn_kernel", fl);
+            return PSB_ERR_ARG;
+        }
+        int path;
+        if (p->semi_split) path = TOPN_SEMI_SPLIT;
+        else if (fl <= 16 && !m->fixed_point) path = semi ? TOPN_SEMI_PAIRS : TOPN_PTM_SCAN;
+        else if (m->fixed_point) path = TOPN_FIXED;
+        else path = semi ? TOPN_SEMI_SCALAR : TOPN_PTM_SCALAR;
+        p->topn_paths |= 1u << path;
+    }
+    // the 16x2 kernels bias every value by SEN_BIAS; fast_logmath_add's results stay above -(TOPN - 1) * tab[0]
+    const bool bias_ok = (TOPN - 1) * m->logadd8_max < SEN_BIAS;
+    if (semi) {
+        PSB_REQUIRE(K <= 512, "semi_senone_kernel handles at most 512 streams (got %d)", K);
+        if (!m->mixw_4bit && bias_ok && m->mixw_stride % 4 == 0 && m->n_feat <= PSB_MAX_FEAT) {
+            p->senone = SEN_SEMI4; p->threads = 512; p->smem = 0;
+        }
+        else {
+            p->senone = m->mixw_4bit ? SEN_SEMI_4B : SEN_SEMI_8B;
+            p->threads = 256;
+            p->smem = (size_t)K * 32 + PSB_LOGADD8_N + 16;
+        }
+        return PSB_OK;
+    }
+    PSB_REQUIRE(K <= 512, "ptm_senone_kernel handles at most 512 (codebook, stream) pairs (got %d)", K);
+    PSB_REQUIRE((size_t)m->n_feat * m->n_density * m->mixw_stride < (1ull << 32), "mixture-weight table too large for 32-bit offsets");
+    const size_t smem = (size_t)K * 32 + 8 * 4 + 32 * 4 + PSB_LOGADD8_N + 16 + (size_t)m->n_sen * 2;
+    if (m->mixw_4bit || !bias_ok) {
+        p->senone = m->mixw_4bit ? SEN_PTM_4B : SEN_PTM_8B;
+        p->threads = 512;
+        p->smem = smem;
+    }
+    else {
+        // four senones per thread; threads sized so that the quads divide evenly over the block,
+        // at least 256 threads (log-add table staging) and one thread per (codebook, stream) pair
+        const int n_quads = (m->n_sen + 3) / 4;
+        const int iters = (n_quads + 511) / 512;
+        p->senone = SEN_PTM4;
+        p->threads = std::min(512, std::max(std::max(256, roundup(K, 32)), roundup((n_quads + iters - 1) / iters, 32)));
+        p->smem = smem + 8 + (size_t)K * 16;
+    }
+    PSB_REQUIRE(p->smem <= TM_SMEM_MAX, "%d senones do not fit the PTM senone kernel's shared memory (%zu bytes, at most %zu)",
+                m->n_sen, p->smem, TM_SMEM_MAX);
+    return PSB_OK;
+}
+
 }  // namespace
+
+extern "C" int psb_batch_tm_plan(psb_batch_t *b, int64_t total_frames, int64_t *out, int32_t n)
+{
+    PSB_REQUIRE(b && (out || n == 0) && n >= 0 && total_frames >= 0, "psb_batch_tm_plan: bad argument");
+    TmPlan p;
+    const int rc = tm_plan(b->m, &p);
+    if (rc) return rc;
+    const int64_t v[PSB_TM_PLAN_N] = {p.topn_paths, p.senone, p.threads, b->m->n_bsen, (int64_t)p.smem};
+    memcpy(out, v, sizeof(int64_t) * (size_t)std::min<int32_t>(n, PSB_TM_PLAN_N));
+    return PSB_OK;
+}
 
 // Host side of one batched scoring pass.  d_feats: [total][D] on the device.
 int psb_launch_ptm_batch(psb_batch_t *b, const float *d_feats, const int32_t *utt_off, int32_t n_utt,
                          int16_t *d_senscr)
 {
     psb_model_t *m = b->m;
-    PSB_REQUIRE(m->kind == PSB_KIND_PTM || m->kind == PSB_KIND_SEMI, "psb_launch_ptm_batch: model is neither PTM nor semi-continuous");
+    TmPlan plan;
+    int rc = tm_plan(m, &plan);
+    if (rc) return rc;
     const bool semi = m->kind == PSB_KIND_SEMI;
-    PSB_REQUIRE(m->topn == TOPN, "tied-mixture batch kernels are built for -topn 4 (got %d)", m->topn);
-    PSB_REQUIRE(m->n_density % 32 == 0 && m->n_density <= 32 * MAX_NDW,
-                "PTM batch kernels need n_density in {32..256, multiple of 32} (got %d)", m->n_density);
     const long long total = utt_off[n_utt];
     PSB_REQUIRE(n_utt <= b->max_utts && total <= b->max_frames, "batch too large for this psb_batch_t");
     b->last_frames = total;
@@ -1273,7 +1371,7 @@ int psb_launch_ptm_batch(psb_batch_t *b, const float *d_feats, const int32_t *ut
     size_t n32 = (size_t)n_groups * 64 + n_groups + K + PSB_MAX_FEAT;
     n32 = (n32 + 1) & ~(size_t)1;
     size_t need = n32 + 2 * (size_t)(2 * n_groups + 1);
-    int rc = b->d_tab.reserve(need, need);
+    rc = b->d_tab.reserve(need, need);
     if (!rc) rc = b->h_tab.reserve(need, need);
     if (rc) return rc;
     int32_t *lane_len = b->h_tab, *lane_off = lane_len + n_groups * 32, *grp_maxT = lane_off + n_groups * 32;
@@ -1322,7 +1420,7 @@ int psb_launch_ptm_batch(psb_batch_t *b, const float *d_feats, const int32_t *ut
     tabs.grp_base = reinterpret_cast<const long long *>(b->d_tab + n32);
     const long long *d_warp_base = tabs.grp_base + n_groups;
 
-    const bool use_tc = !semi && psb_tc_usable(m);
+    const bool use_tc = plan.topn_paths == 1u << TOPN_TC_FILTER;
     PSB_CUDA(cudaEventRecord(b->ev[0], b->stream));
     if (!use_tc) {
         int warps = 8;
@@ -1336,8 +1434,7 @@ int psb_launch_ptm_batch(psb_batch_t *b, const float *d_feats, const int32_t *ut
     }
     PSB_CUDA(cudaEventRecord(b->ev[1], b->stream));
     // semi-continuous: distances out of the time loop, one warp per (utterance, stream)
-    const bool semi_split = semi && !m->fixed_point && m->n_mgau == 1 && m->n_density <= 256 &&
-                            (m->n_density == 64 || m->n_density == 128 || m->n_density == 256);
+    const bool semi_split = plan.semi_split;
     if (use_tc) {
         // no recurrence over time: tensor-core filter, exact rescoring of the survivors, tie fix-up (psb_ptm_tc.cu)
         rc = psb_launch_ptm_tc(b, d_feats, utt_off, n_utt, d_klist, d_featoff);
@@ -1393,49 +1490,30 @@ int psb_launch_ptm_batch(psb_batch_t *b, const float *d_feats, const int32_t *ut
     }
     PSB_CUDA(cudaEventRecord(b->ev[2], b->stream));
     if (semi) {
-        size_t smem = (size_t)K * 32 + PSB_LOGADD8_N + 16;
-        PSB_REQUIRE(K <= 512, "semi_senone_kernel handles at most 512 streams (got %d)", K);
-        const int threads = 256;
-        dim3 grid((m->n_sen + threads - 1) / threads, (unsigned)total);
         PSB_REQUIRE(total <= 65535LL * 32768, "too many frames for one launch");
-        if (!m->mixw_4bit && (TOPN - 1) * m->logadd8_max < SEN_BIAS && m->mixw_stride % 4 == 0 &&
-            m->n_feat <= PSB_MAX_FEAT)
-            semi_senone4_kernel<<<(unsigned)total, 512, 0, b->stream>>>(b->d_topn, m->d_mixw, m->d_logadd8, d_senscr, m->n_sen,
-                                                                      m->n_feat, m->n_density, m->mixw_stride);
-        else if (m->mixw_4bit)
-            semi_senone_kernel<true><<<dim3((unsigned)total, (m->n_sen + threads - 1) / threads), threads, smem, b->stream>>>(
+        const dim3 grid((unsigned)total, (m->n_sen + plan.threads - 1) / plan.threads);
+        if (plan.senone == SEN_SEMI4)
+            semi_senone4_kernel<<<(unsigned)total, plan.threads, 0, b->stream>>>(b->d_topn, m->d_mixw, m->d_logadd8, d_senscr,
+                                                                               m->n_sen, m->n_feat, m->n_density, m->mixw_stride);
+        else if (plan.senone == SEN_SEMI_4B)
+            semi_senone_kernel<true><<<grid, plan.threads, plan.smem, b->stream>>>(
                 b->d_topn, m->d_mixw, m->d_mixw_cb, m->d_logadd8, d_senscr, m->n_sen, m->n_feat, m->n_density, m->mixw_stride);
         else
-            semi_senone_kernel<false><<<dim3((unsigned)total, (m->n_sen + threads - 1) / threads), threads, smem, b->stream>>>(
+            semi_senone_kernel<false><<<grid, plan.threads, plan.smem, b->stream>>>(
                 b->d_topn, m->d_mixw, m->d_mixw_cb, m->d_logadd8, d_senscr, m->n_sen, m->n_feat, m->n_density, m->mixw_stride);
-        (void)grid;
         PSB_LAUNCH_CHECK();
     }
     else {
-        size_t smem = (size_t)K * 32 + 8 * 4 + 32 * 4 + PSB_LOGADD8_N + 16 + (size_t)m->n_sen * 2;
-        PSB_REQUIRE(K <= 512, "ptm_senone_kernel handles at most 512 (codebook, stream) pairs (got %d)", K);
-        PSB_REQUIRE((size_t)m->n_feat * m->n_density * m->mixw_stride < (1ull << 32), "mixture-weight table too large for 32-bit offsets");
-        if (m->mixw_4bit) {
-            PSB_CUDA(cudaFuncSetAttribute(ptm_senone_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            ptm_senone_kernel<true><<<(unsigned)total, 512, smem, b->stream>>>(
-                b->d_topn, m->d_mixw, m->d_mixw_cb, m->d_sen2cb, m->d_logadd8, d_senscr, m->n_sen, m->n_feat,
-                m->n_density, K, m->mixw_stride);
-        }
-        else if ((TOPN - 1) * m->logadd8_max >= SEN_BIAS) {
-            PSB_CUDA(cudaFuncSetAttribute(ptm_senone_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            ptm_senone_kernel<false><<<(unsigned)total, 512, smem, b->stream>>>(
+        if (plan.senone == SEN_PTM_4B || plan.senone == SEN_PTM_8B) {
+            auto kern = plan.senone == SEN_PTM_4B ? ptm_senone_kernel<true> : ptm_senone_kernel<false>;
+            PSB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem));
+            kern<<<(unsigned)total, plan.threads, plan.smem, b->stream>>>(
                 b->d_topn, m->d_mixw, m->d_mixw_cb, m->d_sen2cb, m->d_logadd8, d_senscr, m->n_sen, m->n_feat,
                 m->n_density, K, m->mixw_stride);
         }
         else {
-            // four senones per thread; threads sized so that the quads divide evenly over the block
-            const int n_quads = (m->n_sen + 3) / 4;
-            const int iters = (n_quads + 511) / 512;
-            // at least 256 threads (log-add table staging) and one thread per (codebook, stream) pair
-            const int threads = std::min(512, std::max(std::max(256, roundup(K, 32)), roundup((n_quads + iters - 1) / iters, 32)));
-            const size_t smem4 = smem + 8 + (size_t)K * 16;
-            PSB_CUDA(cudaFuncSetAttribute(ptm_senone4_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem4));
-            ptm_senone4_kernel<<<(unsigned)total, threads, smem4, b->stream>>>(
+            PSB_CUDA(cudaFuncSetAttribute(ptm_senone4_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem));
+            ptm_senone4_kernel<<<(unsigned)total, plan.threads, plan.smem, b->stream>>>(
                 b->d_topn, m->d_mixw, m->d_sen2cb, m->d_quadcb, m->d_bsen, m->n_bsen, m->d_logadd8, d_senscr, m->n_sen,
                 m->n_feat, m->n_density, K, m->mixw_stride);
         }

@@ -163,50 +163,98 @@ def make_logadd8(base=1.0001, shift=10):
     return table
 
 
+SEN2CB_LAYOUTS = ("cuts", "small", "single", "identity")
+
+
+def _ptm_sen2cb(rng, layout, n_sen, n_mgau, n_ci, n_emit_state):
+    """The senone -> codebook map of synth_ptm (see there)."""
+    if layout == "cuts":
+        sen2cb = np.empty(n_sen, np.int32)
+        sen2cb[:n_ci] = np.repeat(np.arange(n_mgau), n_emit_state)
+        cuts = np.sort(rng.choice(np.arange(1, n_sen - n_ci), n_mgau - 1, replace=False))
+        sizes = np.diff(np.concatenate([[0], cuts, [n_sen - n_ci]]))
+        sen2cb[n_ci:] = np.repeat(np.arange(n_mgau), sizes)
+        return sen2cb
+    if layout == "small":
+        sizes = []
+        while sum(sizes) < n_sen:
+            sizes.append(int(rng.integers(1, 4)))
+        sizes[-1] -= sum(sizes) - n_sen
+        return np.repeat(np.arange(len(sizes)) % n_mgau, sizes).astype(np.int32)
+    if layout == "single":
+        return np.zeros(n_sen, np.int32)
+    assert layout == "identity" and n_mgau == n_sen, "sen2cb='identity' needs n_mgau == n_sen"
+    return np.arange(n_sen, dtype=np.int32)
+
+
+def _pack_4bit(rng, q, n_sen):
+    """Cluster 8-bit mixture weights [f][cw][sen] to 16 values and pack them as a clustered sendump stores them:
+    row (n_sen + 1) // 2 bytes, senone 2i in the low nibble of byte i, 2i + 1 in the high one, an odd last senone
+    alone in the low nibble of the last byte.  Returns (packed, mixw_cb)."""
+    mixw_cb = np.sort(rng.choice(np.arange(0, 160), 16, replace=False)).astype(np.uint8)
+    idx = np.abs(q[..., None].astype(np.int32) - mixw_cb.astype(np.int32)).argmin(-1).astype(np.uint8)
+    row = (n_sen + 1) // 2
+    packed = np.zeros(q.shape[:-1] + (row,), np.uint8)
+    packed[..., :n_sen // 2] |= idx[..., 0:n_sen - (n_sen & 1):2]
+    packed[..., :n_sen // 2] |= idx[..., 1:n_sen:2] << 4
+    if n_sen & 1:
+        packed[..., row - 1] |= idx[..., n_sen - 1]
+    return packed, mixw_cb
+
+
 def synth_ptm(seed=0, n_mgau=42, n_feat=3, n_density=256, featlen=13, n_sen=5138, topn=4,
-              n_tmat=None, n_emit_state=3, skip_arcs=False, return_raw=False):
+              n_tmat=None, n_emit_state=3, skip_arcs=False, four_bit=False, sen2cb="cuts", featlens=None,
+              return_raw=False):
     """Synthetic PTM model of the BASELINE.json shape (42 cb x 3 streams x 256 Gaussians x 13
     dims, 5138 senones).  Generated as RAW parameters (means, variances, transition
     probabilities, quantised mixture weights) and passed through mirrors of the reference's
     loaders (s3io.precompute_gaussians / quantize_tmat), so that the same model can also be
     written as Sphinx-3 files (s3io.write_model_dir) and loaded by the unmodified reference.
-    CI senones first (n_emit_state per codebook), the rest in contiguous per-codebook runs."""
+    featlens: stream lengths (n_feat streams of featlen dimensions by default).
+    four_bit: clustered 4-bit mixture weights (mixw_cb), packed as _pack_4bit describes.
+    sen2cb: "cuts" (CI senones first, n_emit_state per codebook, the rest in contiguous per-codebook runs cut at
+    random), "small" (runs of 1-3 senones, codebooks in turn), "single" (every senone on codebook 0) or "identity"
+    (n_mgau == n_sen, senone s on codebook s).  Only "cuts" is a map the reference derives from an mdef."""
     from . import s3io
     rng = np.random.default_rng(seed)
-    fl = np.full(n_feat, featlen, np.int32)
+    fl = np.array(featlens if featlens is not None else [featlen] * n_feat, np.int32)
+    n_feat = len(fl)
     scale = np.array([3.0, 1.0, 0.5] + [1.0] * max(0, n_feat - 3), np.float32)[:n_feat]
-    mean = (rng.normal(0.0, 1.0, (n_mgau, n_feat, n_density, featlen)) * scale[None, :, None, None]).astype(np.float32)
-    var_raw = (rng.uniform(0.05, 2.0, (n_mgau, n_feat, n_density, featlen))
-               * (scale[None, :, None, None].astype(np.float64) ** 2)).astype(np.float32)
+    if featlens is None:
+        mean = (rng.normal(0.0, 1.0, (n_mgau, n_feat, n_density, featlen)) * scale[None, :, None, None]).astype(np.float32)
+        var_raw = (rng.uniform(0.05, 2.0, (n_mgau, n_feat, n_density, featlen))
+                   * (scale[None, :, None, None].astype(np.float64) ** 2)).astype(np.float32)
+    else:
+        mean, var_raw = _synth_gaussians(rng, n_mgau, fl, n_density, scale)
     var, det = s3io.precompute_gaussians(var_raw, n_mgau, n_feat, n_density, fl)
     n_ci = n_mgau * n_emit_state
-    assert n_sen > n_ci
-    sen2cb = np.empty(n_sen, np.int32)
-    sen2cb[:n_ci] = np.repeat(np.arange(n_mgau), n_emit_state)
-    cuts = np.sort(rng.choice(np.arange(1, n_sen - n_ci), n_mgau - 1, replace=False))
-    sizes = np.diff(np.concatenate([[0], cuts, [n_sen - n_ci]]))
-    sen2cb[n_ci:] = np.repeat(np.arange(n_mgau), sizes)
+    assert sen2cb != "cuts" or n_sen > n_ci
+    s2c = _ptm_sen2cb(rng, sen2cb, n_sen, n_mgau, n_ci, n_emit_state)
     # mixture weights as the sendump stores them: 0..159, most mass on few codewords
     lb = np.log(1.0001)
     w = rng.gamma(0.3, 1.0, (n_sen, n_feat, n_density)) + 1e-7
     w /= w.sum(-1, keepdims=True)
     q = (np.trunc(-np.log(w) / lb).astype(np.int64)) >> 10
     mixw = np.minimum(q, 159).astype(np.uint8).transpose(1, 2, 0).copy()    # [f][cw][sen]
+    mixw_cb = np.zeros(0, np.uint8)
+    if four_bit:
+        mixw, mixw_cb = _pack_4bit(rng, mixw, n_sen)
     n_tmat = n_tmat or n_mgau
     tp_float = synth_tmat_float(rng, n_tmat, n_emit_state, skip_arcs)
     tp = s3io.quantize_tmat(tp_float)
     n_sseq = 4096
     sseq = np.empty((n_sseq, n_emit_state), np.uint16)
-    sseq[:n_mgau] = np.arange(n_ci).reshape(n_mgau, n_emit_state)
+    sseq[:n_mgau] = np.arange(n_ci).reshape(n_mgau, n_emit_state) % n_sen
     sseq[n_mgau:] = rng.integers(0, n_sen, (n_sseq - n_mgau, n_emit_state))
     pm = PackedModel(kind="ptm", n_sen=n_sen, n_mgau=n_mgau, n_feat=n_feat, n_density=n_density,
-                     topn=topn, featlen=fl, mean=mean, var=var, det=det, mixw=mixw, sen2cb=sen2cb,
+                     topn=topn, featlen=fl, mean=mean, var=var, det=det, mixw=mixw, mixw_cb=mixw_cb, sen2cb=s2c,
                      logadd8=make_logadd8(), n_emit_state=n_emit_state, tp=tp, sseq=sseq,
                      phone_ssid=np.arange(n_mgau, dtype=np.int32),
                      phone_tmat=np.arange(n_mgau, dtype=np.int32) % n_tmat,
-                     n_ciphone=n_mgau, n_ci_sen=n_ci)
+                     n_ciphone=n_mgau, n_ci_sen=min(n_ci, n_sen))
     if return_raw:
-        return pm, dict(mean=mean, var_raw=var_raw, tp_float=tp_float, mixw_q=mixw)
+        return pm, dict(mean=mean, var_raw=var_raw, tp_float=tp_float, mixw_q=mixw,
+                        mixw_cb=mixw_cb if four_bit else None)
     return pm
 
 
@@ -296,15 +344,7 @@ def synth_semi(seed=0, featlens=(12, 24, 3, 12), n_density=256, n_sen=670, topn=
     q = q.transpose(1, 2, 0).copy()                        # [f][cw][sen]
     mixw_cb = np.zeros(0, np.uint8)
     if four_bit:
-        mixw_cb = np.sort(rng.choice(np.arange(0, 160), 16, replace=False)).astype(np.uint8)
-        idx = np.abs(q[..., None].astype(np.int32) - mixw_cb[None, None, None, :].astype(np.int32)).argmin(-1).astype(np.uint8)
-        row = (n_sen + 1) // 2
-        packed = np.zeros((n_feat, n_density, row), np.uint8)
-        packed[..., :n_sen // 2] |= idx[..., 0:n_sen - (n_sen & 1):2]
-        packed[..., :n_sen // 2] |= idx[..., 1:n_sen:2] << 4
-        if n_sen & 1:
-            packed[..., row - 1] |= idx[..., n_sen - 1]
-        q = packed
+        q, mixw_cb = _pack_4bit(rng, q, n_sen)
     tp_float = synth_tmat_float(rng, 10, 3)
     pm = PackedModel(kind="s2_semi", n_sen=n_sen, n_mgau=1, n_feat=n_feat, n_density=n_density, topn=topn,
                      featlen=np.array(featlens, np.int32), mean=mean, var=var, det=det, mixw=q, mixw_cb=mixw_cb,
