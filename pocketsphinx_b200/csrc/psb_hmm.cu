@@ -17,7 +17,6 @@ struct psb_phoneloop_s {
     Stream stream;                // declared first: destroyed after the buffers below
     DevBuf<int32_t> d_ssid, d_tmatid;
     DevBuf<uint16_t> d_senid;     // [n_emit][n_phones]
-    DevBuf<int32_t> d_flags;      // [1] pathological-regime counter
 };
 
 namespace {
@@ -112,7 +111,7 @@ phoneloop_kernel(const int16_t *__restrict__ senscr, const int32_t *__restrict__
                  PlParams P, const uint16_t *__restrict__ senid_g, const int32_t *__restrict__ tmatid_g,
                  const int32_t *__restrict__ ssid_g,
                  int32_t *__restrict__ best_out, int32_t *__restrict__ pen_out,
-                 psb_hmm_t *__restrict__ final_out, psb_hmm_t *__restrict__ trace_out, int32_t *flags)
+                 psb_hmm_t *__restrict__ final_out, psb_hmm_t *__restrict__ trace_out)
 {
     extern __shared__ int sm[];
     const int H = P.n_phones, N = c.n_emit, tid = threadIdx.x;
@@ -179,7 +178,9 @@ phoneloop_kernel(const int16_t *__restrict__ senscr, const int32_t *__restrict__
         // prune_hmms (:241-261)
         const int nf = t + 1;
         int thresh = best_score + P.beam;
-        // phone_transition (:263-299): candidates among the survivors
+        // phone_transition (:263-299): candidates among the survivors.  The reference's loop also visits phones an
+        // earlier source entered in this frame; they were idle or just cleared, so their candidate, WORST_SCORE + pip,
+        // never beats the score the entering source left in any phone, and the max over survivors is exact
         const int xthresh = best_score + P.pbeam;
         int cand = INT_MIN, cidx = 0x7fffffff;
         for (int i = tid; i < H; i += blockDim.x) {
@@ -197,11 +198,7 @@ phoneloop_kernel(const int16_t *__restrict__ senscr, const int32_t *__restrict__
         }
         int widx;
         cand = block_reduce_max_pair<int>(cand, cidx, sidx, sval, widx);
-        if (tid == 0) {
-            if (best_out) best_out[f0 + t] = best_score;
-            // sequential-order corner the max formulation does not cover (see DESIGN.md)
-            if (cand != INT_MIN && PSB_WORST_SCORE + P.pip > xthresh) atomicAdd(flags, 1);
-        }
+        if (tid == 0 && best_out) best_out[f0 + t] = best_score;
         if (cand != INT_MIN) {
             const int whist = out_hist[widx];
             __syncthreads();
@@ -382,12 +379,10 @@ extern "C" int psb_phoneloop_create(psb_hmmctx_t *c, int32_t n_phones, const int
     rc = p->d_senid.reserve(senid.size());
     if (!rc) rc = p->d_tmatid.reserve((size_t)n_phones);
     if (!rc) rc = p->d_ssid.reserve((size_t)n_phones);
-    if (!rc) rc = p->d_flags.reserve(1);
     if (rc) return rc;
     cudaError_t e = cudaMemcpy(p->d_senid, senid.data(), senid.size() * 2, cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaMemcpy(p->d_tmatid, tmatid, (size_t)n_phones * 4, cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaMemcpy(p->d_ssid, ssid, (size_t)n_phones * 4, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemset(p->d_flags, 0, 4);
     if (e == cudaSuccess) e = p->stream.create();
     if (e != cudaSuccess) {
         psb_set_error("psb_phoneloop_create: %s", cudaGetErrorString(e));
@@ -417,7 +412,7 @@ int psb_phoneloop_launch(psb_phoneloop_t *p, const int16_t *d_senscr, const int3
     P.n_phones = H; P.window = p->window; P.beam = p->beam; P.pbeam = p->pbeam; P.pip = p->pip;
     P.penalty_weight = p->penalty_weight;
     phoneloop_kernel<<<n_utt, threads, smem, st>>>(d_senscr, d_utt_off, dev_ctx(p->c), P, p->d_senid, p->d_tmatid, p->d_ssid,
-                                                   d_best, d_pen, d_final, d_trace, p->d_flags);
+                                                   d_best, d_pen, d_final, d_trace);
     PSB_LAUNCH_CHECK();
     return PSB_OK;
 }

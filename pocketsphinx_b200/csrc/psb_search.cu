@@ -245,8 +245,8 @@ extern "C" int psb_ngram_fwdtree_batch_device(psb_hmmctx_t *c, const psb_ngram_d
                     "or the score stack (%d entries / %d scores allowed)", u, bp_cap_per_utt, bss_cap_per_utt);
         PSB_REQUIRE(result[u * 3 + 2] != -3, "psb_ngram_fwdtree_batch_device: utterance %d ran out of fan-out blocks "
                     "(PSB_NGS_BLOCKS)", u);
-        PSB_REQUIRE(result[u * 3 + 2] >= 0, "psb_ngram_fwdtree_batch_device: utterance %d needs score renormalisation "
-                    "(not done on the device)", u);
+        PSB_REQUIRE(result[u * 3 + 2] >= 0, "psb_ngram_fwdtree_batch_device: utterance %d: internal error (search status %d)",
+                    u, result[u * 3 + 2]);
     }
     return PSB_OK;
 }
@@ -364,8 +364,8 @@ extern "C" int psb_ngram_fwdflat_batch_device(psb_hmmctx_t *c, const psb_ngram_d
                     "or the score stack (%d entries / %d scores allowed)", u, bp_cap_per_utt, bss_cap_per_utt);
         PSB_REQUIRE(result[u * 3 + 2] != -3, "psb_ngram_fwdflat_batch_device: utterance %d: its vocabulary does not fit the state "
                     "area (PSB_NGF_CHANNELS)", u);
-        PSB_REQUIRE(result[u * 3 + 2] >= 0, "psb_ngram_fwdflat_batch_device: utterance %d needs score renormalisation "
-                    "(not done on the device)", u);
+        PSB_REQUIRE(result[u * 3 + 2] >= 0, "psb_ngram_fwdflat_batch_device: utterance %d: internal error (search status %d)",
+                    u, result[u * 3 + 2]);
     }
     return PSB_OK;
 }
@@ -447,7 +447,9 @@ extern "C" int psb_ngram_two_pass_batch_device(psb_hmmctx_t *c, const psb_ngram_
                     u, bp_cap_per_utt, bss_cap_per_utt);
         PSB_REQUIRE(r1[(size_t)u * 3 + 2] != -3 && result[u * 3 + 2] != -3, "psb_ngram_two_pass_batch_device: utterance %d ran out of fan-out blocks "
                     "(PSB_NGS_BLOCKS) or state channels (PSB_NGF_CHANNELS)", u);
-        PSB_REQUIRE(r1[(size_t)u * 3 + 2] >= 0 && result[u * 3 + 2] >= 0, "psb_ngram_two_pass_batch_device: utterance %d needs score renormalisation", u);
+        PSB_REQUIRE(r1[(size_t)u * 3 + 2] >= 0 && result[u * 3 + 2] >= 0,
+                    "psb_ngram_two_pass_batch_device: utterance %d: internal error (search status %d in the first pass, %d in "
+                    "the second)", u, r1[(size_t)u * 3 + 2], result[u * 3 + 2]);
     }
     return PSB_OK;
 }

@@ -202,14 +202,33 @@ def _band_cases(n_emit):
         H = len(word)
         ssid = rng.integers(0, len(pm.sseq), H).astype(np.int32)
         tmat = rng.integers(0, pm.tp.shape[0], H).astype(np.int32)
-        hi_scr = k in (3, 9)                                 # renormalisation
+        hi_scr = k in (3, 9)                                 # large scores, far from the floor in so few frames
         scr = rng.integers(20000, 32000, (max(T, 1), pm.n_sen)) if hi_scr else rng.integers(0, 400, (max(T, 1), pm.n_sen))
         cases.append((ssid, tmat, sf, ef, scr[:max(T, 1)].astype(np.int16)))
     # untimed chains: the full width
     H = 30
     cases.append((rng.integers(0, len(pm.sseq), H).astype(np.int32), rng.integers(0, pm.tp.shape[0], H).astype(np.int32),
                   None, None, rng.integers(0, 400, (150, pm.n_sen)).astype(np.int16)))
+    cases.append(_renorm_case(pm, n_emit))
     return pm, cases
+
+
+RENORM_T = 20000
+
+
+def _renorm_case(pm, n_emit):
+    """A windowed chain over RENORM_T frames at >= 30 000 per frame: the best score falls below the alignment's
+    bound (best_score - 0x300000 < WORST_SCORE, -533 725 184) by frame 17 792, and the search renormalises."""
+    from pocketsphinx_b200.align import phone_windows
+    rng = np.random.default_rng(50 + n_emit)
+    n_words = 30
+    dur = rng.multinomial(RENORM_T - 20 * n_words, np.ones(n_words) / n_words) + 20
+    start = np.concatenate([[0], np.cumsum(dur)[:-1]])
+    word = np.repeat(np.arange(n_words), rng.integers(1, 4, n_words))
+    sf, ef = phone_windows(start[word], dur[word], n_emit)
+    H = len(word)
+    return (rng.integers(0, len(pm.sseq), H).astype(np.int32), rng.integers(0, pm.tp.shape[0], H).astype(np.int32), sf, ef,
+            rng.integers(30000, 32768, (RENORM_T, pm.n_sen)).astype(np.int16))
 
 
 @pytest.mark.parametrize("n_emit", [3, 5])
@@ -220,7 +239,7 @@ def test_band_restatement_keeps_every_token_and_result(n_emit):
     pm, cases = _band_cases(n_emit)
     kinds = set()
     narrower = 0
-    for ssid, tmat, sf, ef, scr in cases:
+    for k, (ssid, tmat, sf, ef, scr) in enumerate(cases):
         T, H = len(scr), len(ssid)
         lo, hi = align_cases.band(H, T, sf, ef)
         plo, phi = token_band(sf, ef, T, H)
@@ -232,6 +251,10 @@ def test_band_restatement_keeps_every_token_and_result(n_emit):
         for a, b in zip(got[1:4], want[1:4]):
             assert np.array_equal(a, b)
         kinds.add(0 if want[0] == 0 else (-1 if want[0] == -1 else -2))
+        if k == len(cases) - 1:
+            # the bound was crossed: without renormalisation no state scores above 0 (token scores only fall along a
+            # path), while a state that spans it scores a normalised minus a raw token score
+            assert T == RENORM_T and want[0] == 0 and (want[3] > 0).any()
         n = band_tokens(sf, ef, T, H, n_emit)
         assert n <= T * H * n_emit
         narrower += n < T * H * n_emit

@@ -789,7 +789,8 @@ def test_align_batch_matches_oracle(api, n_emit):
     ssid = [rng.integers(0, len(pm.sseq), n).astype(np.int32) for n in n_phones]
     tmat = [rng.integers(0, pm.tp.shape[0], n).astype(np.int32) for n in n_phones]
     scr = [rng.integers(0, 400, (t, pm.n_sen)).astype(np.int16) for t in frames]
-    # renormalisation: one utterance with huge negative scores so that best_score sinks below the bound
+    # one utterance with large senone scores: 500 frames sink the best score by ~13 M, far short of the
+    # renormalisation bound (tests/test_gpu_viterbi_renorm.py crosses it)
     scr[8] = rng.integers(20000, 32000, (frames[8], pm.n_sen)).astype(np.int16)
     sf = [np.zeros(n, np.int32) for n in n_phones]
     ef = [np.full(n, 2**31 - 1, np.int32) for n in n_phones]
