@@ -164,7 +164,7 @@ int psb_batch_ms_plan(psb_batch_t *b, int64_t total_frames, int64_t *out, int32_
 /* debugging/tests: how a batch of total_frames frames on a ptm or semi-continuous model is scored -- the plan the batch
  * launcher runs.  out[0..n-1] receives the first n of, in order: the top-N paths its streams take, as bits
  * (1 tensor-core filter, 2 PTM deferred-insertion scan, 4 PTM scalar scan, 8 semi-continuous split distances and scan,
- * 16 semi-continuous paired scan, 32 semi-continuous scalar scan, 64 fixed-point scan); the senone kernel (0
+ * 16 fixed-point scan); the senone kernel (0
  * ptm_senone4, 1 ptm_senone 8-bit, 2 ptm_senone 4-bit, 3 semi_senone4, 4 semi_senone 8-bit, 5 semi_senone 4-bit); its
  * threads per CTA; the senones ptm_senone4 evaluates one by one (quads that straddle a codebook boundary, and the
  * tail); its dynamic shared memory in bytes.  What the batch kernels refuse (a -topn other than 4, more than 512

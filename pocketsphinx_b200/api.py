@@ -223,7 +223,7 @@ class Batch:
         check(lib().psb_batch_ms_plan(self.h, int(total_frames), _p(v), len(v)), "psb_batch_ms_plan")
         return {k: int(x) for k, x in zip(self.MS_PLAN, v)}
 
-    TM_TOPN = ("tc_filter", "ptm_scan", "ptm_scalar", "semi_split", "semi_pairs", "semi_scalar", "fixed")
+    TM_TOPN = ("tc_filter", "ptm_scan", "ptm_scalar", "semi_split", "fixed")
     TM_SENONE = ("ptm_senone4", "ptm_senone_8b", "ptm_senone_4b", "semi_senone4", "semi_senone_8b", "semi_senone_4b")
 
     def tm_plan(self, total_frames):

@@ -87,8 +87,8 @@ static int build_records(psb_model_t *m, const float *mean, const float *var, co
         if (rc) return rc;
     }
     PSB_CUDA(cudaMemcpy(m->d_rec, rec.data(), total * sizeof(float), cudaMemcpyHostToDevice));
-    if (m->kind != PSB_KIND_MS && m->n_density % 2 == 0 && !m->fixed_point) {
-        // pair-interleaved, negated copy for ptm_topn2_kernel: per (cb, f) nd/2 pair records
+    if (m->kind == PSB_KIND_PTM && m->n_density % 2 == 0 && !m->fixed_point) {
+        // pair-interleaved, negated copy for ptm_topnq_kernel: per (cb, f) nd/2 pair records
         // {detA, detB, -muA_0, -muB_0, -vA_0, -vB_0, ...} padded to a multiple of 4 floats
         size_t total2 = 0;
         std::vector<size_t> off2(m->K);
@@ -157,6 +157,8 @@ extern "C" int psb_model_create(const psb_model_desc_t *d, int device, psb_model
     PSB_REQUIRE(d->n_sen > 0 && d->n_mgau > 0 && d->n_density > 0, "empty model");
     PSB_REQUIRE(d->topn >= 1 && d->topn <= PSB_MAX_TOPN, "topn %d out of range", d->topn);
     PSB_REQUIRE(d->mean && d->var && d->det && d->mixw && d->sen2cb, "missing model array");
+    // the reference loads semi-continuous models with a single codebook only (s2_semi_mgau.c:1269)
+    PSB_REQUIRE(d->kind != PSB_KIND_SEMI || d->n_mgau == 1, "a semi-continuous model has one codebook (got n_mgau %d)", d->n_mgau);
     PSB_CUDA(cudaSetDevice(device));
     PSB_REQUIRE(!(d->fixed_point && d->kind == PSB_KIND_MS), "fixed-point arithmetic is implemented for ptm and semi-continuous models only");
     std::unique_ptr<psb_model_t> m(new psb_model_t());

@@ -1,5 +1,5 @@
 // psb_gau.cuh -- the Gaussian exponent with the reference's roundings, shared by the top-N kernels
-// (psb_ptm.cu: scans over time; psb_ptm_tc.cu: tensor-core filter + exact rescoring).
+// (psb_ptm.cu: scans over time; psb_ptm_tc.cu: tensor-core filter + exact rescoring; psb_scorer.cu: per frame).
 #pragma once
 #include "psb_internal.cuh"
 
@@ -10,6 +10,18 @@ __device__ __forceinline__ int f2i_clamped(float d)
     // (int32)d, clamped first like ptm_mgau.c:129-132,219-222.  cvt.rzi saturates, which is
     // the same thing for d < INT_MIN; d > INT_MAX cannot occur (d <= det).
     return __float2int_rz(d);
+}
+
+// FIXED_POINT build of the reference (mfcc_t = int32 Q12, SURVEY A.1.11).  FIXMUL (fe/fixpoint.h:98-100) is the
+// 64-bit product shifted right by 12 and truncated to 32 bits; GMMSUB (tied_mgau_common.h:62-66) as gcc compiles it
+// is (b < 0) ? INT_MIN : wrap32(a - b).
+__device__ __forceinline__ int fx_mul(int a, int b)
+{
+    return (int)(unsigned)(((long long)a * (long long)b) >> 12);
+}
+__device__ __forceinline__ int fx_gmmsub(int a, int b)
+{
+    return b < 0 ? INT_MIN : (int)((unsigned)a - (unsigned)b);
 }
 
 // dpen (optional) = the partial sum before the last dimension's term: the semi-continuous

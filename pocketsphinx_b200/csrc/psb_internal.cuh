@@ -94,7 +94,7 @@ struct psb_model_s {
     DevBuf<float> d_rec;          // records; (cb, f) block at rec_off[cb * n_feat + f]
     std::vector<size_t> rec_off;  // float offsets, host copy
     DevBuf<size_t> d_rec_off;
-    DevBuf<float> d_rec2;         // pair-interleaved, negated records for the codeword-pair kernels
+    DevBuf<float> d_rec2;         // pair-interleaved, negated records for ptm_topnq_kernel (float PTM models)
     DevBuf<size_t> d_rec2_off;
     DevBuf<uint8_t> d_mixw;       // [n_feat][n_density][mixw_stride] (ptm/semi) or raw pdf (ms)
     DevBuf<uint8_t> d_mixw_cb;    // 16 bytes or null

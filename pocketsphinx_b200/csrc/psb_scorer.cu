@@ -4,7 +4,9 @@
 // Latency path (one frame per call), so the mapping differs from the batch kernels: one CTA
 // per (codebook, stream) pair with one *thread per codeword* computing the full distance, then
 // a single thread replays the reference's insertion scan over the staged distances.
+#include "psb_gau.cuh"
 #include "psb_internal.cuh"
+#include "psb_tm.cuh"
 
 #include <string.h>
 
@@ -28,13 +30,6 @@ struct psb_scorer_s {
 
 namespace {
 
-__device__ __forceinline__ int logadd8(const uint8_t *tab, int x, int y)
-{
-    const int d = x - y;
-    const int r = d > 0 ? y : x;
-    return r - tab[d > 0 ? d : -d];
-}
-
 // eval_topn + eval_cb for every (codebook, stream) pair of one frame (ptm_mgau.c:232-254;
 // SEMI: mgau_dist, s2_semi_mgau.c:172-183, whose scan also needs the partial sum before the last
 // dimension, :137-155).
@@ -52,7 +47,7 @@ scorer_topn_kernel(const float *__restrict__ rec, const size_t *__restrict__ rec
     const int rf = (1 + 2 * fl + 3) / 4 * 4;
     if (threadIdx.x < fl) sx[threadIdx.x] = feat[fo + threadIdx.x];
     __syncthreads();
-    // FIXED_POINT arithmetic (fx): Q12 integers, FIXMUL / GMMSUB, and because the scan's early exits are
+    // FIXED_POINT arithmetic (fx): Q12 integers, fx_mul / fx_gmmsub, and because the scan's early exits are
     // observable there, the minimum of d over the reference's test points next to the final value
     // (see gau_dist_fx in psb_ptm.cu); sd[] then carries int32 bit patterns.
     if (fx) {
@@ -62,9 +57,7 @@ scorer_topn_kernel(const float *__restrict__ rec, const size_t *__restrict__ rec
             for (int j = 0; j < fl; ++j) {
                 if (SEMI || j < fl % 4 || (j - fl % 4) % 4 == 0) mn = min(mn, d);
                 const int diff = (int)((unsigned)__float_as_int(sx[j]) - (unsigned)__float_as_int(r[1 + 2 * j]));
-                const int sq = (int)(unsigned)(((long long)diff * diff) >> 12);
-                const int c2 = (int)(unsigned)(((long long)sq * __float_as_int(r[2 + 2 * j])) >> 12);
-                d = c2 < 0 ? INT_MIN : (int)((unsigned)d - (unsigned)c2);
+                d = fx_gmmsub(d, fx_mul(fx_mul(diff, diff), __float_as_int(r[2 + 2 * j])));
             }
             sd[c] = __int_as_float(d);
             sd[nd + c] = __int_as_float(min(mn, d));
@@ -186,14 +179,8 @@ scorer_senone_kernel(int32_t *__restrict__ slot_cw, int32_t *__restrict__ slot_s
             const uint8_t *row = mixw + (size_t)f * nd * mixw_stride;
             int fden = 0;
             for (int j = 0; j < topn; ++j) {
-                int w;
-                if (FOURBIT) {
-                    int b = row[(size_t)cw[base + j] * mixw_stride + (s >> 1)];
-                    b = (b & 1) ? b >> 4 : b & 0x0f;
-                    w = cb16[b];
-                }
-                else
-                    w = row[(size_t)cw[base + j] * mixw_stride + s];
+                const int w = FOURBIT ? ptm_weight4(cb16, row[(size_t)cw[base + j] * mixw_stride + (s >> 1)])
+                                      : row[(size_t)cw[base + j] * mixw_stride + s];
                 const int v = w + sc[base + j];
                 fden = j == 0 ? v : logadd8(tab, fden, v);
             }
@@ -202,17 +189,7 @@ scorer_senone_kernel(int32_t *__restrict__ slot_cw, int32_t *__restrict__ slot_s
         best = min(best, ascore);
         asc[s] = (int16_t)ascore;     // duplicate ids in a bridged list recompute the same value
     }
-    best = __reduce_min_sync(0xffffffffu, best);
-    if ((tid & 31) == 0) red[tid >> 5] = best;
-    __syncthreads();
-    if (tid < 32) {
-        int v = tid < (int)(blockDim.x >> 5) ? red[tid] : 0x7fffffff;
-        v = __reduce_min_sync(0xffffffffu, v);
-        if (tid == 0) red[0] = v;
-    }
-    __syncthreads();
-    best = red[0];
-    for (int i = tid; i < n_sen; i += blockDim.x) senscr[i] = (int16_t)(asc[i] - best);    // :398-400
+    store_relative_to_best(best, red, asc, senscr, n_sen);
     for (int i = tid; i < K * topn; i += blockDim.x) slot_sc[i] = sc[i];
 }
 
@@ -266,13 +243,8 @@ scorer_semi_senone_kernel(int32_t *__restrict__ slot_cw, int32_t *__restrict__ s
             const uint8_t *row = mixw + (size_t)f * nd * mixw_stride;
             int tmp = 0;
             for (int k = 0; k == 0 || k < tn; ++k) {
-                int w;
-                if (FOURBIT) {
-                    const int b = row[(size_t)cw[f * topn + k] * mixw_stride + (s >> 1)];
-                    w = cb16[(s & 1) ? b >> 4 : b & 0x0f];
-                }
-                else
-                    w = row[(size_t)cw[f * topn + k] * mixw_stride + s];
+                const int w = FOURBIT ? semi_weight4(cb16, row[(size_t)cw[f * topn + k] * mixw_stride + (s >> 1)], s)
+                                      : row[(size_t)cw[f * topn + k] * mixw_stride + s];
                 int v = w + sc[f * topn + k];
                 if (wrap8) v &= 0xff;
                 tmp = k == 0 ? v : logadd8(tab, tmp, v);

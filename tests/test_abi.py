@@ -102,3 +102,16 @@ def test_fe_create_rejects_bad_descriptors_before_touching_the_device():
                        (dict(n_filt=200), "n_cep <= n_filt")):
         rc = L.psb_fe_create(C.byref(desc(**over)), 0, C.byref(h))
         assert rc < 0 and word in L.psb_last_error().decode(), (over, L.psb_last_error())
+
+
+def test_model_create_refuses_a_semi_model_with_several_codebooks_before_touching_the_device():
+    """A semi-continuous model has one codebook (the reference refuses others, s2_semi_mgau.c:1269): psb_model_create
+    says so without a GPU."""
+    import copy
+    import pytest
+    from pocketsphinx_b200 import api
+    from pocketsphinx_b200.model import synth_semi
+    pm = copy.copy(synth_semi(n_density=64, n_sen=100))
+    pm.n_mgau = 2
+    with pytest.raises(api.PsbError, match="one codebook"):
+        api.Model(pm)

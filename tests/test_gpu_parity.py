@@ -191,12 +191,16 @@ def test_decode_host_end_to_end(api, en_us, en_us_dev):
 # ---------------------------------------------------------------------------------------
 # semi-continuous (s2_semi_mgau) and generic multi-stream (ms_mgau) back-ends, batched
 
-def _batch_vs_oracle(api, pm, feats_by_utt):
+def _batch_vs_oracle(api, pm, feats_by_utt, topn_path=None):
+    """Score a batch on the device and compare every utterance with the oracle; topn_path: the top-N path the plan
+    must name (Batch.tm_plan)."""
     from oracle import oracle
     m = api.Model(pm)
     lens = [len(f) for f in feats_by_utt]
     b = api.Batch(m, len(lens) + 1, sum(lens) + 8)
     off = api.Batch.offsets(lens)
+    if topn_path is not None:
+        assert b.tm_plan(int(off[-1]))["topn"] == topn_path, b.tm_plan(int(off[-1]))
     scr = b.score_host(np.concatenate(feats_by_utt), off)
     rec = b.get_topn(int(off[-1])) if pm.kind == "ptm" else None
     om = oracle.OracleModel(pm)
@@ -376,14 +380,15 @@ def _ragged_70(pm):
     return [feats[u][:n].reshape(n, pm.sumlen) for u, n in enumerate(lens)]
 
 
-# path -> model maker (seed, n_density, n_sen); the semi paths that need other densities ignore n_density
+# case -> (top-N path, model maker (seed, n_density, n_sen)); the semi cases of other shapes ignore n_density
 TOPN_PATHS = {
-    "tc_filter": lambda seed, nd, n_sen: synth_ptm(seed=seed, n_density=nd, n_sen=n_sen),
-    "ptm_scan": lambda seed, nd, n_sen: synth_ptm(seed=seed, n_density=nd, n_sen=n_sen, featlen=12),
-    "ptm_scalar": lambda seed, nd, n_sen: synth_ptm(seed=seed, n_density=nd, n_sen=n_sen, featlen=39),
-    "semi_split": lambda seed, nd, n_sen: synth_semi(seed=seed, n_density=nd, n_sen=n_sen),
-    "semi_pairs": lambda seed, nd, n_sen: synth_semi(seed=seed, n_density=96, n_sen=n_sen),
-    "semi_scalar": lambda seed, nd, n_sen: synth_semi(seed=seed, n_density=96, n_sen=n_sen, featlens=(39,)),
+    "tc_filter": ("tc_filter", lambda seed, nd, n_sen: synth_ptm(seed=seed, n_density=nd, n_sen=n_sen)),
+    "ptm_scan": ("ptm_scan", lambda seed, nd, n_sen: synth_ptm(seed=seed, n_density=nd, n_sen=n_sen, featlen=12)),
+    "ptm_scalar": ("ptm_scalar", lambda seed, nd, n_sen: synth_ptm(seed=seed, n_density=nd, n_sen=n_sen, featlen=39)),
+    "semi_split": ("semi_split", lambda seed, nd, n_sen: synth_semi(seed=seed, n_density=nd, n_sen=n_sen)),
+    "semi_split_nd96": ("semi_split", lambda seed, nd, n_sen: synth_semi(seed=seed, n_density=96, n_sen=n_sen)),
+    "semi_split_fl39": ("semi_split",
+                        lambda seed, nd, n_sen: synth_semi(seed=seed, n_density=96, n_sen=n_sen, featlens=(39,))),
 }
 
 
@@ -393,12 +398,12 @@ def test_topn_path_follows_the_model(api, en_us, en_us_dev, path):
     tc_filter   13-dimensional PTM, 64/128/256 densities, -ds 1: tensor-core filter, exact rows, fix-up
     ptm_scan    other PTM with streams of up to 16 dimensions: ptm_topnq_kernel
     ptm_scalar  streams longer than 16 dimensions: ptm_topn_kernel<FL, false, false>
-    semi_split  semi-continuous, one codebook of 64/128/256 densities: semi_dist_kernel + semi_scan_kernel
-    semi_pairs  other semi-continuous models, streams of up to 16 dimensions: ptm_topn2_kernel
-    semi_scalar semi-continuous, streams longer than 16 dimensions: ptm_topn_kernel<FL, true, false>"""
+    semi_split  semi-continuous (float): semi_dist_kernel + semi_scan_kernel, whatever the density count (a multiple
+                of 32) and stream length: 256 densities of s2_4x streams, 96 densities of s2_4x streams, 96 densities
+                of one 39-dimensional stream"""
     import copy
     from oracle import oracle
-    make = TOPN_PATHS[path]
+    want_path, make = TOPN_PATHS[path]
     g = golden("en_us_goforward.npz")
     if path == "tc_filter":
         # (1) shipped model, real features
@@ -414,7 +419,7 @@ def test_topn_path_follows_the_model(api, en_us, en_us_dev, path):
         _batch_vs_oracle(api, en2, [g["feats"]])
     # (2) ragged batch of 70 utterances
     pm = make(11, 256, 600)
-    _batch_vs_oracle(api, pm, _ragged_70(pm))
+    _batch_vs_oracle(api, pm, _ragged_70(pm), topn_path=want_path)
     # (3) exact ties everywhere
     pmq, gen = quantize_for_ties(make(2, 64, 400), seed=6)
     _batch_vs_oracle(api, pmq, list(gen(40, 25, s=9)))
