@@ -430,6 +430,17 @@ int psb_allphone_net_batch_device(psb_hmmctx_t *c, const int16_t *d_senscr, cons
                                   const int32_t *tg, int32_t cap_per_utt, int32_t *res, int32_t *segs,
                                   int32_t seg_cap, int32_t *hist);
 
+/* The phone LM's tables for the two entry points above, from the LM itself (host code, no device work;
+ * once per decoder: 42^3 cells on en-us).  lm_block is the int32 block of psb_ngram_desc_t.lm_arrays
+ * (the binary trie LM with -lw / -wip applied, as ngram_model_read applies them, lm/ngram_model.c:173-178)
+ * whose "dictionary" is the model's n_ci CI phones in CI order: its widmap is allphone_search_init's
+ * ci2lmwid (allphone_search.c:552-577), a phone the LM lacks mapped to SIL's LM word.  Fills
+ *   bg [n_ci][n_ci]        bg[a][b]    = ngram_bg_score(lm, wid[a], wid[b]) >> SENSCR_SHIFT
+ *   tg [n_ci][n_ci][n_ci]  tg[a][b][c] = ngram_tg_score(lm, wid[a], wid[b], wid[c]) >> SENSCR_SHIFT
+ * with the scorer the n-gram kernels use (psb_lm_core.h).  Refuses n_ci outside 1..64, a block whose
+ * widmap is not n_ci entries, and a widmap entry outside the LM's vocabulary, before writing anything. */
+int psb_allphone_lm_tables(const int32_t *lm_block, int32_t n_ci, int32_t *bg, int32_t *tg);
+
 /* ------------------------------------------------------------------------------------ */
 /* STATUS of the search entry points below (psb_fsg_batch_device, psb_ngram_*_batch_device): their phase
  * code reproduces the reference's tables in host emulation and is race-checked (tests/emul/), the kernels

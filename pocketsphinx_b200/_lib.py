@@ -118,6 +118,7 @@ SYMBOLS = [
     ("psb_allphone_batch_device", C.c_int, [_VP, _VP, _VP, _I32, _I32, _VP, _VP, _VP, _VP, _I32, _I32, _I32, _I32, _VP, _I32, _VP]),
     ("psb_allphone_lm_batch_device", C.c_int, [_VP, _VP, _VP, _I32, _I32, _VP, _VP, _VP, _VP, _I32, _I32, _I32, _I32, _VP, _VP, _VP, _VP, _I32, _VP]),
     ("psb_allphone_net_batch_device", C.c_int, [_VP, _VP, _VP, _I32, _I32, _VP, _VP, _VP, _VP, _VP, _I32, _I32, _I32, _I32, _I32, _VP, _VP, _I32, _VP, _VP, _I32, _VP]),
+    ("psb_allphone_lm_tables", C.c_int, [_VP, _I32, _VP, _VP]),
     ("psb_kws_batch_device", C.c_int, [_VP, _VP, _VP, _I32, _I32, _VP, _VP, _I32, _VP, _VP, _VP, _VP, _I32, _I32, _VP, _I32, _VP]),
     ("psb_fsg_batch_device", C.c_int, [_VP, C.POINTER(FsgDesc), _VP, _VP, _I32, _VP, _I32, _VP]),
     ("psb_ngram_fwdtree_batch_device", C.c_int, [_VP, C.POINTER(NgramDesc), _VP, _VP, _I32, _VP, _I32, _VP, _I32, _VP, _I32, _VP, _VP]),

@@ -138,6 +138,31 @@ extern "C" int32_t psb_ngram_backtrace(const int32_t *bp, int32_t n_bp, int32_t 
     return n;
 }
 
+// The phone LM's dense tables of allphone_search (allphone_search.c:420-441, 497-513), scored through the
+// same restatement of ngram_tg_score the n-gram kernels use: the block's "dictionary" is the CI phones, its
+// widmap allphone_search_init's ci2lmwid (:552-577).  Everything is checked before the first write.
+extern "C" int psb_allphone_lm_tables(const int32_t *lm_block, int32_t n_ci, int32_t *bg, int32_t *tg)
+{
+    PSB_REQUIRE(lm_block && bg && tg, "psb_allphone_lm_tables: bad arguments");
+    PSB_REQUIRE(n_ci > 0 && n_ci <= 64, "psb_allphone_lm_tables: %d CI phones (1 to 64: the phone net's context sets are 64-bit masks)", n_ci);
+    PSB_REQUIRE(lm_block[7] == n_ci, "psb_allphone_lm_tables: the block maps %d words, not the %d CI phones", lm_block[7], n_ci);
+    std::string err;
+    if (lm_arr_check(lm_block, (long long)lm_arr_words(lm_block), n_ci, err) != 0)
+        PSB_REQUIRE(false, "psb_allphone_lm_tables: %s", err.c_str());
+    LmArr L;
+    lm_arr_bind(L, lm_block, lm_block);
+    for (int a = 0; a < n_ci; ++a)
+        PSB_REQUIRE(L.widmap[a] >= 0 && L.widmap[a] < L.V, "psb_allphone_lm_tables: CI phone %d maps to LM word %d, outside the LM's %d words",
+                    a, L.widmap[a], L.V);
+    for (int a = 0; a < n_ci; ++a)
+        for (int b = 0; b < n_ci; ++b) {
+            bg[a * n_ci + b] = lm_tg_score(L, a, b, -1) >> PSB_SENSCR_SHIFT;       // ngram_bg_score(lm, wid[a], wid[b])
+            for (int c = 0; c < n_ci; ++c)
+                tg[((size_t)a * n_ci + b) * n_ci + c] = lm_tg_score(L, a, b, c) >> PSB_SENSCR_SHIFT;
+        }
+    return PSB_OK;
+}
+
 // ngram_search_bp2itor (ngram_search.c:886-928) for every entry of the chain: what ps_seg_iter reports
 // without -bestpath.  seg [cap][7] = {entry, wid, sf, ef, path score, ascr, lscr}; the right-context
 // exit score of the predecessor comes from the score stack (ngram_search_exit_score :655-676), the LM
