@@ -809,6 +809,45 @@ int psb_vad_feed_device(psb_vad_t *v, const int32_t *slots, int32_t n, const int
                         const int8_t *final, int8_t *d_flags, int32_t *frame_off, int32_t *d_seg_n, int64_t *d_segs,
                         double *d_times, psb_vad_live_status_t *d_status, float *ms);
 
+/* ------------------------------------------------------------------------------------ */
+/* YIN pitch tracking for whole batches of int16 streams (fe/yin.c, driven as pocketsphinx_pitch's
+ * extract_pitch drives it): each stream gets a fresh yin_t; frame f is samples f * frame_shift ..
+ * f * frame_shift + frame_size - 1, so a stream of N samples has 1 + (N - frame_size) / frame_shift frames
+ * when N >= frame_size and none otherwise; yin_write then yin_read run on every frame, then yin_end and
+ * yin_read until it fails.  The outputs are the (period, bestdiff) of every read that succeeds, bit for bit,
+ * including the reference's quirks: never-written window slots read period 0 and a row of zeros, and
+ * the uint16 frame counter makes smooth_window + 1 reads fail after every 65 536 frames.
+ * Options as the program's: frame_size = (size_t)(0.5 + sample_rate * flen), frame_shift likewise from
+ * fshift, voice_thresh and search_range become (uint16)((float)value * 32768).
+ * Refused: sample_rate <= 0, frame_size < 2 (ndiff = frame_size / 2 < 1), frame_shift of 0 or greater than
+ * frame_size, smooth_window outside 0..127 (the window of 2 * smooth_window + 1 frames is an unsigned
+ * char), thresholds whose Q15 value does not fit 0..65535.  Also refused, though the reference accepts
+ * it: frame_size above PSB_PITCH_MAX_FRAME samples (a frame and its per-lag sums are kept in one CTA's
+ * shared memory). */
+#define PSB_PITCH_MAX_FRAME 16384
+typedef struct psb_pitch_opts_s {
+    int32_t sample_rate;          /* Hz (-samprate) */
+    int32_t smooth_window;        /* frames on either side of the current one (-smooth_window) */
+    double flen, fshift;          /* seconds (-flen, -fshift) */
+    double voice_thresh;          /* -voice_thresh */
+    double search_range;          /* -search_range */
+} psb_pitch_opts_t;
+typedef struct psb_pitch_s psb_pitch_t;
+int psb_pitch_create(const psb_pitch_opts_t *o, int device, psb_pitch_t **out);
+void psb_pitch_free(psb_pitch_t *h);
+int32_t psb_pitch_frame_size(const psb_pitch_t *h);    /* samples per frame */
+int32_t psb_pitch_frame_shift(const psb_pitch_t *h);   /* samples between frames */
+int32_t psb_pitch_ndiff(const psb_pitch_t *h);         /* lags per frame: frame_size / 2 */
+/* pcm: the streams' samples back to back, samp_off int64[n_streams + 1] (host, samp_off[0] = 0).
+ * Outputs: out_off int32[n_streams + 1] (host): stream s's reads are out_off[s] .. out_off[s + 1] - 1 of
+ * period and bestdiff (uint16, as yin_read returns them); a stream has at most one read per frame, so
+ * room for the streams' frames is enough.  _device: pcm, period and bestdiff on the device.  *ms (may
+ * be NULL) = device time of the kernels. */
+int psb_pitch_process_host(psb_pitch_t *h, const int16_t *pcm, const int64_t *samp_off, int32_t n_streams,
+                           int32_t *out_off, uint16_t *period, uint16_t *bestdiff, float *ms);
+int psb_pitch_process_device(psb_pitch_t *h, const int16_t *d_pcm, const int64_t *samp_off, int32_t n_streams,
+                             int32_t *out_off, uint16_t *d_period, uint16_t *d_bestdiff, float *ms);
+
 /* number of kernels launched by this library in the calling process so far */
 int64_t psb_kernel_launch_count(void);
 /* bytes of device and pinned host memory this library holds now, over all handles */

@@ -66,6 +66,11 @@ class VadOpts(C.Structure):
                 ("ratio", C.c_double), ("warmup", C.c_int32)]
 
 
+class PitchOpts(C.Structure):
+    _fields_ = [("sample_rate", C.c_int32), ("smooth_window", C.c_int32), ("flen", C.c_double), ("fshift", C.c_double),
+                ("voice_thresh", C.c_double), ("search_range", C.c_double)]
+
+
 class NgramDesc(C.Structure):
     _fields_ = [("info", C.c_void_p), ("model", C.c_void_p), ("model_len", C.c_int64), ("ci_tmat", C.c_void_p),
                 ("ci_ssid", C.c_void_p), ("lm_arrays", C.c_void_p), ("lm_arrays_len", C.c_int64)]
@@ -177,6 +182,13 @@ SYMBOLS = [
     ("psb_vad_live_reset", C.c_int, [_VP, _VP, _I32]),
     ("psb_vad_feed_host", C.c_int, [_VP, _VP, _I32, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP]),
     ("psb_vad_feed_device", C.c_int, [_VP, _VP, _I32, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, _VP, C.POINTER(C.c_float)]),
+    ("psb_pitch_create", C.c_int, [C.POINTER(PitchOpts), C.c_int, C.POINTER(_VP)]),
+    ("psb_pitch_free", None, [_VP]),
+    ("psb_pitch_frame_size", _I32, [_VP]),
+    ("psb_pitch_frame_shift", _I32, [_VP]),
+    ("psb_pitch_ndiff", _I32, [_VP]),
+    ("psb_pitch_process_host", C.c_int, [_VP, _VP, _VP, _I32, _VP, _VP, _VP, C.POINTER(C.c_float)]),
+    ("psb_pitch_process_device", C.c_int, [_VP, _VP, _VP, _I32, _VP, _VP, _VP, C.POINTER(C.c_float)]),
     ("psb_kernel_launch_count", _I64, []),
     ("psb_device_bytes_live", _I64, []),
 ]

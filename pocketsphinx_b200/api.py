@@ -1095,3 +1095,82 @@ class Vad(Endpointer):
 
     def __init__(self, mode=0, sample_rate=16000, frame_length=0.03, device=0, warmup=None):
         super().__init__(0.3, 0.9, mode, sample_rate, frame_length, device, warmup)
+
+
+def pitch_main_reads(n_frames, smooth_window):
+    """The reads pocketsphinx_pitch makes inside its frame loop that succeed (psb_pitch_main_reads): yin_t's uint16
+    frame counter makes smooth_window + 1 of them fail after every 65 536 frames."""
+    if smooth_window == 0:
+        return n_frames
+    r = n_frames % 65536
+    return n_frames // 65536 * (65535 - smooth_window) + max(r - smooth_window, 0)
+
+
+def pitch_result(period, bestdiff, main_reads, frame_shift, sample_rate):
+    """One stream's reads as pocketsphinx_pitch prints them: period and bestdiff (uint16, as yin_read returns them),
+    time (the samples of the main loop's reads before this one over the rate: every read after the loop shares the
+    last time), voicing (1 - bestdiff / 32768, 0 above 32768) and pitch (sample_rate / period, sample_rate for 0)."""
+    period = np.asarray(period, np.uint16)
+    bestdiff = np.asarray(bestdiff, np.uint16)
+    k = np.minimum(np.arange(len(period), dtype=np.int64), main_reads)
+    bd = bestdiff.astype(np.float64)
+    p = period.astype(np.float64)
+    return dict(period=period, bestdiff=bestdiff,
+                time=(k * frame_shift).astype(np.float64) / sample_rate,
+                voicing=np.where(bestdiff > 32768, 0.0, 1.0 - bd / 32768),
+                pitch=np.where(period == 0, float(sample_rate), float(sample_rate) / np.where(period == 0, 1.0, p)))
+
+
+def pitch_lines(result, sample_rate):
+    """pocketsphinx_pitch's output lines for one stream's result ("%.3f %.2f %.2f\\n" each: time, voicing, pitch, with
+    voicing and pitch computed from bestdiff and period as the program computes them); joined, they are the program's
+    output file byte for byte."""
+    sps = float(sample_rate)
+    return ["%.3f %.2f %.2f\n" % (t, 0.0 if bd > 32768 else 1.0 - bd / 32768.0, sps if p == 0 else sps / p)
+            for t, p, bd in zip(result["time"].tolist(), result["period"].tolist(), result["bestdiff"].tolist())]
+
+
+class PitchTracker:
+    """YIN pitch tracking (the reference's pocketsphinx_pitch, fe/yin.c) for whole batches of int16 streams on the
+    device.  Keywords are the program's options; each stream is tracked by a fresh yin_t, bit for bit."""
+
+    def __init__(self, sample_rate=16000, flen=0.025, fshift=0.01, smooth_window=2, voice_thresh=0.1, search_range=0.2,
+                 device=0):
+        from ._lib import PitchOpts
+        o = PitchOpts()
+        o.sample_rate, o.smooth_window = int(sample_rate), int(smooth_window)
+        o.flen, o.fshift = float(flen), float(fshift)
+        o.voice_thresh, o.search_range = float(voice_thresh), float(search_range)
+        h = C.c_void_p()
+        check(lib().psb_pitch_create(C.byref(o), device, C.byref(h)), "psb_pitch_create")
+        self.h = h
+        L = lib()
+        self.sample_rate, self.smooth_window = int(sample_rate), int(smooth_window)
+        self.frame_size, self.frame_shift, self.ndiff = L.psb_pitch_frame_size(h), L.psb_pitch_frame_shift(h), L.psb_pitch_ndiff(h)
+
+    def n_frames(self, n_samples):
+        return 1 + (n_samples - self.frame_size) // self.frame_shift if n_samples >= self.frame_size else 0
+
+    def track_batch(self, streams):
+        """Per stream, a dict of period, bestdiff (uint16), time, voicing and pitch (float64): one entry per yin_read
+        that succeeds, as pitch_result describes them."""
+        streams = [np.ascontiguousarray(s, np.int16) for s in streams]
+        n = len(streams)
+        samp_off = np.zeros(n + 1, np.int64)
+        samp_off[1:] = np.cumsum([len(s) for s in streams])
+        pcm = np.concatenate(streams) if n else np.zeros(0, np.int16)
+        frames = [self.n_frames(len(s)) for s in streams]
+        cap = max(sum(frames), 1)                                      # at most one read per frame
+        period = np.zeros(cap, np.uint16)
+        bestdiff = np.zeros(cap, np.uint16)
+        out_off = np.zeros(n + 1, np.int32)
+        check(lib().psb_pitch_process_host(self.h, _p(pcm) if pcm.size else None, _p(samp_off), n, _p(out_off),
+                                           _p(period), _p(bestdiff), None), "psb_pitch_process_host")
+        return [pitch_result(period[out_off[i]:out_off[i + 1]].copy(), bestdiff[out_off[i]:out_off[i + 1]].copy(),
+                             pitch_main_reads(frames[i], self.smooth_window), self.frame_shift, self.sample_rate)
+                for i in range(n)]
+
+    def close(self):
+        if self.h:
+            lib().psb_pitch_free(self.h)
+            self.h = None
