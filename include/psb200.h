@@ -848,6 +848,46 @@ int psb_pitch_process_host(psb_pitch_t *h, const int16_t *pcm, const int64_t *sa
 int psb_pitch_process_device(psb_pitch_t *h, const int16_t *d_pcm, const int64_t *samp_off, int32_t n_streams,
                              int32_t *out_off, uint16_t *d_period, uint16_t *d_bestdiff, float *ms);
 
+/* Live pitch tracking: the handle keeps n_slots streams, each one yin_t driven as extract_pitch drives it while its
+ * samples arrive over several calls.  Frame f of a slot is samples f * frame_shift .. f * frame_shift +
+ * frame_size - 1 of everything fed since the slot was made fresh; yin_write then yin_read run on a frame in the call
+ * that completes it, and a final call then runs yin_end and yin_read until it fails.  A slot's reads joined over its
+ * calls are, for any chunking, bit for bit psb_pitch_process_*'s for the whole stream (never-written window slots
+ * and the uint16 frame counter's wrap included).  Whole-stream calls on the same handle never read or change the
+ * slots.
+ * psb_pitch_live_open: creates the slot table, or grows it; every slot starts fresh (yin_init: zeroed window,
+ * wcur 0).
+ * psb_pitch_live_reset: the listed slots start fresh.  The reference's yin_start clears neither the window nor
+ * wcur, and pocketsphinx_pitch never reuses a yin_t, so a slot that has had its final call is refused until it is
+ * reset rather than carried on with a stale window.
+ * psb_pitch_feed_*: fed slot i = slots[i] (host, each slot at most once per call) gets the samples
+ * pcm[samp_off[i] .. samp_off[i + 1] - 1] (host samp_off int64[n + 1], samp_off[0] = 0; zero samples is
+ * allowed).  final (host int8[n], may be NULL): where non-zero, the slot's stream ends after these samples (the
+ * samples after its last frame are dropped).
+ * Outputs:
+ *   out_off int32[n + 1] (host): fed slot i's reads in this call are out_off[i] .. out_off[i + 1] - 1 of period and
+ *     bestdiff (uint16).  Sizing: a slot gets at most its new frames + 2 * smooth_window reads in one call (the drain
+ *     of a final call), and its new frames are at most ceil(samples / frame_shift);
+ *   status[n] (host): the slot's state at the end of the call.
+ * Refused before any launch, and then no slot changes: feeding or resetting before psb_pitch_live_open, a slot
+ * outside 0 .. n_slots - 1, a slot fed twice in one call, feeding a slot that has ended, samp_off[0] != 0 or
+ * decreasing, a slot taken past 2^31 - 1 frames.  _device: pcm, period and bestdiff on the device, *ms (may be
+ * NULL) = device time of the call's kernels. */
+typedef struct psb_pitch_live_status_s {
+    int32_t frames;               /* frames written since the slot was made fresh */
+    int32_t main_reads;           /* reads of the frame loop so far: read k's time is min(k, main_reads) * frame_shift */
+    int32_t reads;                /* all reads so far, the drain after a final call included */
+    int32_t ended;                /* 1 after a final call: refused until reset */
+} psb_pitch_live_status_t;
+int psb_pitch_live_open(psb_pitch_t *h, int32_t n_slots);
+int psb_pitch_live_reset(psb_pitch_t *h, const int32_t *slots, int32_t n);
+int psb_pitch_feed_host(psb_pitch_t *h, const int32_t *slots, int32_t n, const int16_t *pcm, const int64_t *samp_off,
+                        const int8_t *final, int32_t *out_off, uint16_t *period, uint16_t *bestdiff,
+                        psb_pitch_live_status_t *status, float *ms);
+int psb_pitch_feed_device(psb_pitch_t *h, const int32_t *slots, int32_t n, const int16_t *d_pcm, const int64_t *samp_off,
+                          const int8_t *final, int32_t *out_off, uint16_t *d_period, uint16_t *d_bestdiff,
+                          psb_pitch_live_status_t *status, float *ms);
+
 /* number of kernels launched by this library in the calling process so far */
 int64_t psb_kernel_launch_count(void);
 /* bytes of device and pinned host memory this library holds now, over all handles */

@@ -189,6 +189,10 @@ SYMBOLS = [
     ("psb_pitch_ndiff", _I32, [_VP]),
     ("psb_pitch_process_host", C.c_int, [_VP, _VP, _VP, _I32, _VP, _VP, _VP, C.POINTER(C.c_float)]),
     ("psb_pitch_process_device", C.c_int, [_VP, _VP, _VP, _I32, _VP, _VP, _VP, C.POINTER(C.c_float)]),
+    ("psb_pitch_live_open", C.c_int, [_VP, _I32]),
+    ("psb_pitch_live_reset", C.c_int, [_VP, _VP, _I32]),
+    ("psb_pitch_feed_host", C.c_int, [_VP, _VP, _I32, _VP, _VP, _VP, _VP, _VP, _VP, _VP, C.POINTER(C.c_float)]),
+    ("psb_pitch_feed_device", C.c_int, [_VP, _VP, _I32, _VP, _VP, _VP, _VP, _VP, _VP, _VP, C.POINTER(C.c_float)]),
     ("psb_kernel_launch_count", _I64, []),
     ("psb_device_bytes_live", _I64, []),
 ]

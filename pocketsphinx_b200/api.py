@@ -1174,3 +1174,70 @@ class PitchTracker:
         if self.h:
             lib().psb_pitch_free(self.h)
             self.h = None
+
+
+PITCH_LIVE_STATUS = np.dtype([("frames", np.int32), ("main_reads", np.int32), ("reads", np.int32),
+                              ("ended", np.int32)])                               # psb_pitch_live_status_t
+
+
+def pitch_live_result(period, bestdiff, status, frame_shift, sample_rate):
+    """One slot's reads of one live call as pitch_result gives them for the whole stream: the call's reads are the
+    stream's reads status["reads"] - len(period) .. status["reads"] - 1, so their times continue across calls.  Adds
+    the slot's frames, main_reads (so far) and ended."""
+    period = np.asarray(period, np.uint16)
+    reads, main = int(status["reads"]), int(status["main_reads"])
+    res = pitch_result(period, bestdiff, 0, frame_shift, sample_rate)
+    k = np.minimum(np.arange(reads - len(period), reads, dtype=np.int64), main)
+    res["time"] = (k * frame_shift).astype(np.float64) / sample_rate
+    res.update(frames=int(status["frames"]), main_reads=main, ended=bool(status["ended"]))
+    return res
+
+
+class LivePitchTracker(PitchTracker):
+    """YIN pitch tracking for n_slots live streams on the device: feed() hands each listed slot its next samples, in
+    any lengths, and returns the reads those samples complete.  A slot's results joined over its calls are
+    track_batch's for the whole stream, bit for bit, whatever the chunking.  Options as PitchTracker's; track_batch on
+    this handle leaves the slots alone."""
+
+    def __init__(self, n_slots, sample_rate=16000, flen=0.025, fshift=0.01, smooth_window=2, voice_thresh=0.1,
+                 search_range=0.2, device=0):
+        super().__init__(sample_rate, flen, fshift, smooth_window, voice_thresh, search_range, device)
+        try:
+            check(lib().psb_pitch_live_open(self.h, int(n_slots)), "psb_pitch_live_open")
+        except PsbError:
+            self.close()
+            raise
+        self.n_slots = int(n_slots)
+
+    def feed(self, chunks, slots=None, final=None):
+        """chunks: int16 arrays, one per slot in `slots` (default: slots 0 .. len(chunks) - 1).  final: per slot, true
+        to end the stream after these samples (yin_end; the slot is then refused until reset).  Returns one dict per
+        fed slot: period, bestdiff, time, voicing and pitch of this call's reads (as pitch_live_result), frames (fed
+        since the slot was made fresh), main_reads and ended."""
+        chunks = [np.ascontiguousarray(c, np.int16) for c in chunks]
+        n = len(chunks)
+        slots = np.arange(n, dtype=np.int32) if slots is None else np.ascontiguousarray(slots, np.int32)
+        if len(slots) != n:
+            raise ValueError("feed: %d chunks for %d slots" % (n, len(slots)))
+        fin = None if final is None else np.ascontiguousarray([bool(f) for f in final], np.int8)
+        if fin is not None and len(fin) != n:
+            raise ValueError("feed: %d final flags for %d slots" % (len(fin), n))
+        samp_off = np.zeros(n + 1, np.int64)
+        samp_off[1:] = np.cumsum([len(c) for c in chunks])
+        pcm = np.concatenate(chunks) if n else np.zeros(0, np.int16)
+        # new frames + the drain of a final call, per slot
+        cap = int(sum(-(-len(c) // self.frame_shift) + 2 * self.smooth_window for c in chunks))
+        period = np.zeros(max(cap, 1), np.uint16)
+        bestdiff = np.zeros(max(cap, 1), np.uint16)
+        out_off = np.zeros(n + 1, np.int32)
+        status = np.zeros(max(n, 1), PITCH_LIVE_STATUS)
+        check(lib().psb_pitch_feed_host(self.h, _p(slots) if n else None, n, _p(pcm) if pcm.size else None, _p(samp_off),
+                                        _p(fin) if fin is not None else None, _p(out_off), _p(period), _p(bestdiff),
+                                        _p(status), None), "psb_pitch_feed_host")
+        return [pitch_live_result(period[out_off[i]:out_off[i + 1]].copy(), bestdiff[out_off[i]:out_off[i + 1]].copy(),
+                                  status[i], self.frame_shift, self.sample_rate) for i in range(n)]
+
+    def reset(self, slots):
+        """The listed slots start fresh streams (a new yin_init)."""
+        slots = np.ascontiguousarray(slots, np.int32)
+        check(lib().psb_pitch_live_reset(self.h, _p(slots) if len(slots) else None, len(slots)), "psb_pitch_live_reset")

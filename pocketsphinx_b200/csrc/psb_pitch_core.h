@@ -1,7 +1,7 @@
 // psb_pitch_core.h -- the integer arithmetic of the reference's YIN pitch tracker (fe/yin.c) and the
 // read schedule of pocketsphinx_pitch's extract_pitch loop, as __host__ __device__ functions.  psb_pitch.cu's
-// kernels and tests/emul/pitch_emul.cpp (the CPU restatement the tests pin against the compiled reference) are
-// built from this one file.
+// kernels and tests/emul/pitch_emul.cpp / pitch_live_emul.cpp (the CPU restatements the tests pin against the
+// compiled reference) are built from this one file.
 //
 // Restated as gcc -O3 on x86-64 executes the reference (checked against its disassembly):
 //   cmn_diff            yin.c:69-128   the square of a difference wraps in int; it is shifted arithmetically
@@ -15,12 +15,15 @@
 #define PSB_PITCH_CORE_H
 
 #include <limits.h>
+#include <stddef.h>
 #include <stdint.h>
 
 #ifdef __CUDACC__
 #define PSB_PITCH_HD __host__ __device__ __forceinline__
+#define PSB_PITCH_MEMBER __host__ __device__ __forceinline__
 #else
 #define PSB_PITCH_HD static inline
+#define PSB_PITCH_MEMBER inline
 #endif
 
 // how many bits t can be scaled up by in cmn_diff: one below the count of leading zeros of ndiff
@@ -116,6 +119,13 @@ PSB_PITCH_HD int32_t psb_pitch_n_reads(int32_t n_frames, int half)
     return m + ((n_frames - m) % wsize);
 }
 
+// reads of one live call that takes a slot from f0 to f1 frames: the main loop's reads of the new frames, and on a
+// final call the drain after them (at most f1 - f0 + 2 * half)
+PSB_PITCH_HD int32_t psb_pitch_live_reads(int32_t f0, int32_t f1, int half, int final)
+{
+    return (final ? psb_pitch_n_reads(f1, half) : psb_pitch_main_reads(f1, half)) - psb_pitch_main_reads(f0, half);
+}
+
 // the frame slot `slot` holds after F writes (frame f goes to slot f % wsize), -1 when never written
 PSB_PITCH_HD int32_t psb_pitch_slot_frame(int slot, int32_t F, int wsize)
 {
@@ -158,11 +168,27 @@ PSB_PITCH_HD psb_pitch_read_t psb_pitch_read_at(int32_t k, int32_t n_frames, int
     return r;
 }
 
+// A live slot's frames as one call's reads see them: frames f0 and later were written by this call and sit in `call`
+// (frame f at f - f0), earlier ones in the slot's ring of wsize entries (frame f at f % wsize, as diff_window keeps
+// them).  stride: values per frame, 1 for periods and diffs, ndiff for rows.  A read of this call needs no frame
+// before f0 - wsize: its window ends at the frames written when it is made, never fewer than f0.
+struct psb_pitch_live_frames_t {
+    const int32_t *call, *ring;
+    int32_t f0;
+    int wsize, stride;
+    PSB_PITCH_MEMBER const int32_t *at(int32_t f) const
+    {
+        return f >= f0 ? call + (size_t)(f - f0) * stride : ring + (size_t)(f % wsize) * stride;
+    }
+    PSB_PITCH_MEMBER int32_t operator[](int32_t f) const { return *at(f); }
+};
+
 // The decision of one yin_read.  period[f] / pdiff[f] are frame f's period and diff at that period; row(f) is frame
-// f's diff row (ndiff values).  A never-written slot reads period 0, diff 0 and a row of zeros.
-template <class RowOf>
+// f's diff row (ndiff values).  period / pdiff are arrays indexed by frame, or accessors with an operator[] that
+// finds frame f elsewhere (a live slot's ring).  A never-written slot reads period 0, diff 0 and a row of zeros.
+template <class PeriodOf, class DiffOf, class RowOf>
 PSB_PITCH_HD void psb_pitch_decide(const psb_pitch_read_t &r, int half, int ndiff, int32_t threshold, int32_t range,
-                                   const int32_t *period, const int32_t *pdiff, RowOf row, uint16_t *out_period,
+                                   const PeriodOf &period, const DiffOf &pdiff, RowOf row, uint16_t *out_period,
                                    uint16_t *out_bestdiff)
 {
     const int wsize = 2 * half + 1;
